@@ -5,12 +5,12 @@
   python bench.py --impl reference --gpus N ...          the reference's own CPU implementation on this box's host cores
 
 Workload at N=1 = BASELINE.json configs[1]: brute-force KNN, 10M x 768 fp32, inner product, k=10, batch of 1024 queries on one
-B200.  A "step" is one batch of 1024 queries against the resident index.  For N>1 the namespace is sharded by row range, 10M rows
+H100 (80 GB: the fp32 rows and their bf16 shadow take 46 GB).  A "step" is one batch of 1024 queries against the resident index.  For N>1 the namespace is sharded by row range, 10M rows
 per GPU (weak scaling, configs[4] at N=8); every rank scans its shard for all 1024 queries and ONE C-ABI call per rank
 (rxgpu_sharded_search_knn: scan, ncclAllGather, device merge) yields the global top-k; `value` counts the (query x 10M-row-shard)
 scans all ranks complete per second.
 Synthetic data: rows and queries from the counter-based generator in reindexer_b200/csrc/common.cuh (sigma 0.25, like the
-reference's own test generator), produced directly in HBM.  Inputs are far larger than L2 (30.7 GB vs 126 MB), so no flush.
+reference's own test generator), produced directly in HBM.  Inputs are far larger than L2 (30.7 GB vs 50 MB), so no flush.
 
 At N=1 the line also carries `sub`: driver-visible records of the other BASELINE configs -- Q=1 / Q=4 latency on the same 10M x 768
 index (the >= 70 % HBM-roofline headline), config 0 (100k x 128, L2-resident), config 3 (ft_fast BM25, 50M docs) and config 2 (HNSW,
@@ -57,7 +57,7 @@ def hbm_peak():
     p = load_peaks()
     if p.get("hbm_gbs"):
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def host_threads():
@@ -111,7 +111,7 @@ def host_mem_available_gb():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     def __init__(self, gpu_index):
         self.gpu = gpu_index
@@ -161,7 +161,7 @@ class ClockSampler:
             for name, val in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[5:9]):
                 if val.lower().startswith("active"):
                     reasons.add(name)
-            try:  # board power next to its enforced limit: the filter kernel runs AT the limit (DESIGN 9), which is what bounds it
+            try:  # board power next to its enforced limit: a number measured on a power-limited card is only valid beside it
                 watts.append(float(f[3]))
                 limit = float(f[9]) if len(f) > 9 else limit
             except ValueError:
@@ -279,12 +279,15 @@ def run_reference(args):
 
 
 # ----------------------------------------------------------------------------------------------------------------- GPU arm
-def roofline_record(stats_sum, ms_total, rows, tc_used, qt, nlaunch_timed, scan_ms, alg_bytes, passes):
+def roofline_record(stats_sum, ms_total, rows, tc_used, queries_timed, nlaunch_timed, scan_ms, alg_bytes, passes):
     peak, peak_src = hbm_peak()
     peaks_all = load_peaks()
+    # a filter launch serves one cluster of query blocks, and the last cluster of a batch may be padded: price every launch at the
+    # queries it actually served (the timed queries over the timed launches), not at the largest cluster's tile
+    qpl = queries_timed / max(nlaunch_timed, 1)
     if tc_used:  # dominant kernel = the tensor-core filter: bf16 shadow rows + row norms + the resident query block, per launch
-        per_launch_bytes = rows * DIM * 2 + rows * 8 + qt * DIM * 2
-        kernel = {5: "knn_tc_filter_p"}.get(stats_sum.get("tc_kernel"), "knn_tc_filter_q")
+        per_launch_bytes = rows * DIM * 2 + rows * 8 + qpl * DIM * 2
+        kernel = "knn_tc_filter"
     else:
         per_launch_bytes = alg_bytes / max(passes, 1)
         kernel = "knn_scan_warp"
@@ -296,14 +299,12 @@ def roofline_record(stats_sum, ms_total, rows, tc_used, qt, nlaunch_timed, scan_
     tensor_burst, tensor_sust = peaks_all.get("bf16_tflops"), peaks_all.get("bf16_tflops_sustained")
     tensor_src = "measured (MEASURED_PEAKS.json bf16_tflops, burst: the timed region is < 1 s)"
     if not tensor_burst:
-        tensor_burst, tensor_sust, tensor_src = 1590.0, 1590.0, "fallback (B200_PROFILING.md 1.59 PFLOP/s)"
-    flops_per_launch = 2.0 * rows * DIM * qt if tc_used else 0.0
+        tensor_burst, tensor_sust, tensor_src = 989.0, 989.0, "fallback (H100 SXM data sheet, dense BF16 989 TFLOP/s at 700 W)"
+    flops_per_launch = 2.0 * rows * DIM * qpl if tc_used else 0.0
     tensor_tflops = flops_per_launch / (avg_launch_ms * 1e-3) / 1e12 if tc_used and avg_launch_ms > 0 else None
     t_hbm = per_launch_bytes / (peak * 1e9)
     t_tensor = flops_per_launch / (tensor_burst * 1e12) if tc_used else 0.0
     common = {
-        # dram__bytes_read.sum + dram__bytes_write.sum per launch from the ncu --set full captures under profiles/, full-size workload only
-        "traffic": (None if rows != ROWS_FULL else 15.4224e9 if tc_used else 30.7201e9),
         "kernel": kernel, "bytes_per_launch": per_launch_bytes, "flops_per_launch": flops_per_launch, "avg_launch_ms": avg_launch_ms,
         "launches_timed": nlaunch_timed, "kernel_share_of_step": scan_ms / ms_total if ms_total else None,
         "hbm": {"achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src},
@@ -348,8 +349,7 @@ def sub_small_batches(idx, rx, hq, cpu, threads):
                        "ms_per_call": wall * 1e3},
                "roofline": {"bound": "hbm", "kernel": "knn_scan_warp", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
                             "peak_source": peak_src + " -- a copy (read + write) figure; a read-only stream can exceed it",
-                            "bytes_per_launch": per_launch, "avg_launch_ms": ms / max(nl, 1), "launches_timed": nl,
-                            "traffic": 30.7201e9 if rows == ROWS_FULL else None}}
+                            "bytes_per_launch": per_launch, "avg_launch_ms": ms / max(nl, 1), "launches_timed": nl}}
         if cpu is not None:
             dt, _, _ = cpu.round(hq[:1] if cpu.kind == "reference" else hq[:1])  # ONE query on ONE thread: the reference's latency
             if cpu.kind == "reference":
@@ -394,7 +394,7 @@ def sub_config0(rx):
            "roofline": {"bound": "latency (51 MB set is L2-resident; launch + copies dominate)", "kernel": "knn_scan_warp",
                         "achieved": bytes_q / (ms / max(nl, 1) * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                         "frac": bytes_q / (ms / max(nl, 1) * 1e-3) / 1e9 / peak, "peak_source": peak_src + " (HBM figure; the data comes from L2)",
-                        "avg_launch_ms": ms / max(nl, 1), "bytes_per_launch": bytes_q, "traffic": None}}
+                        "avg_launch_ms": ms / max(nl, 1), "bytes_per_launch": bytes_q}}
     kind = "reference" if O.ref_knn_available() else "port"
     vecs = O.synth_matrix(0x5EED0000, n, dim)
     cpu = (O.RefBF if kind == "reference" else O.PortBF)(O.L2, dim, n)
@@ -413,6 +413,22 @@ def sub_config0(rx):
     rec["parity"] = f"{same}/8 queries: labels identical to the CPU reference"
     gpu.close()
     return rec
+
+
+def dump_outputs(out_dir, dist, labels, counts, rows=None):
+    """What the timed call returned in its last step, as float32 / float64 .npy files (well under 1 MB at 1024 queries): distances,
+    the 64-bit labels split into exact 32-bit halves, result counts and, on one GPU, the internal row indices."""
+    def arr(x):
+        return x.detach().cpu().numpy() if hasattr(x, "detach") else np.asarray(x)
+
+    os.makedirs(out_dir, exist_ok=True)
+    lab = arr(labels).astype(np.int64).view(np.uint64)
+    out = {"distances": arr(dist).astype(np.float32), "labels_hi": (lab >> np.uint64(32)).astype(np.float64),
+           "labels_lo": (lab & np.uint64(0xFFFFFFFF)).astype(np.float64), "counts": arr(counts).astype(np.float64)}
+    if rows is not None:
+        out["row_indices"] = arr(rows).astype(np.float64)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def run_ours(args):
@@ -511,8 +527,9 @@ def run_ours(args):
     main_stats = {}
     ev0.record(stream)
     t_wall0 = time.perf_counter()
+    last = None
     for _ in range(args.steps):
-        step_resident()
+        last = step_resident()
         st = rx.last_search_stats()
         launches += st["launches"]
         passes += st["passes"]
@@ -525,6 +542,8 @@ def run_ours(args):
     ev1.record(stream)
     barrier()
     wall_ms = (time.perf_counter() - t_wall0) * 1e3
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *(last if sharded is not None else (od, ol, oc, oi)))
     clocks = sampler.stop(t_begin, time.perf_counter())
     # sharded steps run on the library's stream inside one blocking C call each: the events on torch's stream bracket them through the
     # host-side ordering, so take the larger of the event time and the host clock around the same region
@@ -570,11 +589,9 @@ def run_ours(args):
         ms_per_step = ms_total / args.steps
         value = world * NQ / (ms_per_step / 1000.0)
         e2e_value = world * NQ / (e2e_s / args.steps)
-        roofline = roofline_record(main_stats, ms_total, rows, tc_used, qt, scan_launches, scan_ms, alg_bytes, passes)
-        kernel_name = {5: "knn_tc_filter_p (tcgen05 cta_group::2 bf16 filter: CTA pairs, queries in TMEM, half a row tile per SM, certified bound) + knn_rerank (exact fp32)",
-                       2: "knn_tc_filter_q (tcgen05 bf16 filter, queries in TMEM, certified bound) + knn_rerank (exact fp32)",
-                       1: "knn_tc_filter (tcgen05 bf16 filter, queries in shared memory) + knn_rerank (exact fp32)"}.get(
-            main_stats.get("tc_kernel") if tc_used else 0, "knn_scan_warp (fp32 FMA, fused top-k)")
+        roofline = roofline_record(main_stats, ms_total, rows, tc_used, NQ * args.steps, scan_launches, scan_ms, alg_bytes, passes)
+        kernel_name = ("knn_tc_filter (wgmma bf16 filter, queries in shared memory, row tiles multicast in a cluster, certified bound) + "
+                       "knn_rerank (exact fp32)") if tc_used else "knn_scan_warp (fp32 FMA, fused top-k)"
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
@@ -582,9 +599,6 @@ def run_ours(args):
             "config": workload_config(world, rows),
             "details": {"query_tile": qt, "kernel": kernel_name, "tc_candidates_per_step": main_stats["tc_candidates"],
                         "tc_fallbacks": main_stats["tc_fallbacks"], "tc_cluster": main_stats["tc_cluster"],
-                        "tail_grid": "clusters of 4 fit 33 times (132 of 148 SMs); 2-CTA clusters of the same kernel scan the last ~10 % of the "
-                                     "row tiles on the other 16 SMs beside every main launch (second stream); roofline.avg_launch_ms is the main "
-                                     "launch, whose window covers all rows for its 512 queries",
                         "l2_policy": "inputs (30.7 GB/GPU) larger than L2, no flush",
                         "global_queries_per_s": NQ / (ms_per_step / 1000.0), "index_fill_s": round(fill_s, 2),
                         "value_definition": "(query x 10M-row shard) scans per second over all ranks",
@@ -662,11 +676,15 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--rows", type=int, default=0, help="rows per GPU (default 10M = BASELINE config)")
     ap.add_argument("--query-tile", type=int, default=0)
-    ap.add_argument("--tc", type=int, default=0, help="tensor-core filter: 0 auto, 1 on, 2 off (exact fp32 scan only), 3..6, 9, 14..16 kernel variants")
+    ap.add_argument("--tc", type=int, default=0, help="tensor-core filter: 0 auto, 1 on, 2 off (exact fp32 scan only), 3 single CTAs (the default shape), 4 clusters of up to two")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-sub", action="store_true", help="skip the sub-records of the other BASELINE configs")
     ap.add_argument("--quick-sub", action="store_true", help="small sub-record sizes (smoke)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path returned in its last step as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,4 +1,4 @@
-/* rxgpu.h -- C ABI of librxgpu.so: the B200 (sm_100a) replacement for Reindexer's float_vector KNN hot path.
+/* rxgpu.h -- C ABI of librxgpu.so: the H100 (sm_90a) replacement for Reindexer's float_vector KNN hot path.
  *
  * This is the drop-in boundary (SURVEY.md §8b).  Every entry point names the reference interface it replaces
  * (paths relative to /root/reference/cpp_src).  Plain C: opaque handles, pointers and sizes only, no exceptions,
@@ -473,17 +473,12 @@ typedef struct {
 	uint32_t tc_fallbacks;      /* queries whose candidate list overflowed and were answered by the exact scan */
 	uint64_t tc_candidates;     /* rows re-ranked exactly */
 	uint32_t tc_cluster;        /* CTAs per cluster in the filter kernel (row tiles are TMA-multicast inside a cluster) */
-	uint32_t tc_kernel;         /* 1 = knn_tc_filter (queries in shared memory), 2 = knn_tc_filter_q (queries in TMEM), 5 = knn_tc_filter_p
-								 * (CTA pairs multiply as one: tcgen05 cta_group::2, UMMA M = 256, N = 128) */
+	uint32_t tc_kernel;         /* 1 = knn_tc_filter (wgmma, queries in shared memory) */
 } rxgpu_search_stats;
 void rxgpu_last_search_stats(rxgpu_search_stats* out);
 /* large query batches: bf16 tensor-core filter + exact fp32 re-rank (results identical to the exact scan).
  * mode 0 = automatic (batches >= 64 queries on >= 100k rows, k <= 127), 1 = whenever possible, 2 = never;
- * the other values force kernel variants for tests/benchmarks (all give the same bits): 3 / 4 = first-generation kernel (queries in
- * shared memory) with 1 CTA / a CTA pair per row tile; 5 / 6 / 9 = knn_tc_filter_q (query block in TMEM, accumulators of 64 rows;
- * the default) with single CTAs / clusters of up to 4 / up to 8; 14 / 15 / 16 = knn_tc_filter_p (CTA pairs multiply as one,
- * cta_group::2, every SM stages half a 128-row tile) with clusters of up to 4 / 2 / 8 CTAs; 17 = the default kernel without its tail grid
- * (2-CTA clusters that scan the last row tiles on the SMs a cluster-of-4 grid cannot use).  DESIGN.md section 9 has the measurements. */
+ * 3 / 4 = as 1 with single CTAs (the default) / clusters of up to two CTAs sharing every row tile; all give the same bits. */
 int rxgpu_set_tensor_core_filter(rxgpu_index*, int mode);
 /* process-wide switch: bracket every scan-kernel launch with CUDA events (used by bench.py for the roofline figure) */
 int rxgpu_set_profile(int on);

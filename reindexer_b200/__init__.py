@@ -1,4 +1,4 @@
-"""reindexer_b200 -- B200-native (sm_100a) replacement for Reindexer's float_vector KNN / ft_fast BM25 hot path.
+"""reindexer_b200 -- H100-native (sm_90a) replacement for Reindexer's float_vector KNN / ft_fast BM25 hot path.
 
 The product is the C-ABI library ``librxgpu.so`` (include/rxgpu.h) and the C++ adapter under ``host/``; this package is
 the thin Python driver used by tests, the benchmark and the multi-GPU (one process per GPU, torch.distributed) plumbing.

@@ -1316,7 +1316,7 @@ thread_local rxgpu_ft_stats g_ft_stats{};
 
 struct rxgpu_ft_index {
 	int device = 0;
-	int sm_count = 148;
+	int sm_count = 132;
 	uint32_t total_docs = 0, nfields = 0;
 	DevBuf<uint32_t> words;
 	DevBuf<float> avg;

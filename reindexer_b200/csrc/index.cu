@@ -1,4 +1,4 @@
-// librxgpu: C ABI (include/rxgpu.h) over the sm_100a brute-force float_vector kernels.
+// librxgpu: C ABI (include/rxgpu.h) over the sm_90a brute-force float_vector kernels.
 // Host logic mirrors hnswlib::BruteforceSearch (cpp_src/core/index/float_vector/hnswlib/bruteforce.{h,cc}) and the
 // search/select wrappers of HnswIndexBase<Map> (cpp_src/core/index/float_vector/hnsw_index.cc:160-288).
 // There is no CPU fallback anywhere in this file: without a usable CUDA device every compute entry point fails.
@@ -21,8 +21,6 @@
 #include "../host/knn_select.h"
 #include "knn_scan.cuh"
 #include "knn_tc.cuh"
-#include "knn_tc_q.cuh"
-#include "knn_tc_p.cuh"
 
 using namespace rxgpu;
 
@@ -237,11 +235,21 @@ int makeBf16Map(CUtensorMap* m, void* base, uint64_t cols, uint64_t rows, uint64
 	return 0;
 }
 
-constexpr size_t kTcSmemLimit = 227 * 1024;
+constexpr size_t kTcSmemLimit = 227 * 1024;  // the per-block opt-in maximum of sm_90
 constexpr uint32_t kTcCandCap = 4096;
 
+// knn_tc_filter<query block, cluster size>: one instantiation per wgmma N and per cluster shape
+using TcKernel = void (*)(const CUtensorMap, const TcArgs);
+TcKernel tcKernel(uint32_t nqb, uint32_t cluster) {
+	static const TcKernel table[4][2] = {{knn_tc_filter<32, 1>, knn_tc_filter<32, 2>},
+										 {knn_tc_filter<64, 1>, knn_tc_filter<64, 2>},
+										 {knn_tc_filter<96, 1>, knn_tc_filter<96, 2>},
+										 {knn_tc_filter<128, 1>, knn_tc_filter<128, 2>}};
+	return table[nqb / 32 - 1][cluster == 2 ? 1 : 0];
+}
+
 uint32_t tcQueryBlock(uint32_t nq, uint32_t kchunks) {
-	uint32_t nqb = std::min<uint32_t>(256, (nq + 31u) & ~31u);
+	uint32_t nqb = std::min<uint32_t>(kTcMaxNq, (nq + 31u) & ~31u);
 	while (nqb >= 32 && tc_smem_bytes(nqb, kchunks) > kTcSmemLimit) {
 		nqb -= 32;
 	}
@@ -325,7 +333,10 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	const uint32_t pitchBf = ix->pitch_bf, kchunks = pitchBf / kTcChunkK;
 	const uint32_t nqb = tcQueryBlock(nq, kchunks);
 	const uint32_t nblocks = (nq + nqb - 1) / nqb;
-	const uint32_t nqPad = std::max<uint32_t>(nblocks * nqb, (nq + 511u) / 512u * 512u);  // both kernel generations index it
+	// single CTAs by default: measured on an H100 at config 1, 10.5 k queries/s against 8.1 k with clusters of two and 4.4 k with clusters
+	// of four -- a multicast stage waits for the slowest consumer of the cluster, which costs more than the shared L2 reads save
+	const uint32_t clusterMax = ix->tc_cluster_max ? ix->tc_cluster_max : 1u;
+	const uint32_t nqPad = nblocks * nqb;
 	RX_CUDA(ws.d_qbf.ensure(size_t(nqPad) * pitchBf));
 	RX_CUDA(ws.d_qnorm.ensure(nqPad));
 	RX_CUDA(ws.d_tau.ensure(nqPad));
@@ -345,221 +356,42 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	RX_CUDA(cudaGetLastError());
 	g_stats.launches += 2;
 	const uint32_t ntiles = uint32_t((ix->size + kTcTileRows - 1) / kTcTileRows);
-	bool launched = false;
-	if ((ix->tc_variant == 0 || ix->tc_variant == 14) && kchunks <= kTqMaxKchunks) {
-		// query block in tensor memory, deep TMA ring, row tiles multicast inside a cluster.  tc_variant 0: knn_tc_filter_q (every CTA
-		// multiplies on its own, two accumulators of 64 rows; default); 14: knn_tc_filter_p (CTA pairs multiply as one, cta_group::2, every
-		// SM stages half a 128-row tile, one accumulator).  Both run at the board's power limit and land on the same time (DESIGN 9).
-		using TqKernel = void (*)(TqArgs);
-		const bool pairs = ix->tc_variant == 14;
-		const TqKernel kernels[4] = {pairs ? knn_tc_filter_p<2> : knn_tc_filter_q<1>, pairs ? knn_tc_filter_p<2> : knn_tc_filter_q<2>,
-									 pairs ? knn_tc_filter_p<4> : knn_tc_filter_q<4>, pairs ? knn_tc_filter_p<8> : knn_tc_filter_q<8>};
-		auto kernelOf = [&](int c) { return kernels[c == 8 ? 3 : (c == 4 ? 2 : (c == 2 ? 1 : 0))]; };
-		const uint32_t tileRows = pairs ? kTpTileRows : kTqTileRows;
-		const unsigned threads = pairs ? kTpThreads : kTqThreads;
-		auto smemOf = [&](uint32_t st) { return pairs ? tp_smem_bytes(st) : tq_smem_bytes(st); };
-		const uint32_t qblocks = (nq + kTqQueries - 1) / kTqQueries;
-		uint32_t stages = 2;
-		while (smemOf(stages + 1) <= kTcSmemLimit && stages < 64) {
-			++stages;
-		}
-		const size_t smem = smemOf(stages);
-		for (const TqKernel kfn : kernels) {
-			RX_CUDA(raiseSmemCeilingOnce(kfn, ix->device, int(kTcSmemLimit)));
-		}
-		// a cluster of C CTAs reads every row tile from HBM once for C x 128 queries (TMA multicast)
-		const uint32_t clusterMax = ix->tc_cluster_max ? ix->tc_cluster_max : 4u;  // mode 9: up to 8 (one launch serves 1024 queries)
-		int cluster = qblocks >= 5 ? 8 : (qblocks >= 3 ? 4 : (qblocks == 2 ? 2 : 1));
-		cluster = std::min<int>(cluster, int(clusterMax));
-		if (pairs) {
-			cluster = std::max(cluster, 2);  // whole CTA pairs (a second CTA without queries multiplies zeros)
-		}
-		const uint32_t qtiles = uint32_t((ix->size + tileRows - 1) / tileRows);
-		unsigned grid = 0;
-		int residentClusters = 0;
-		for (;;) {  // how many clusters of this size can be resident at once (GPC boundaries strand SMs for size 4)
-			cudaLaunchConfig_t cfg{};
-			cfg.gridDim = dim3(unsigned(ix->sm_count) / cluster * cluster);
-			cfg.blockDim = dim3(threads);
-			cfg.dynamicSmemBytes = smem;
-			cudaLaunchAttribute attr[1];
-			attr[0].id = cudaLaunchAttributeClusterDimension;
-			attr[0].val.clusterDim.x = unsigned(cluster);
-			attr[0].val.clusterDim.y = 1;
-			attr[0].val.clusterDim.z = 1;
-			cfg.attrs = attr;
-			cfg.numAttrs = 1;
-			int maxClusters = 0;
-			const cudaError_t e = cudaOccupancyMaxActiveClusters(&maxClusters, kernelOf(cluster), &cfg);
-			if (e == cudaSuccess && maxClusters > 0) {
-				grid = unsigned(std::min<uint64_t>(uint64_t(maxClusters), std::max<uint32_t>(qtiles, 1))) * cluster;
-				residentClusters = maxClusters;
-				break;
-			}
-			cudaGetLastError();
-			if (cluster == (pairs ? 2 : 1)) {
-				return fail(RXGPU_ERR_SYSTEM, "rxgpu: tensor-core filter kernel cannot be made resident");
-			}
-			cluster /= 2;
-		}
-		// Tail grid: clusters of 4 fit 33 times on a B200 (132 of 148 SMs, GPC boundaries).  The kernel is power-bound (DESIGN 9), so more
-		// units at a lower clock is the lever left: 2-CTA clusters of the same kernel take the stranded SMs and scan the last
-		// Ct / (2 Cm + Ct) of the row tiles -- twice per main launch, once for each half of its 4 query blocks -- on a second stream.
-		// Candidate lists, thresholds and bound lists are per query and global, so both grids feed the same re-rank.
-		uint32_t tailClusters = 0, tilesMain = qtiles;
-		if (ix->tc_tail && cluster == 4 && int(grid) == residentClusters * cluster && qtiles >= 256) {
-			const uint32_t spare = uint32_t(ix->sm_count) - grid;
-			tailClusters = spare / 2;
-			if (tailClusters) {
-				const uint32_t cm = grid / cluster;
-				// the tail's share by SM count would be Ct / (2 Cm + Ct) = 10.8 %; measured best at 10 % (80 / 100 / 120 / 140 permille:
-			// 71.4 / 72.5 / 70.8 / 68.1 k queries/s on one box): a 2-CTA cluster reads its rows from HBM once per 256 queries, not 512
-			uint32_t tilesTail = uint32_t(uint64_t(qtiles) * tailClusters * 15 / ((2ull * cm + tailClusters) * 16));
-			static const char* tp = std::getenv("RXGPU_TC_TAIL_PERMILLE");  // tuning aid: the tail's share of the row tiles
-			if (tp) {
-				tilesTail = uint32_t(uint64_t(qtiles) * uint32_t(std::atoi(tp)) / 1000);
-			}
-				tilesMain = qtiles - tilesTail;
-				if (!ws.tail_stream) {
-					RX_CUDA(cudaStreamCreateWithFlags(&ws.tail_stream, cudaStreamNonBlocking));
-					RX_CUDA(cudaEventCreateWithFlags(&ws.tail_fork, cudaEventDisableTiming));
-					RX_CUDA(cudaEventCreateWithFlags(&ws.tail_join, cudaEventDisableTiming));
-				}
-				RX_CUDA(cudaEventRecord(ws.tail_fork, st));
-				RX_CUDA(cudaStreamWaitEvent(ws.tail_stream, ws.tail_fork, 0));
-			}
-		}
-		const uint32_t rowsMain = uint32_t(std::min<uint64_t>(ix->size, uint64_t(tilesMain) * tileRows));
-		for (uint32_t b = 0; b < qblocks; b += cluster) {
-			TqArgs a{};
-			a.shadow = static_cast<const unsigned char*>(ix->d_shadow);
-			a.vnorm = ix->d_vnorm;
-			a.vw = ix->d_vw;
-			a.vinv = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
-			a.qnorm = ws.d_qnorm.p;
-			a.qbf = ws.d_qbf.p;
-			a.tau = ws.d_tau.p;
-			a.ub_list = ws.d_ub_list.p;
-			a.ub_lock = ws.d_ub_lock.p;
-			a.cand_rows = ws.d_cand_rows.p;
-			a.cand_count = ws.d_cand_count.p;
-			a.cand_cap = kTcCandCap;
-			a.init_rows = uint32_t(std::min<uint64_t>(ix->size, kTcInitRows));
-			a.n = rowsMain;
-			a.kchunks = kchunks;
-			a.pitch_bf = pitchBf;
-			a.nq_total = nq;
-			a.q0 = b * kTqQueries;
-			a.k1 = k1;
-			a.stages = stages;
-			a.metric = ix->metric;
-			{
-				static const char* pf = std::getenv("RXGPU_TC_PREFETCH");  // tuning aid: L2 prefetch distance in tiles
-				a.prefetch = pf ? uint32_t(std::atoi(pf)) : 0u;
-				static const char* si = std::getenv("RXGPU_TC_SINGLE_ISSUER");  // tuning aid for knn_tc_filter_q
-				a.single_issuer = si ? uint32_t(std::atoi(si)) : 0u;  // measured: no effect (the ring is not what limits the kernel), off by default
-			}
-			static DevBuf<unsigned long long> traceBuf;  // profiling aid: RXGPU_TC_TRACE=<file> dumps per-tile timestamps of CTA 0
-			const char* tracePath = std::getenv("RXGPU_TC_TRACE");
-			if (tracePath && b == 0) {
-				RX_CUDA(traceBuf.ensure(256 * 16));
-				RX_CUDA(cudaMemsetAsync(traceBuf.p, 0, 256 * 16 * 8, st));
-				a.trace = traceBuf.p;
-				const char* first = std::getenv("RXGPU_TC_TRACE_FIRST");
-				a.trace_first = first ? uint32_t(std::atoi(first)) : 0u;
-			}
-			cudaEvent_t e0 = nullptr, e1 = nullptr;
-			if (g_profile.load(std::memory_order_relaxed)) {
-				RX_CUDA(cudaEventCreate(&e0));
-				RX_CUDA(cudaEventCreate(&e1));
-				RX_CUDA(cudaEventRecord(e0, st));
-			}
-			cudaLaunchConfig_t cfg{};
-			cfg.gridDim = dim3(grid);
-			cfg.blockDim = dim3(threads);
-			cfg.dynamicSmemBytes = smem;
-			cfg.stream = st;
-			cudaLaunchAttribute attr[1];
-			attr[0].id = cudaLaunchAttributeClusterDimension;
-			attr[0].val.clusterDim.x = unsigned(cluster);
-			attr[0].val.clusterDim.y = 1;
-			attr[0].val.clusterDim.z = 1;
-			cfg.attrs = attr;
-			cfg.numAttrs = 1;
-			RX_CUDA(cudaLaunchKernelEx(&cfg, kernelOf(cluster), a));
-			RX_CUDA(cudaGetLastError());
-			if (e0) {
-				RX_CUDA(cudaEventRecord(e1, st));
-				g_prof_events.emplace_back(e0, e1);
-			}
-			g_stats.launches += 1;
-			g_stats.passes += 1;
-			for (uint32_t pb = b; tailClusters && pb < std::min<uint32_t>(b + uint32_t(cluster), qblocks); pb += 2) {
-				TqArgs t = a;
-				t.trace = nullptr;
-				t.row_base = rowsMain;
-				t.shadow = a.shadow + size_t(rowsMain) * pitchBf * 2;
-				t.vw = a.vw + rowsMain;
-				t.n = uint32_t(ix->size) - rowsMain;
-				t.q0 = pb * kTqQueries;
-				cudaLaunchConfig_t tcfg{};
-				tcfg.gridDim = dim3(tailClusters * 2);
-				tcfg.blockDim = dim3(threads);
-				tcfg.dynamicSmemBytes = smem;
-				tcfg.stream = ws.tail_stream;
-				cudaLaunchAttribute tattr[1];
-				tattr[0].id = cudaLaunchAttributeClusterDimension;
-				tattr[0].val.clusterDim.x = 2;
-				tattr[0].val.clusterDim.y = 1;
-				tattr[0].val.clusterDim.z = 1;
-				tcfg.attrs = tattr;
-				tcfg.numAttrs = 1;
-				RX_CUDA(cudaLaunchKernelEx(&tcfg, kernelOf(2), t));
-				RX_CUDA(cudaGetLastError());
-				g_stats.launches += 1;
-			}
-			if (a.trace) {
-				std::vector<unsigned long long> h(256 * 16);
-				RX_CUDA(cudaStreamSynchronize(st));
-				RX_CUDA(cudaMemcpy(h.data(), a.trace, h.size() * 8, cudaMemcpyDeviceToHost));
-				if (FILE* f = std::fopen(std::getenv("RXGPU_TC_TRACE"), "w")) {
-					for (int i = 0; i < 256; ++i) {
-						for (int j = 0; j < 16; ++j) {
-							std::fprintf(f, "%llu%c", h[i * 16 + j], j == 15 ? '\n' : ' ');
-						}
-					}
-					std::fclose(f);
-				}
-			}
-		}
-		if (tailClusters) {
-			RX_CUDA(cudaEventRecord(ws.tail_join, ws.tail_stream));
-			RX_CUDA(cudaStreamWaitEvent(st, ws.tail_join, 0));
-		}
-		g_stats.tc_cluster = uint32_t(cluster);
-		g_stats.tc_kernel = pairs ? 5 : 2;
-		g_stats.query_tile = uint32_t(kTqQueries * cluster);
-		g_stats.algorithmic_bytes += uint64_t((qblocks + cluster - 1) / cluster) * (uint64_t(ix->size) * pitchBf * 2 + uint64_t(ix->size) * 4) +
-									 uint64_t(nq) * pitchBf * 2;
-		launched = true;
-	}
-	if (!launched) {
-	// Two CTAs per cluster share every row tile (TMA multicast) and own different query blocks: one pass serves 2*nqb queries.
-	const int cluster = (ix->tc_variant == 3 || nblocks < 2 || ix->sm_count < 2 || ntiles < 2) ? 1 : 2;
 	CUtensorMap mapQ;
 	if (int rc = makeBf16Map(&mapQ, ws.d_qbf.p, pitchBf, nqPad, uint64_t(pitchBf) * 2, nqb)) {
 		return rc;
 	}
 	const size_t smem = tc_smem_bytes(nqb, kchunks);
-	RX_CUDA(raiseSmemCeilingOnce(knn_tc_filter<1>, ix->device, int(kTcSmemLimit)));
-	RX_CUDA(raiseSmemCeilingOnce(knn_tc_filter<2>, ix->device, int(kTcSmemLimit)));
-	unsigned grid = std::min<unsigned>(unsigned(ix->sm_count), ntiles * cluster);
-	grid -= grid % cluster;
-	for (uint32_t b = 0; b < nblocks; b += cluster) {
+	// A cluster of C CTAs owns C consecutive query blocks and reads every row tile from HBM once for all of them (TMA multicast); a
+	// leftover single block runs alone.
+	uint32_t clusterUsed = 1;
+	for (uint32_t b = 0; b < nblocks;) {
+		uint32_t cluster = 1;
+		while (cluster < std::min(clusterMax, nblocks - b) && ntiles >= 2) {
+			cluster *= 2;
+		}
+		const TcKernel kfn = tcKernel(nqb, cluster);
+		RX_CUDA(raiseSmemCeilingOnce(kfn, ix->device, int(kTcSmemLimit)));
+		cudaLaunchConfig_t cfg{};
+		cfg.gridDim = dim3(unsigned(ix->sm_count) / cluster * cluster);
+		cfg.blockDim = dim3(kTcThreads);
+		cfg.dynamicSmemBytes = smem;
+		cfg.stream = st;
+		cudaLaunchAttribute attr[1];
+		attr[0].id = cudaLaunchAttributeClusterDimension;
+		attr[0].val.clusterDim.x = cluster;
+		attr[0].val.clusterDim.y = 1;
+		attr[0].val.clusterDim.z = 1;
+		cfg.attrs = attr;
+		cfg.numAttrs = 1;
+		int resident = 0;  // GPC boundaries can strand SMs for clusters: ask how many fit at once
+		RX_CUDA(cudaOccupancyMaxActiveClusters(&resident, kfn, &cfg));
+		if (resident < 1) {
+			return fail(RXGPU_ERR_SYSTEM, "rxgpu: tensor-core filter kernel cannot be made resident");
+		}
+		cfg.gridDim = dim3(unsigned(std::min<uint64_t>(uint64_t(resident), ntiles)) * cluster);
 		TcArgs a{};
 		a.shadow = static_cast<const unsigned char*>(ix->d_shadow);
-		a.vnorm = ix->d_vnorm;
-		a.vinv = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
+		a.vw = ix->d_vw;
 		a.qnorm = ws.d_qnorm.p;
 		a.tau = ws.d_tau.p;
 		a.ub_list = ws.d_ub_list.p;
@@ -570,7 +402,6 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 		a.cand_cap = kTcCandCap;
 		a.n = uint32_t(ix->size);
 		a.kchunks = kchunks;
-		a.nq_block = nqb;
 		a.q0 = b * nqb;
 		a.nq_total = nq;
 		a.k1 = k1;
@@ -581,23 +412,7 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 			RX_CUDA(cudaEventCreate(&e1));
 			RX_CUDA(cudaEventRecord(e0, st));
 		}
-		if (cluster == 2) {
-			cudaLaunchConfig_t cfg{};
-			cfg.gridDim = dim3(grid);
-			cfg.blockDim = dim3(kTcThreads);
-			cfg.dynamicSmemBytes = smem;
-			cfg.stream = st;
-			cudaLaunchAttribute attr[1];
-			attr[0].id = cudaLaunchAttributeClusterDimension;
-			attr[0].val.clusterDim.x = 2;
-			attr[0].val.clusterDim.y = 1;
-			attr[0].val.clusterDim.z = 1;
-			cfg.attrs = attr;
-			cfg.numAttrs = 1;
-			RX_CUDA(cudaLaunchKernelEx(&cfg, knn_tc_filter<2>, mapQ, a));
-		} else {
-			knn_tc_filter<1><<<grid, kTcThreads, smem, st>>>(mapQ, a);
-		}
+		RX_CUDA(cudaLaunchKernelEx(&cfg, kfn, mapQ, a));
 		RX_CUDA(cudaGetLastError());
 		if (e0) {
 			RX_CUDA(cudaEventRecord(e1, st));
@@ -605,13 +420,14 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 		}
 		g_stats.launches += 1;
 		g_stats.passes += 1;
+		const uint32_t served = std::min(nqb * cluster, nq - b * nqb);  // queries of this launch, padding excluded
+		g_stats.algorithmic_bytes += uint64_t(ix->size) * pitchBf * 2 + uint64_t(ix->size) * 8 + uint64_t(served) * pitchBf * 2;
+		clusterUsed = std::max(clusterUsed, cluster);
+		b += cluster;
 	}
-	g_stats.tc_cluster = uint32_t(cluster);
+	g_stats.tc_cluster = clusterUsed;
 	g_stats.tc_kernel = 1;
-	g_stats.query_tile = nqb;
-	g_stats.algorithmic_bytes += uint64_t((nblocks + cluster - 1) / cluster) * (uint64_t(ix->size) * pitchBf * 2 + uint64_t(ix->size) * 4 +
-																			   uint64_t(nqb) * pitchBf * 2);
-	}
+	g_stats.query_tile = nqb * clusterUsed;
 	// exact re-rank of the candidates with the arithmetic of knn_scan_warp, then decode + labels
 	const size_t rsmem = size_t((ix->dim + 127) / 128) * 512 + size_t(kScanWarps) * (k1 + kCandBuf) * 8;
 	const float* norms = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
@@ -868,7 +684,6 @@ int rxgpu_index_clone(rxgpu_index** out, const rxgpu_index* src, uint64_t new_ca
 	ix->size = src->size;
 	ix->qt_override = src->qt_override;
 	ix->tc_mode = src->tc_mode;
-	ix->tc_variant = src->tc_variant;
 	ix->tc_cluster_max = src->tc_cluster_max;
 	RX_CUDA(cudaMemcpyAsync(ix->d_rows, src->d_rows, size_t(src->size) * src->pitch * sizeof(float), cudaMemcpyDeviceToDevice, ix->stream));
 	RX_CUDA(cudaMemcpyAsync(ix->d_labels, src->d_labels, size_t(src->size) * sizeof(uint64_t), cudaMemcpyDeviceToDevice, ix->stream));
@@ -1138,13 +953,11 @@ int rxgpu_set_query_tile(rxgpu_index* ix, uint32_t qt) {
 	return 0;
 }
 int rxgpu_set_tensor_core_filter(rxgpu_index* ix, int mode) {
-	if (!ix || mode < 0 || mode > 17 || mode == 7 || mode == 8 || (mode >= 10 && mode <= 13)) {
-		return fail(RXGPU_ERR_PARAMS, "rxgpu: tensor-core filter mode must be 0..6, 9 or 14..17");
+	if (!ix || mode < 0 || mode > 4) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: tensor-core filter mode must be 0..4");
 	}
 	ix->tc_mode = uint32_t(mode >= 3 ? 1 : mode);
-	ix->tc_variant = (mode == 3 || mode == 4) ? uint32_t(mode) : ((mode >= 14 && mode <= 16) ? 14u : 0u);
-	ix->tc_tail = mode == 17 ? 0u : 1u;
-	ix->tc_cluster_max = mode == 5 ? 1u : ((mode == 6 || mode == 14) ? 4u : ((mode == 9 || mode == 16) ? 8u : (mode == 15 ? 2u : 0u)));
+	ix->tc_cluster_max = mode == 4 ? 2u : 0u;
 	return 0;
 }
 int rxgpu_set_profile(int on) {

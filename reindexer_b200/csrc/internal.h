@@ -123,8 +123,6 @@ inline cudaError_t raiseSmemCeilingOnce(Kernel kfn, int device, int bytes) {  //
 // per-call scratch: searches are re-entrant, each takes one workspace from the pool
 struct Workspace {
 	cudaStream_t stream = nullptr;
-	cudaStream_t tail_stream = nullptr;  // the filter's tail grid (CTA pairs on the SMs the cluster-of-4 grid strands) runs beside the main one
-	cudaEvent_t tail_fork = nullptr, tail_join = nullptr;
 	DevBuf<float> d_queries;
 	DevBuf<uint64_t> d_lists;
 	DevBuf<uint64_t> d_floor;  // per-query floor keys between the rounds of a k > 255 search
@@ -160,11 +158,6 @@ struct Workspace {
 		if (stream) {
 			cudaStreamDestroy(stream);
 		}
-		if (tail_stream) {
-			cudaStreamDestroy(tail_stream);
-			cudaEventDestroy(tail_fork);
-			cudaEventDestroy(tail_join);
-		}
 	}
 };
 
@@ -187,7 +180,7 @@ struct rxgpu_index {
 	uint64_t size = 0;
 	int device = 0;
 	uint32_t flags = 0;
-	int sm_count = 148;
+	int sm_count = 132;
 	uint32_t qt_override = 0;
 	uint64_t version = 0;  // bumped by every mutation of rows/labels (staleness check of attached structures)
 
@@ -236,8 +229,6 @@ struct rxgpu_index {
 		}
 	}
 	uint32_t tc_mode = 0;  // 0 auto, 1 force on, 2 off
-	uint32_t tc_tail = 1;         // 1 = a tail grid of 2-CTA clusters scans a slice of the rows on the SMs the main grid cannot use
-	uint32_t tc_variant = 0;      // 0 = knn_tc_filter_q (query block in TMEM) when the dimension allows; 14 = knn_tc_filter_p (CTA pairs, cta_group::2); 3 / 4 = first-generation kernel (1 CTA / CTA pair)
 	uint32_t tc_cluster_max = 0;  // 0 = up to 4 CTAs per cluster
 
 	~rxgpu_index() {

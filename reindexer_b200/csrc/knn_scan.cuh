@@ -1,4 +1,4 @@
-// Brute-force float_vector scan kernels for sm_100a: distance (L2 / inner product / cosine) fused with top-k selection.
+// Brute-force float_vector scan kernels for sm_90a: distance (L2 / inner product / cosine) fused with top-k selection.
 //
 // Replaces the hot loop of hnswlib::BruteforceSearch::SearchKnn / SearchRange
 // (cpp_src/core/index/float_vector/hnswlib/bruteforce.cc:103-127, :129-143) and the distance functors it calls

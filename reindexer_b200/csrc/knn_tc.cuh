@@ -1,9 +1,9 @@
-// Tensor-core candidate filter for large query batches (sm_100a: TMA + tcgen05.mma + TMEM), exact results.
+// Tensor-core candidate filter for large query batches (sm_90a: TMA + wgmma + mbarrier, thread-block clusters), exact results.
 //
 // knn_scan_warp is HBM-bound only while <= ~16 queries share a pass; a batch of 1024 queries is FMA-bound there.  This kernel
-// computes APPROXIMATE scores for a block of NQ queries against every row with bf16 operands on the 5th-gen tensor cores and
-// keeps, per query, only the rows that can still be among the k best under a CERTIFIED error bound; the survivors (a few hundred
-// per query) are then re-ranked with the exact fp32 routine of knn_scan_warp, so the final result is identical to the exact scan.
+// computes APPROXIMATE scores for a block of NQ queries against every row with bf16 operands on the tensor cores and keeps, per
+// query, only the rows that can still be among the k best under a CERTIFIED error bound; the survivors (a few hundred per query)
+// are then re-ranked with the exact fp32 routine of knn_scan_warp, so the final result is identical to the exact scan.
 //
 //   error bound   |q~.v~ - q.v| <= c * ||q|| * ||v||,  c = 2^-8 + 2^-18 (two bf16 roundings, unit roundoff 2^-9 each)
 //                                                        + dim * 2^-23 (fp32 accumulation in the MMA); c = 0.0042 leaves 5% slack
@@ -14,15 +14,16 @@
 //                 upper bound of the final k1-th best TRUE distance; a row is a candidate iff lb <= tau_q.  tau starts from an
 //                 exact scan of the first rows (tc_init_tau) and only decreases.
 //
-// Roles (192 threads, 1 CTA per SM, persistent over 128-row tiles):
-//   warp 0    producer: bf16 shadow rows, 128 x 64 tiles (16 KB) through a 4-stage mbarrier ring.  The shadow is stored TILED and
-//             PRE-SWIZZLED in HBM ([tile of 64 rows][K chunk][64 x 128 B in the SWIZZLE_128B pattern]) so a stage is two
-//             contiguous 8 KB cp.async.bulk copies (row-major fp32 stays the source of truth; the shadow is private, derived)
-//   warp 1    allocates TMEM (512 columns), issues tcgen05.mma (M=128 rows, N=NQ queries, K=16) from shared-memory descriptors;
-//             the query block (NQ x dim bf16) is loaded once by TMA and stays resident in shared memory
-//   warps 2-5 epilogue: tcgen05.ld the 128 x NQ fp32 accumulators (double buffered in TMEM so the next tile's MMAs overlap),
-//             apply the metric, test against tau, append candidates to per-query lists in HBM, tighten tau
-// Bound: HBM (bf16 shadow: n*dim*2 bytes per pass of NQ queries); MMA time per tile is ~4x below the tile's HBM time.
+// Roles (384 threads = three warpgroups, 1 CTA per SM, persistent over 128-row tiles):
+//   warp 0       producer: the query block (NQ x dim bf16) once by TMA, then the bf16 shadow rows, 128 rows x 64 K (16 KB) per stage
+//                through a 4-stage mbarrier ring.  The shadow is stored TILED and PRE-SWIZZLED in HBM ([tile of 64 rows][K chunk]
+//                [64 x 128 B in the SWIZZLE_128B pattern]) so a stage is two contiguous 8 KB cp.async.bulk copies (row-major fp32
+//                stays the source of truth; the shadow is private, derived).  In a cluster of two CTAs (optional; single CTAs are
+//                faster on the H100) each CTA fetches half of every stage and multicasts it to both: one pass serves two query blocks.
+//   warpgroups 1, 2   consumers: warpgroup w multiplies rows [64 w, 64 w + 64) of every tile with the whole query block
+//                (wgmma.m64nNQk16, both operands from shared memory, fp32 accumulators in registers), releases each stage as soon
+//                as its MMAs retired, then applies the metric to its 64 x NQ scores, tests them against tau, appends candidates to
+//                per-query lists in HBM and tightens tau.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -32,20 +33,20 @@
 
 namespace rxgpu {
 
-constexpr int kTcThreads = 192;
-constexpr int kTcTileRows = 128;     // UMMA M
+constexpr int kTcThreads = 384;
+constexpr int kTcTileRows = 128;     // two wgmma M = 64 halves, one per consumer warpgroup
 constexpr int kTcChunkK = 64;        // bf16 elements per 128-byte swizzle row
 constexpr int kTcStages = 4;
-constexpr int kTcStageBytes = kTcTileRows * kTcChunkK * 2;  // 16 KB
+constexpr int kTcBlockBytes = 64 * kTcChunkK * 2;           // 8 KB: one 64-row shadow block of one K chunk
+constexpr int kTcStageBytes = 2 * kTcBlockBytes;            // 16 KB
+constexpr uint32_t kTcMaxNq = 128;   // queries per CTA (wgmma N <= 128 keeps the accumulators at <= 64 registers per thread)
 constexpr uint32_t kTcMaxK1 = 128;  // k + 1 <= 128: the bound list is scanned linearly under the per-query lock and ~25-35 (k + 1) candidates
                                     // per query must fit the 4096-entry lists (k = 10: 330; k = 63: 1600; an overflowing query takes the exact scan)
-constexpr uint32_t kTcQueueCap = 512;
 constexpr float kTcErrCoef = 0.0042f;  // see header comment
 
 struct TcArgs {
 	const unsigned char* shadow;  // bf16 shadow, [tile of 64 rows][K chunk][64 rows x 128 B, SWIZZLE_128B pattern pre-applied]
-	const float* vnorm;        // [n] ||row||_2 (fp32)
-	const float* vinv;         // [n] 1/||row|| (Cosine) or nullptr
+	const float2* vw;          // tc_make_vw: [rows padded to whole tiles] (max(||v||, tiny), w)
 	const float* qnorm;        // [nq_total] ||q||_2
 	unsigned int* tau;         // [nq_total] ordered-uint of the current threshold (map space), shared by all CTAs
 	float* ub_list;            // [nq_total][kTcMaxK1] the k1 smallest upper bounds over ALL rows seen by any CTA (guarded by ub_lock)
@@ -56,16 +57,16 @@ struct TcArgs {
 	uint32_t cand_cap;
 	uint32_t n;                // rows
 	uint32_t kchunks;          // padded dim / 64
-	uint32_t nq_block;         // UMMA N (multiple of 32, <= 256): queries resident in this launch
 	uint32_t nq_total;         // queries in the whole batch
-	uint32_t q0;               // first query of this launch; CTA rank r of a cluster owns queries [q0 + r*nq_block, +nq_block)
+	uint32_t q0;               // first query of this launch; CTA rank r of a cluster owns queries [q0 + r*NQ, +NQ)
 	uint32_t k1;
 	int metric;                // kL2 / kIP / kCos
 };
 
+// shared memory: query block, stage ring, barriers, then per consumer warpgroup the (P, R) pairs and thresholds of the block
 __host__ __device__ inline size_t tc_smem_bytes(uint32_t nq_block, uint32_t kchunks) {
 	return 1024 /*align slack*/ + size_t(nq_block) * kchunks * 128 + size_t(kTcStages) * kTcStageBytes + 256 /*barriers*/ +
-		   size_t(nq_block) * (4 + 4 + 8) + size_t(kTcQueueCap) * 8 + 64;
+		   size_t(nq_block) * (4 /*qe*/ + 2 * (4 + 8) /*thr, pr per warpgroup*/) + 64;
 }
 
 // ---- PTX wrappers -------------------------------------------------------------------------------------------------------------
@@ -92,6 +93,12 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 		"r"(parity)
 		: "memory");
 }
+// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster (the CTA itself included)
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+	uint32_t remote;
+	asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
+	asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int32_t x, int32_t y) {
 	asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
 					 smem_u32(dst)),
@@ -104,31 +111,14 @@ __device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t b
 				 "r"(bytes), "r"(smem_u32(bar))
 				 : "memory");
 }
-// warm the L2 with a block this SM will copy a few tiles from now: the later bulk copy then pays the L2 latency, not the HBM one,
-// which a shared-memory ring of only one or two tiles cannot hide
-__device__ __forceinline__ void bulk_prefetch_l2(const void* src, uint32_t bytes) {
-	asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ void bulk_load_mc(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint16_t mask) {
 	asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
 					 smem_u32(dst)),
 				 "l"(src), "r"(bytes), "r"(smem_u32(bar)), "h"(mask)
 				 : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_mc(void* dst, const CUtensorMap* map, uint64_t* bar, int32_t x, int32_t y, uint16_t mask) {
-	asm volatile(
-		"cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;" ::
-			"r"(smem_u32(dst)),
-		"l"(map), "r"(smem_u32(bar)), "r"(x), "r"(y), "h"(mask)
-		: "memory");
-}
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-	asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-				 "h"(mask)
-				 : "memory");
-}
-// true in exactly one lane of a converged warp (elect.sync): the single-thread tcgen05 / TMA instructions are issued under this
-// predicate from warp-uniform code, so their operands stay in uniform registers
+// true in exactly one lane of a converged warp (elect.sync): the single-thread TMA instructions are issued under this predicate
+// from warp-uniform code, so their operands stay in uniform registers
 __device__ __forceinline__ bool elect_one_sync() {
 	uint32_t p;
 	asm volatile(
@@ -149,43 +139,100 @@ __device__ __forceinline__ void cluster_sync_all() {
 	asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
 	asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// shared-memory matrix descriptor, K-major, SWIZZLE_128B: 8-row groups are 1024 B apart (SBO), one swizzle atom along K (LBO unused)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// wgmma shared-memory matrix descriptor, K-major, SWIZZLE_128B: 8-row groups are 1024 B apart (SBO), one swizzle atom along K
+// (LBO unused); the K step of 16 bf16 inside the atom advances the start address by 32 bytes
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
 	uint64_t d = 0;
 	d |= uint64_t((smem_addr & 0x3FFFFu) >> 4);  // start address, bits [0,14)
-	d |= uint64_t(0) << 16;                      // leading byte offset (unused for swizzled K-major)
+	d |= uint64_t(1) << 16;                      // leading byte offset (unused for swizzled K-major)
 	d |= uint64_t(1024 >> 4) << 32;              // stride byte offset, bits [32,46)
-	d |= uint64_t(1) << 46;                      // descriptor version (sm_100)
-	d |= uint64_t(2) << 61;                      // layout type: SWIZZLE_128B
+	d |= uint64_t(1) << 62;                      // layout type: SWIZZLE_128B
 	return d;
 }
-// instruction descriptor, kind::f16: D = f32, A = B = bf16, both K-major, dense
-__device__ __forceinline__ uint32_t umma_idesc_bf16(uint32_t m, uint32_t n) {
-	return (1u << 4) | (1u << 7) | (1u << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+	asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D[64 rows x N queries] (+)= A[64 x 16] (smem) x B[N x 16]^T (smem), bf16 in, fp32 accumulate; d = the thread's N / 2 accumulators
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
 	asm volatile(
 		"{\n"
 		".reg .pred p;\n"
-		"setp.ne.b32 p, %4, 0;\n"
-		"tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-		"}\n" ::"r"(tmem_d),
-		"l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-		: "memory");
+		"setp.ne.b32 p, %18, 0;\n"
+		"wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+		"{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, "
+		"%16, %17, p, 1, 1, 0, 0;\n"
+		"}\n"
+		: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+		  "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+		: "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-	asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
 	asm volatile(
-		"tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-		"{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-		: "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-		  "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-		  "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-		  "=r"(r[31])
-		: "r"(taddr));
-	asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+		"{\n"
+		".reg .pred p;\n"
+		"setp.ne.b32 p, %34, 0;\n"
+		"wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+		"{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+		"%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+		"%32, %33, p, 1, 1, 0, 0;\n"
+		"}\n"
+		: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+		  "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+		  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+		: "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_m64n96k16(float (&d)[48], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+	asm volatile(
+		"{\n"
+		".reg .pred p;\n"
+		"setp.ne.b32 p, %50, 0;\n"
+		"wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 "
+		"{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+		"%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+		"%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47}, "
+		"%48, %49, p, 1, 1, 0, 0;\n"
+		"}\n"
+		: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+		  "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+		  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+		  "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+		: "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+	asm volatile(
+		"{\n"
+		".reg .pred p;\n"
+		"setp.ne.b32 p, %66, 0;\n"
+		"wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+		"{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+		"%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+		"%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+		"%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+		"%64, %65, p, 1, 1, 0, 0;\n"
+		"}\n"
+		: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+		  "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+		  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+		  "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+		  "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
+		  "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+		: "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+	if constexpr (N == 32) {
+		wgmma_m64n32k16(d, adesc, bdesc, accumulate);
+	} else if constexpr (N == 64) {
+		wgmma_m64n64k16(d, adesc, bdesc, accumulate);
+	} else if constexpr (N == 96) {
+		wgmma_m64n96k16(d, adesc, bdesc, accumulate);
+	} else {
+		static_assert(N == 128, "query block of 32, 64, 96 or 128");
+		wgmma_m64n128k16(d, adesc, bdesc, accumulate);
+	}
 }
 
 // The candidate test  lb = d~ - e <= tau  rewritten as ONE fused multiply-add and one compare on the raw accumulator s = q~.v~:
@@ -206,85 +253,116 @@ __device__ __forceinline__ float2 tc_make_pr(int metric, float tau, float qe) {
 	return make_float2(-qe, 0.5f * ((1.f - kTcL2Eps) * qn * qn - tau));
 }
 
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-	asm volatile(
-		"tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-		"{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-		: "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-		  "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-		  "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-		  "=r"(r[31])
-		: "r"(taddr));
+// The rare path of the epilogue: row `row` passed the test for query `q` (raw accumulator s, row norm vn, qe = c * ||q||).  Appends
+// the candidate, and when its upper bound beats the query's current threshold, inserts it into the query's global bound list (under
+// the per-query lock; other CTAs contend) and tightens the global tau.  Returns the new threshold (+inf when it did not change).
+// Kept out of line: it runs for a few hundred of 10M rows per query, and inlining it at every accumulator only costs instruction cache.
+__device__ __noinline__ float tc_candidate(const TcArgs& a, uint32_t q, uint32_t row, float s, float vn, float qe, float tau) {
+	float d, e;
+	if (a.metric == kL2) {
+		const float qn = qe * (1.f / kTcErrCoef);
+		d = fmaf(-2.f, s, fmaf(qn, qn, vn * vn));
+		e = 2.f * qe * vn + kTcL2Eps * (qn * qn + vn * vn);
+	} else if (a.metric == kCos) {
+		const float vinv = 1.f / vn;  // within 1e-5 of the stored coefficient (normalize.cc shortcut), inside the slack
+		d = -s * vinv;
+		e = qe * 1.0001f;
+	} else {
+		d = -s;
+		e = qe * vn;
+	}
+	const unsigned pos = atomicAdd(&a.cand_count[q], 1u);
+	if (pos < a.cand_cap) {
+		a.cand_rows[size_t(q) * a.cand_cap + pos] = row;
+	}
+	const float ub = d + e;
+	float tightened = INFINITY;
+	if (ub < tau && row >= a.init_rows) {
+		while (atomicCAS(&a.ub_lock[q], 0u, 1u) != 0u) {
+		}
+		__threadfence();
+		volatile float* list = a.ub_list + size_t(q) * kTcMaxK1;
+		uint32_t mi = 0;
+		float mx = list[0];
+		for (uint32_t x = 1; x < a.k1; ++x) {
+			const float y = list[x];
+			if (y > mx) {
+				mx = y;
+				mi = x;
+			}
+		}
+		if (ub < mx) {
+			list[mi] = ub;
+			float nmx = list[0];
+			for (uint32_t x = 1; x < a.k1; ++x) {
+				nmx = fmaxf(nmx, list[x]);
+			}
+			atomicMin(&a.tau[q], float_ord(nmx));
+			tightened = nmx;
+		} else {
+			tightened = mx;
+		}
+		__threadfence();
+		atomicExch(&a.ub_lock[q], 0u);
+	}
+	return tightened;
 }
 
 // ---- the filter kernel -----------------------------------------------------------------------------------------------------------
-// kCluster == 2: a cluster of two CTAs walks the same row tiles with DIFFERENT query blocks; each CTA fetches half of every
-// stage (64 rows) and TMA-multicasts it into both CTAs' shared memory, so one pass over the shadow serves 2 x nq_block queries.
-template <int kCluster>
+// kNq = queries per CTA (wgmma N); kCluster = CTAs that walk the same row tiles with DIFFERENT query blocks, sharing every stage
+// through TMA multicast.
+template <int kNq, int kCluster>
 __global__ void __launch_bounds__(kTcThreads, 1)
-	knn_tc_filter(const __grid_constant__ CUtensorMap map_queries, const TcArgs a) {
+	knn_tc_filter(const __grid_constant__ CUtensorMap map_queries, const __grid_constant__ TcArgs a) {
+	static_assert(kNq % 32 == 0 && kNq <= int(kTcMaxNq), "query block");
+	static_assert(kCluster == 1 || kCluster == 2, "a stage is split in 1 or 2 equal copies");
 	extern __shared__ unsigned char smem_raw[];
 	unsigned char* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // offset arithmetic keeps the shared window
-	const uint32_t qchunk_bytes = a.nq_block * 128;                   // one K-chunk of the query block: nq_block rows x 128 B
-	unsigned char* s_q = base;                                        // [kchunks][nq_block][128 B], swizzled by TMA
-	unsigned char* s_rows = s_q + size_t(a.kchunks) * qchunk_bytes;   // [stages][128][128 B]   (1024-aligned: nq_block % 8 == 0)
+	constexpr uint32_t kQchunkBytes = kNq * 128;                       // one K-chunk of the query block: kNq rows x 128 B
+	unsigned char* s_q = base;                                         // [kchunks][kNq][128 B], swizzled by TMA
+	unsigned char* s_rows = s_q + size_t(a.kchunks) * kQchunkBytes;    // [stages][2 blocks][64][128 B]   (1024-aligned: kNq % 8 == 0)
 	uint64_t* bars = reinterpret_cast<uint64_t*>(s_rows + size_t(kTcStages) * kTcStageBytes);
 	uint64_t* full_bar = bars;                   // [stages] TMA -> MMA
-	uint64_t* empty_bar = bars + kTcStages;      // [stages] MMA -> TMA
+	uint64_t* empty_bar = bars + kTcStages;      // [stages] MMA (every consumer warp of every CTA of the cluster) -> TMA
 	uint64_t* q_bar = bars + 2 * kTcStages;      // queries resident
-	uint64_t* acc_full = q_bar + 1;              // [2] MMA -> epilogue
-	uint64_t* acc_empty = acc_full + 2;          // [2] epilogue -> MMA
-	uint32_t* s_tmem = reinterpret_cast<uint32_t*>(acc_empty + 2);
-	float* s_thr = reinterpret_cast<float*>(bars + 32);                // [nq_block] current tau (map space)
-	float* s_qe = s_thr + a.nq_block;                                  // [nq_block] c * ||q||
-	float2* s_pr = reinterpret_cast<float2*>(s_qe + a.nq_block);      // [nq_block] (P, R): candidate iff s - w_row >= fma(P, ||v||, R)
-	uint2* s_queue = reinterpret_cast<uint2*>(s_pr + a.nq_block);     // (query, ub bits)
-	uint32_t* s_qcount = reinterpret_cast<uint32_t*>(s_queue + kTcQueueCap);
+	float* s_qe = reinterpret_cast<float*>(bars + 32);                 // [kNq] c * ||q||
+	float* s_thr = s_qe + kNq;                                         // [2][kNq] current tau (map space), per consumer warpgroup
+	float2* s_pr = reinterpret_cast<float2*>(s_thr + 2 * kNq);         // [2][kNq] (P, R): candidate iff s - w_row >= fma(P, ||v||, R)
 
 	const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;  // provably warp-uniform
 	const uint32_t ntiles = (a.n + kTcTileRows - 1) / kTcTileRows;
 	const uint32_t crank = kCluster > 1 ? cluster_ctarank() : 0u;
 	const uint32_t cid = blockIdx.x / kCluster, ncl = gridDim.x / kCluster;  // tile walkers
-	const uint32_t q0 = a.q0 + crank * a.nq_block;
-	const uint32_t nq_valid = q0 < a.nq_total ? min(a.nq_block, a.nq_total - q0) : 0u;
+	const uint32_t q0 = a.q0 + crank * kNq;
+	const uint32_t nq_valid = q0 < a.nq_total ? min(uint32_t(kNq), a.nq_total - q0) : 0u;
 
 	if (threadIdx.x == 0) {
 		for (int s = 0; s < kTcStages; ++s) {
 			mbar_init(&full_bar[s], 1);
-			mbar_init(&empty_bar[s], kCluster);  // every consumer CTA of the stage must release it
+			mbar_init(&empty_bar[s], 8 * kCluster);  // the eight consumer warps of every CTA that reads the stage's bytes
 		}
 		mbar_init(q_bar, 1);
-		for (int s = 0; s < 2; ++s) {
-			mbar_init(&acc_full[s], 1);
-			mbar_init(&acc_empty[s], 4);  // one arrive per epilogue warp
-		}
-		*s_qcount = 0;
 		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 	}
-	for (uint32_t i = threadIdx.x; i < a.nq_block; i += blockDim.x) {
+	for (uint32_t i = threadIdx.x; i < kNq; i += blockDim.x) {
 		const bool valid = i < nq_valid;
-		s_thr[i] = valid ? ord_float(a.tau[q0 + i]) : -INFINITY;
+		const float thr = valid ? ord_float(a.tau[q0 + i]) : -INFINITY;
 		s_qe[i] = valid ? kTcErrCoef * a.qnorm[q0 + i] : 0.f;
-		s_pr[i] = valid ? tc_make_pr(a.metric, s_thr[i], s_qe[i]) : make_float2(0.f, INFINITY);  // padding queries never match
+		const float2 pr = valid ? tc_make_pr(a.metric, thr, s_qe[i]) : make_float2(0.f, INFINITY);  // padding queries never match
+		s_thr[i] = s_thr[kNq + i] = thr;
+		s_pr[i] = s_pr[kNq + i] = pr;
 	}
-	if (warp == 1) {  // TMEM: 512 columns = 2 accumulator buffers of up to 256 fp32 columns
-		asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(s_tmem)) : "memory");
-		asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-	}
-	asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
 	__syncthreads();
 	if constexpr (kCluster > 1) {
-		cluster_sync_all();  // the peer's barriers exist before anything of ours can signal them
+		cluster_sync_all();  // the peers' barriers exist before anything of ours can signal them
 	}
-	asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-	const uint32_t tmem_base = *s_tmem;
 
 	if (warp == 0) {
 		// ===== TMA producer: the whole warp walks the loop, one elected lane issues (operands stay in uniform registers) =====
 		if (elect_one_sync()) {
-			mbar_expect_tx(q_bar, a.kchunks * qchunk_bytes);
+			mbar_expect_tx(q_bar, a.kchunks * kQchunkBytes);
 			for (uint32_t kc = 0; kc < a.kchunks; ++kc) {
-				tma_load_2d(s_q + size_t(kc) * qchunk_bytes, &map_queries, q_bar, int32_t(kc * kTcChunkK), int32_t(q0));
+				tma_load_2d(s_q + size_t(kc) * kQchunkBytes, &map_queries, q_bar, int32_t(kc * kTcChunkK), int32_t(q0));
 			}
 		}
 		__syncwarp();
@@ -292,17 +370,19 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		for (uint32_t t = cid; t < ntiles; t += ncl) {
 			for (uint32_t kc = 0; kc < a.kchunks; ++kc) {
 				mbar_wait(&empty_bar[stage], phase ^ 1);
-				// a 128-row stage = the 64-row shadow sub-tiles 2t and 2t+1 of this K chunk, 8 KB each, contiguous in HBM
-				const unsigned char* src = a.shadow + (size_t(2 * t) * a.kchunks + kc) * 8192u;
+				// a 128-row stage = the 64-row shadow blocks 2t and 2t+1 of this K chunk, 8 KB each, kchunks * 8 KB apart in HBM
+				const unsigned char* src = a.shadow + (size_t(2 * t) * a.kchunks + kc) * kTcBlockBytes;
 				unsigned char* dst = s_rows + size_t(stage) * kTcStageBytes;
 				if (elect_one_sync()) {
 					mbar_expect_tx(&full_bar[stage], kTcStageBytes);
-					if constexpr (kCluster > 1) {  // my half of the stage, delivered to both CTAs
-						bulk_load_mc(dst + crank * 8192u, src + size_t(crank) * a.kchunks * 8192u, 8192u, &full_bar[stage],
+					if constexpr (kCluster == 1) {
+						bulk_load(dst, src, kTcBlockBytes, &full_bar[stage]);
+						bulk_load(dst + kTcBlockBytes, src + size_t(a.kchunks) * kTcBlockBytes, kTcBlockBytes, &full_bar[stage]);
+					} else {  // my 1/C of the stage, delivered to every CTA of the cluster
+						constexpr uint32_t kPart = kTcStageBytes / kCluster;
+						const uint32_t blk = crank * kPart / kTcBlockBytes, off = crank * kPart % kTcBlockBytes;
+						bulk_load_mc(dst + blk * kTcBlockBytes + off, src + size_t(blk) * a.kchunks * kTcBlockBytes + off, kPart, &full_bar[stage],
 									 uint16_t((1u << kCluster) - 1u));
-					} else {
-						bulk_load(dst, src, 8192u, &full_bar[stage]);
-						bulk_load(dst + 8192u, src + size_t(a.kchunks) * 8192u, 8192u, &full_bar[stage]);
 					}
 				}
 				__syncwarp();
@@ -312,188 +392,103 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 				}
 			}
 		}
-	} else if (warp == 1) {
-		// ===== MMA issuer (same structure: convergent loop, elected issue) =====
-		const uint32_t idesc = umma_idesc_bf16(kTcTileRows, a.nq_block);
+	} else if (warp >= 4) {
+		// ===== consumer warpgroup wg: rows [64 wg, 64 wg + 64) of every tile =====
+		const uint32_t wg = uint32_t(warp) / 4 - 1, wtid = threadIdx.x - 128 * (wg + 1);
+		float* thr = s_thr + wg * kNq;
+		float2* pr = s_pr + wg * kNq;
+		// accumulator fragment of wgmma.m64nN: d[4j + {0,1}] = (row r0, query 8j + 2c + {0,1}), d[4j + {2,3}] = the same for row r0 + 8
+		const uint32_t r0 = (wtid >> 5) * 16 + (lane >> 2), c2 = 2 * (lane & 3);
+		const uint32_t my_q = wtid;  // the query whose threshold this thread refreshes from the global list
+		unsigned int tau_ahead = my_q < nq_valid ? a.tau[q0 + my_q] : 0u;
+		auto release = [&](uint32_t st) {  // this warp is done with stage st in every CTA that reads it
+			if constexpr (kCluster == 1) {
+				mbar_arrive(&empty_bar[st]);
+			} else {
+				for (uint32_t c = 0; c < uint32_t(kCluster); ++c) {
+					mbar_arrive_cluster(&empty_bar[st], c);
+				}
+			}
+		};
 		mbar_wait(q_bar, 0);
-		uint32_t stage = 0, phase = 0, it = 0;
-		for (uint32_t t = cid; t < ntiles; t += ncl, ++it) {
-			const uint32_t acc = it & 1, acc_phase = (it >> 1) & 1;
-			mbar_wait(&acc_empty[acc], acc_phase ^ 1);
-			asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-			const uint32_t tmem_d = tmem_base + acc * 256;
+		uint32_t stage = 0, phase = 0;
+		for (uint32_t t = cid; t < ntiles; t += ncl) {
+			// refresh tau from the other CTAs: the global load was issued during the PREVIOUS tile, so its latency is hidden
+			if (my_q < nq_valid) {
+				const float tn = ord_float(tau_ahead);
+				if (tn < thr[my_q]) {
+					thr[my_q] = tn;
+					pr[my_q] = tc_make_pr(a.metric, tn, s_qe[my_q]);
+				}
+				tau_ahead = a.tau[q0 + my_q];
+			}
+			const uint32_t row0 = t * kTcTileRows + wg * 64 + r0, row1 = row0 + 8;
+			const float2 vw0 = a.vw[row0], vw1 = a.vw[row1];  // rows are padded to whole tiles; consumed after the MMAs
+			float acc[kNq / 2];
+#pragma unroll
+			for (int i = 0; i < kNq / 2; ++i) {
+				acc[i] = 0.f;
+			}
+			uint32_t prev = 0;
 			for (uint32_t kc = 0; kc < a.kchunks; ++kc) {
 				mbar_wait(&full_bar[stage], phase);
-				asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-				const uint32_t a_addr = smem_u32(s_rows + size_t(stage) * kTcStageBytes);
-				const uint32_t b_addr = smem_u32(s_q + size_t(kc) * qchunk_bytes);
-				if (elect_one_sync()) {
+				const uint32_t a_addr = smem_u32(s_rows + size_t(stage) * kTcStageBytes + wg * kTcBlockBytes);
+				const uint32_t b_addr = smem_u32(s_q + size_t(kc) * kQchunkBytes);
+				wgmma_fence();
 #pragma unroll
-					for (uint32_t k = 0; k < kTcChunkK / 16; ++k) {  // UMMA_K = 16 bf16 = 32 bytes inside the 128-byte swizzle row
-						umma_bf16(tmem_d, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc, (kc | k) != 0);
-					}
-					if constexpr (kCluster > 1) {  // the stage is rewritten by BOTH producers: release it in both CTAs
-						umma_commit_mc(&empty_bar[stage], uint16_t((1u << kCluster) - 1u));
-					} else {
-						umma_commit(&empty_bar[stage]);  // frees the smem stage when these MMAs retire
-					}
-					if (kc + 1 == a.kchunks) {
-						umma_commit(&acc_full[acc]);  // accumulator complete -> epilogue
+				for (uint32_t k = 0; k < kTcChunkK / 16; ++k) {  // K = 16 bf16 = 32 bytes inside the 128-byte swizzle row
+					wgmma_bf16<kNq>(acc, wgmma_desc_sw128(a_addr + k * 32), wgmma_desc_sw128(b_addr + k * 32), (kc | k) != 0);
+				}
+				wgmma_commit();
+				if (kc > 0) {  // the previous chunk's MMAs have retired: its stage goes back to the producers
+					wgmma_wait<1>();
+					if (lane == 0) {
+						release(prev);
 					}
 				}
-				__syncwarp();
+				prev = stage;
 				if (++stage == kTcStages) {
 					stage = 0;
 					phase ^= 1;
 				}
 			}
-		}
-	} else {
-		// ===== epilogue warps 2..5: TMEM lane quadrant = warp % 4 =====
-		const uint32_t quad = warp & 3;
-		const uint32_t row_in_tile = quad * 32 + lane;
-		uint32_t it = 0;
-		unsigned int tau_ahead0 = float_ord(INFINITY), tau_ahead1 = float_ord(INFINITY);
-		float vn_ahead = 0.f, vinv_ahead = 1.f;
-		{
-			const uint32_t frow = cid * kTcTileRows + row_in_tile;
-			if (cid < ntiles && frow < a.n) {
-				vn_ahead = a.vnorm[frow];
-				vinv_ahead = a.vinv ? a.vinv[frow] : 1.f;
-			}
-		}
-		for (uint32_t t = cid; t < ntiles; t += ncl, ++it) {
-			const uint32_t acc = it & 1, acc_phase = (it >> 1) & 1;
-			const uint32_t row = t * kTcTileRows + row_in_tile;
-			const bool row_ok = row < a.n;
-			// refresh tau from the other CTAs (thread i of the epilogue group owns queries i and i + 128).  The global loads were
-			// issued during the PREVIOUS tile, so their latency is hidden; the ones for the next tile are issued now.
-			{
-				const uint32_t i0 = threadIdx.x - 64, i1 = i0 + 128;
-				if (i0 < nq_valid) {
-					s_thr[i0] = fminf(s_thr[i0], ord_float(tau_ahead0));
-					s_pr[i0] = tc_make_pr(a.metric, s_thr[i0], s_qe[i0]);
-					tau_ahead0 = a.tau[q0 + i0];
-				}
-				if (i1 < nq_valid) {
-					s_thr[i1] = fminf(s_thr[i1], ord_float(tau_ahead1));
-					s_pr[i1] = tc_make_pr(a.metric, s_thr[i1], s_qe[i1]);
-					tau_ahead1 = a.tau[q0 + i1];
-				}
-			}
-			const float vn = vn_ahead, vinv = vinv_ahead;
-			const float w_row = a.metric == kL2 ? 0.5f * (1.f - kTcL2Eps) * vn * vn : 0.f;
-			const float vn_t = fmaxf(vn, 1e-30f);  // keeps -inf * ||v|| = -inf (tau still +inf) for all-zero rows
-			{
-				const uint32_t nrow = (t + ncl) * kTcTileRows + row_in_tile;
-				const bool nok = t + ncl < ntiles && nrow < a.n;
-				vn_ahead = nok ? a.vnorm[nrow] : 0.f;
-				vinv_ahead = (nok && a.vinv) ? a.vinv[nrow] : 1.f;
-			}
-			asm volatile("bar.sync 1, 128;" ::: "memory");
-			mbar_wait(&acc_full[acc], acc_phase);
-			asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-			for (uint32_t c0 = 0; c0 < a.nq_block; c0 += 32) {
-				uint32_t v[32];
-				tmem_ld32(tmem_base + acc * 256 + c0 + ((quad * 32) << 16), v);
-				// hot path: one broadcast LDS.64, one FFMA, one compare per element; hits are collected in a bit mask
-				uint32_t hits = 0;
-#pragma unroll
-				for (int j = 0; j < 32; ++j) {
-					const float2 pr = s_pr[c0 + j];
-					const float sv = __uint_as_float(v[j]) - w_row;
-					hits |= uint32_t(sv >= fmaf(pr.x, vn_t, pr.y)) << j;
-				}
-				hits = row_ok ? hits : 0u;
-				const unsigned any_hits = __reduce_or_sync(0xffffffffu, hits);
-				if (any_hits) {  // rare path: exact bounds, candidate append, threshold tightening (static indices into v[])
-#pragma unroll
-					for (int j = 0; j < 32; ++j) {
-						if (!(any_hits & (1u << j)) || !(hits & (1u << j))) {
-							continue;
-						}
-						const uint32_t q = c0 + j;
-						const float s = __uint_as_float(v[j]);
-						float d, e;
-						if (a.metric == kL2) {
-							const float qn = s_qe[q] * (1.f / kTcErrCoef);
-							d = fmaf(-2.f, s, fmaf(qn, qn, vn * vn));
-							e = 2.f * s_qe[q] * vn + kTcL2Eps * (qn * qn + vn * vn);
-						} else if (a.metric == kCos) {
-							d = -s * vinv;
-							e = s_qe[q] * vn * vinv;
-						} else {
-							d = -s;
-							e = s_qe[q] * vn;
-						}
-						const unsigned pos = atomicAdd(&a.cand_count[q0 + q], 1u);
-						if (pos < a.cand_cap) {
-							a.cand_rows[size_t(q0 + q) * a.cand_cap + pos] = row;
-						}
-						const float ub = d + e;
-						if (ub < s_thr[q] && row >= a.init_rows) {
-							const uint32_t slot = atomicAdd(s_qcount, 1u);
-							if (slot < kTcQueueCap) {
-								s_queue[slot] = make_uint2(q, __float_as_uint(ub));
-							}
-						}
-					}
-				}
-			}
-			// accumulator drained: hand the TMEM buffer back to the MMA warp
-			asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-			__syncwarp();
+			wgmma_wait<0>();
 			if (lane == 0) {
-				mbar_arrive(&acc_empty[acc]);
+				release(prev);
 			}
-			asm volatile("bar.sync 1, 128;" ::: "memory");
-			// tighten tau: one thread folds the queued upper bounds into the per-query global lists (rare after the first tiles)
-			if (threadIdx.x == 64) {
-				const uint32_t cnt = min(*s_qcount, kTcQueueCap);
-				for (uint32_t i = 0; i < cnt; ++i) {
-					const uint32_t q = s_queue[i].x;
-					const float ub = __uint_as_float(s_queue[i].y);
-					const uint32_t gq = q0 + q;
-					if (!(ub < ord_float(*reinterpret_cast<volatile unsigned int*>(&a.tau[gq])))) {
-						continue;
-					}
-					while (atomicCAS(&a.ub_lock[gq], 0u, 1u) != 0u) {
-					}
-					__threadfence();
-					volatile float* list = a.ub_list + size_t(gq) * kTcMaxK1;
-					uint32_t mi = 0;
-					float mx = list[0];
-					for (uint32_t j = 1; j < a.k1; ++j) {
-						const float v = list[j];
-						if (v > mx) {
-							mx = v;
-							mi = j;
-						}
-					}
-					if (ub < mx) {
-						list[mi] = ub;
-						float nmx = list[0];
-						for (uint32_t j = 1; j < a.k1; ++j) {
-							nmx = fmaxf(nmx, list[j]);
-						}
-						atomicMin(&a.tau[gq], float_ord(nmx));
-						s_thr[q] = fminf(s_thr[q], nmx);
-						s_pr[q] = tc_make_pr(a.metric, s_thr[q], s_qe[q]);
-					}
-					__threadfence();
-					atomicExch(&a.ub_lock[gq], 0u);
+			asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // the refreshed (P, R) of all queries are visible
+			// a tightened threshold takes effect at once for the rest of the tile: other threads of the warpgroup may store a looser one
+			// for the same query concurrently, which is still a valid upper bound (each store is a single aligned store)
+			auto tighten = [&](uint32_t qq, float nt) {
+				if (nt < thr[qq]) {
+					thr[qq] = nt;
+					pr[qq] = tc_make_pr(a.metric, nt, s_qe[qq]);
 				}
-				*s_qcount = 0;
+			};
+			// hot path: one broadcast LDS.128 per two queries, one FFMA and one compare per score
+			const bool ok0 = row0 < a.n, ok1 = row1 < a.n;
+#pragma unroll
+			for (int j = 0; j < kNq / 8; ++j) {
+				const uint32_t q = 8 * j + c2;
+				const float4 p2 = *reinterpret_cast<const float4*>(&pr[q]);  // (P, R) of queries q and q + 1
+				const bool h0 = ok0 && acc[4 * j] - vw0.y >= fmaf(p2.x, vw0.x, p2.y);
+				const bool h1 = ok0 && acc[4 * j + 1] - vw0.y >= fmaf(p2.z, vw0.x, p2.w);
+				const bool h2 = ok1 && acc[4 * j + 2] - vw1.y >= fmaf(p2.x, vw1.x, p2.y);
+				const bool h3 = ok1 && acc[4 * j + 3] - vw1.y >= fmaf(p2.z, vw1.x, p2.w);
+				if (h0 | h1 | h2 | h3) {  // rare path: exact bounds, candidate append, threshold tightening
+					if (h0) tighten(q, tc_candidate(a, q0 + q, row0, acc[4 * j], vw0.x, s_qe[q], thr[q]));
+					if (h1) tighten(q + 1, tc_candidate(a, q0 + q + 1, row0, acc[4 * j + 1], vw0.x, s_qe[q + 1], thr[q + 1]));
+					if (h2) tighten(q, tc_candidate(a, q0 + q, row1, acc[4 * j + 2], vw1.x, s_qe[q], thr[q]));
+					if (h3) tighten(q + 1, tc_candidate(a, q0 + q + 1, row1, acc[4 * j + 3], vw1.x, s_qe[q + 1], thr[q + 1]));
+				}
 			}
-			asm volatile("bar.sync 1, 128;" ::: "memory");
+			__syncwarp();  // the rare path diverges (per-lane lock loops): reconverge before the .aligned wgmma of the next tile
+			asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // nobody still reads (P, R) when the next refresh writes them
 		}
 	}
 	__syncthreads();
 	if constexpr (kCluster > 1) {
-		cluster_sync_all();  // nobody leaves while the peer may still multicast into this CTA or signal its barriers
-	}
-	if (warp == 1) {
-		asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
+		cluster_sync_all();  // nobody leaves while a peer may still multicast into this CTA or signal its barriers
 	}
 }
 
@@ -622,7 +617,7 @@ __global__ void tc_make_vw(const float* vnorm, uint32_t n, uint32_t padded, int 
 
 // ---- helpers: bf16 shadow, norms, query preparation, threshold init ---------------------------------------------------------------
 // rows fp32 [n][pitch] -> bf16 shadow + ||row||_2.  Shadow layout: [tile of 64 rows][K chunk of 64][64 rows x 128 bytes], and inside
-// every 8 KB block the 16-byte units of row r are XOR-permuted with (r % 8) -- the SWIZZLE_128B pattern tcgen05.mma expects in
+// every 8 KB block the 16-byte units of row r are XOR-permuted with (r % 8) -- the SWIZZLE_128B pattern wgmma expects in
 // shared memory -- so that a plain contiguous cp.async.bulk brings a ready-to-multiply operand tile.
 __global__ void tc_convert_rows(const float* rows, uint32_t pitch, uint32_t dim, uint32_t row_begin, uint32_t row_end, __nv_bfloat16* shadow,
 								uint32_t kchunks, float* vnorm) {

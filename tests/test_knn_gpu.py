@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA brute-force path, called through the C ABI, against the oracle
+"""GPU parity tests (run with -m gpu on an H100): the CUDA brute-force path, called through the C ABI, against the oracle
 (the reference's own code in oracle/_ref when present, else the pinned C port) and the committed golden fixtures."""
 import threading
 

@@ -1,4 +1,4 @@
-"""GPU tests of the tensor-core filter path (tcgen05 + TMA + TMEM, knn_tc.cuh): for large query batches the bf16 tensor-core
+"""GPU tests of the tensor-core filter path (wgmma + TMA + mbarrier, knn_tc.cuh): for large query batches the bf16 tensor-core
 scores only SELECT candidates under a certified error bound; the exact fp32 routine re-ranks them.  So the answers must be
 bit-identical to the exact scan (same labels, same order, same distance bits) -- and therefore match the oracle like it does."""
 import numpy as np
@@ -25,7 +25,8 @@ def both_paths(gpu, queries, k):
 @pytest.mark.parametrize("metric", [rx.L2, rx.IP, rx.COS])
 @pytest.mark.parametrize("n,dim,nq,k", [(20000, 128, 64, 10), (30000, 100, 100, 10), (12000, 768, 96, 10), (9000, 64, 300, 15),
                                         (5000, 200, 33, 1), (30000, 768, 400, 10), (40000, 256, 700, 5), (6000, 1000, 150, 10),
-                                        (60000, 128, 520, 40), (50000, 96, 200, 63), (80000, 64, 260, 100), (45000, 160, 130, 127)])
+                                        (60000, 128, 520, 40), (50000, 96, 200, 63), (80000, 64, 260, 100), (45000, 160, 130, 127),
+                                        (20000, 64, 32, 10)])  # the last one: a query block of 32 (wgmma N = 32)
 def test_tc_path_is_bit_identical_to_exact_scan(metric, n, dim, nq, k):
     gpu = rx.GpuBruteforceSearch(metric, dim, n)
     gpu.append_synth(0xABC0 + dim, 0, n)
@@ -35,20 +36,15 @@ def test_tc_path_is_bit_identical_to_exact_scan(metric, n, dim, nq, k):
     assert (l0 == l1).all(), np.argwhere(l0 != l1)[:5]
     assert (d0.view(np.uint32) == d1.view(np.uint32)).all()
     assert st["tc_fallbacks"] == 0 and 0 < st["tc_candidates"] < nq * 4096, st
-    # every kernel variant gives the same bits: 3 / 4 = queries in shared memory (1 CTA / CTA pair with TMA multicast),
-    # 5 / 6 / 9 = whole query block in TMEM (accumulators of 64 rows; the default) with single CTAs / clusters of up to 4 / 8 CTAs,
-    # 14 / 15 / 16 = CTA pairs multiply as one (cta_group::2, half a 128-row tile per SM) with clusters of up to 4 / 2 / 8 CTAs
-    # 17 = the default kernel without the tail grid (the 2-CTA clusters that scan the last row tiles on the SMs a cluster-of-4 grid strands)
-    for mode, kernel in ((3, 1), (4, 1), (5, 2), (6, 2), (9, 2), (14, 5), (15, 5), (16, 5), (17, 2)):
+    # every cluster shape gives the same bits: 3 = single CTAs, 4 = clusters of up to two CTAs sharing every row tile (TMA multicast)
+    for mode in (3, 4):
         gpu.set_tensor_core_filter(mode)
         d2, l2, c2 = gpu.search_knn(queries, k)
         s2 = rx.last_search_stats()
-        if dim <= 768:
-            assert s2["tc_kernel"] == kernel, (mode, s2)
+        assert s2["tc_kernel"] == 1 and s2["tc_cluster"] == (2 if mode == 4 and nq > 128 else 1), (mode, s2)
         assert (l2 == l0).all() and (d2.view(np.uint32) == d0.view(np.uint32)).all(), mode
-    assert st["tc_kernel"] == (2 if dim <= 768 else 1)
-    if nq > 128 and dim <= 768:
-        assert st["tc_cluster"] == (4 if nq > 256 else 2)  # default: clusters of up to four CTAs share every row tile
+    assert st["tc_kernel"] == 1
+    assert st["tc_cluster"] == 1, st  # default: single CTAs
 
 
 def test_tc_path_matches_oracle():
