@@ -332,11 +332,14 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	}
 	const uint32_t pitchBf = ix->pitch_bf, kchunks = pitchBf / kTcChunkK;
 	const uint32_t nqb = tcQueryBlock(nq, kchunks);
-	const uint32_t nblocks = (nq + nqb - 1) / nqb;
-	// single CTAs by default: measured on an H100 at config 1, 10.5 k queries/s against 8.1 k with clusters of two and 4.4 k with clusters
-	// of four -- a multicast stage waits for the slowest consumer of the cluster, which costs more than the shared L2 reads save
+	const uint32_t ntiles = uint32_t((ix->size + kTcTileRows - 1) / kTcTileRows);
+	// single CTAs by default: measured on an H100 80GB HBM3 (700 W limit) at config 1, 25.0 k queries/s against 8.2 k with clusters of
+	// two -- a multicast stage waits for the slowest consumer of the cluster, while CTAs that share row tiles through L2 never wait
 	const uint32_t clusterMax = ix->tc_cluster_max ? ix->tc_cluster_max : 1u;
-	const uint32_t nqPad = nblocks * nqb;
+	// a cluster of two owns two consecutive query blocks; an odd block count is padded with a block of no valid queries
+	const uint32_t cluster = clusterMax >= 2 && nq > nqb && ntiles >= 2 ? 2u : 1u;
+	const uint32_t ngroups = ((nq + nqb - 1) / nqb + cluster - 1) / cluster;
+	const uint32_t nqPad = ngroups * cluster * nqb;
 	RX_CUDA(ws.d_qbf.ensure(size_t(nqPad) * pitchBf));
 	RX_CUDA(ws.d_qnorm.ensure(nqPad));
 	RX_CUDA(ws.d_tau.ensure(nqPad));
@@ -355,57 +358,55 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	RX_CUDA(cudaMemsetAsync(ws.d_cand_count.p, 0, size_t(nqPad) * 4, st));
 	RX_CUDA(cudaGetLastError());
 	g_stats.launches += 2;
-	const uint32_t ntiles = uint32_t((ix->size + kTcTileRows - 1) / kTcTileRows);
 	CUtensorMap mapQ;
 	if (int rc = makeBf16Map(&mapQ, ws.d_qbf.p, pitchBf, nqPad, uint64_t(pitchBf) * 2, nqb)) {
 		return rc;
 	}
-	const size_t smem = tc_smem_bytes(nqb, kchunks);
-	// A cluster of C CTAs owns C consecutive query blocks and reads every row tile from HBM once for all of them (TMA multicast); a
-	// leftover single block runs alone.
-	uint32_t clusterUsed = 1;
-	for (uint32_t b = 0; b < nblocks;) {
-		uint32_t cluster = 1;
-		while (cluster < std::min(clusterMax, nblocks - b) && ntiles >= 2) {
-			cluster *= 2;
-		}
-		const TcKernel kfn = tcKernel(nqb, cluster);
-		RX_CUDA(raiseSmemCeilingOnce(kfn, ix->device, int(kTcSmemLimit)));
-		cudaLaunchConfig_t cfg{};
-		cfg.gridDim = dim3(unsigned(ix->sm_count) / cluster * cluster);
-		cfg.blockDim = dim3(kTcThreads);
-		cfg.dynamicSmemBytes = smem;
-		cfg.stream = st;
-		cudaLaunchAttribute attr[1];
-		attr[0].id = cudaLaunchAttributeClusterDimension;
-		attr[0].val.clusterDim.x = cluster;
-		attr[0].val.clusterDim.y = 1;
-		attr[0].val.clusterDim.z = 1;
-		cfg.attrs = attr;
-		cfg.numAttrs = 1;
-		int resident = 0;  // GPC boundaries can strand SMs for clusters: ask how many fit at once
-		RX_CUDA(cudaOccupancyMaxActiveClusters(&resident, kfn, &cfg));
-		if (resident < 1) {
-			return fail(RXGPU_ERR_SYSTEM, "rxgpu: tensor-core filter kernel cannot be made resident");
-		}
-		cfg.gridDim = dim3(unsigned(std::min<uint64_t>(uint64_t(resident), ntiles)) * cluster);
-		TcArgs a{};
-		a.shadow = static_cast<const unsigned char*>(ix->d_shadow);
-		a.vw = ix->d_vw;
-		a.qnorm = ws.d_qnorm.p;
-		a.tau = ws.d_tau.p;
-		a.ub_list = ws.d_ub_list.p;
-		a.ub_lock = ws.d_ub_lock.p;
-		a.init_rows = uint32_t(std::min<uint64_t>(ix->size, kTcInitRows));
-		a.cand_rows = ws.d_cand_rows.p;
-		a.cand_count = ws.d_cand_count.p;
-		a.cand_cap = kTcCandCap;
-		a.n = uint32_t(ix->size);
-		a.kchunks = kchunks;
-		a.q0 = b * nqb;
-		a.nq_total = nq;
-		a.k1 = k1;
-		a.metric = ix->metric;
+	const TcKernel kfn = tcKernel(nqb, cluster);
+	RX_CUDA(raiseSmemCeilingOnce(kfn, ix->device, int(kTcSmemLimit)));
+	cudaLaunchConfig_t cfg{};
+	cfg.gridDim = dim3(unsigned(ix->sm_count) / cluster * cluster);
+	cfg.blockDim = dim3(kTcThreads);
+	cfg.dynamicSmemBytes = tc_smem_bytes(nqb, kchunks);
+	cfg.stream = st;
+	cudaLaunchAttribute attr[1];
+	attr[0].id = cudaLaunchAttributeClusterDimension;
+	attr[0].val.clusterDim.x = cluster;
+	attr[0].val.clusterDim.y = 1;
+	attr[0].val.clusterDim.z = 1;
+	cfg.attrs = attr;
+	cfg.numAttrs = 1;
+	int resident = 0;  // GPC boundaries can strand SMs for clusters: ask how many fit at once
+	RX_CUDA(cudaOccupancyMaxActiveClusters(&resident, kfn, &cfg));
+	if (resident < 1) {
+		return fail(RXGPU_ERR_SYSTEM, "rxgpu: tensor-core filter kernel cannot be made resident");
+	}
+	TcArgs a{};
+	a.shadow = static_cast<const unsigned char*>(ix->d_shadow);
+	a.vw = ix->d_vw;
+	a.qnorm = ws.d_qnorm.p;
+	a.tau = ws.d_tau.p;
+	a.ub_list = ws.d_ub_list.p;
+	a.ub_lock = ws.d_ub_lock.p;
+	a.init_rows = uint32_t(std::min<uint64_t>(ix->size, kTcInitRows));
+	a.cand_rows = ws.d_cand_rows.p;
+	a.cand_count = ws.d_cand_count.p;
+	a.cand_cap = kTcCandCap;
+	a.n = uint32_t(ix->size);
+	a.kchunks = kchunks;
+	a.nq_total = nq;
+	a.k1 = k1;
+	a.metric = ix->metric;
+	// One launch serves G = min(groups left, resident) query groups with W = resident / G tile walkers each, so the G clusters of a
+	// walker read every row tile from HBM about once and from L2 otherwise (config 1: 11 blocks x 12 walkers = 132 CTAs, the shadow
+	// streamed once per batch instead of once per block).  The grid never exceeds what is resident at once: a second wave would put
+	// the clusters of one walker far apart in time and lose the L2 reuse.  Larger batches take several such launches.
+	for (uint32_t g0 = 0; g0 < ngroups;) {
+		const uint32_t groups = std::min<uint32_t>(ngroups - g0, uint32_t(resident));
+		const uint32_t walkers = uint32_t(std::min<uint64_t>(uint32_t(resident) / groups, ntiles));
+		cfg.gridDim = dim3(groups * walkers * cluster);
+		a.q0 = g0 * cluster * nqb;
+		a.groups = groups;
 		cudaEvent_t e0 = nullptr, e1 = nullptr;
 		if (g_profile.load(std::memory_order_relaxed)) {
 			RX_CUDA(cudaEventCreate(&e0));
@@ -420,14 +421,13 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 		}
 		g_stats.launches += 1;
 		g_stats.passes += 1;
-		const uint32_t served = std::min(nqb * cluster, nq - b * nqb);  // queries of this launch, padding excluded
+		const uint32_t served = std::min(groups * cluster * nqb, nq - a.q0);  // queries of this launch, padding excluded
 		g_stats.algorithmic_bytes += uint64_t(ix->size) * pitchBf * 2 + uint64_t(ix->size) * 8 + uint64_t(served) * pitchBf * 2;
-		clusterUsed = std::max(clusterUsed, cluster);
-		b += cluster;
+		g0 += groups;
 	}
-	g_stats.tc_cluster = clusterUsed;
+	g_stats.tc_cluster = cluster;
 	g_stats.tc_kernel = 1;
-	g_stats.query_tile = nqb * clusterUsed;
+	g_stats.query_tile = nqb * cluster;
 	// exact re-rank of the candidates with the arithmetic of knn_scan_warp, then decode + labels
 	const size_t rsmem = size_t((ix->dim + 127) / 128) * 512 + size_t(kScanWarps) * (k1 + kCandBuf) * 8;
 	const float* norms = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;

@@ -14,12 +14,17 @@
 //                 upper bound of the final k1-th best TRUE distance; a row is a candidate iff lb <= tau_q.  tau starts from an
 //                 exact scan of the first rows (tc_init_tau) and only decreases.
 //
+// Launch shape: one grid covers G query groups (a group = one query block of NQ queries per CTA of a cluster) with W tile walkers
+// each, G x W <= the clusters resident at once (config 1: 11 blocks x 12 walkers = 132 CTAs, one launch per batch).  Walker w visits
+// the 128-row tiles w, w + W, w + 2W, ..., so every tile is visited once per query, and the G CTAs of one walker request the same
+// tiles at about the same time: the first read misses to HBM, the others hit L2, and nothing makes one CTA wait for another.
+//
 // Roles (384 threads = three warpgroups, 1 CTA per SM, persistent over 128-row tiles):
 //   warp 0       producer: the query block (NQ x dim bf16) once by TMA, then the bf16 shadow rows, 128 rows x 64 K (16 KB) per stage
 //                through a 4-stage mbarrier ring.  The shadow is stored TILED and PRE-SWIZZLED in HBM ([tile of 64 rows][K chunk]
 //                [64 x 128 B in the SWIZZLE_128B pattern]) so a stage is two contiguous 8 KB cp.async.bulk copies (row-major fp32
 //                stays the source of truth; the shadow is private, derived).  In a cluster of two CTAs (optional; single CTAs are
-//                faster on the H100) each CTA fetches half of every stage and multicasts it to both: one pass serves two query blocks.
+//                faster on the H100) each CTA fetches half of every stage and multicasts it to both, which own consecutive query blocks.
 //   warpgroups 1, 2   consumers: warpgroup w multiplies rows [64 w, 64 w + 64) of every tile with the whole query block
 //                (wgmma.m64nNQk16, both operands from shared memory, fp32 accumulators in registers), releases each stage as soon
 //                as its MMAs retired, then applies the metric to its 64 x NQ scores, tests them against tau, appends candidates to
@@ -58,7 +63,8 @@ struct TcArgs {
 	uint32_t n;                // rows
 	uint32_t kchunks;          // padded dim / 64
 	uint32_t nq_total;         // queries in the whole batch
-	uint32_t q0;               // first query of this launch; CTA rank r of a cluster owns queries [q0 + r*NQ, +NQ)
+	uint32_t q0;               // first query of this launch
+	uint32_t groups;           // G: query groups of this launch (a group = one query block per CTA of a cluster)
 	uint32_t k1;
 	int metric;                // kL2 / kIP / kCos
 };
@@ -332,8 +338,10 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 	const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;  // provably warp-uniform
 	const uint32_t ntiles = (a.n + kTcTileRows - 1) / kTcTileRows;
 	const uint32_t crank = kCluster > 1 ? cluster_ctarank() : 0u;
-	const uint32_t cid = blockIdx.x / kCluster, ncl = gridDim.x / kCluster;  // tile walkers
-	const uint32_t q0 = a.q0 + crank * kNq;
+	// launch shape (header comment): cluster cid serves query group cid % G as walker cid / G of W = ncl / G
+	const uint32_t cid = blockIdx.x / kCluster, ncl = gridDim.x / kCluster;
+	const uint32_t walker = cid / a.groups, walkers = ncl / a.groups;
+	const uint32_t q0 = a.q0 + ((cid % a.groups) * kCluster + crank) * kNq;
 	const uint32_t nq_valid = q0 < a.nq_total ? min(uint32_t(kNq), a.nq_total - q0) : 0u;
 
 	if (threadIdx.x == 0) {
@@ -367,7 +375,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		}
 		__syncwarp();
 		uint32_t stage = 0, phase = 0;
-		for (uint32_t t = cid; t < ntiles; t += ncl) {
+		for (uint32_t t = walker; t < ntiles; t += walkers) {
 			for (uint32_t kc = 0; kc < a.kchunks; ++kc) {
 				mbar_wait(&empty_bar[stage], phase ^ 1);
 				// a 128-row stage = the 64-row shadow blocks 2t and 2t+1 of this K chunk, 8 KB each, kchunks * 8 KB apart in HBM
@@ -412,7 +420,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		};
 		mbar_wait(q_bar, 0);
 		uint32_t stage = 0, phase = 0;
-		for (uint32_t t = cid; t < ntiles; t += ncl) {
+		for (uint32_t t = walker; t < ntiles; t += walkers) {
 			// refresh tau from the other CTAs: the global load was issued during the PREVIOUS tile, so its latency is hidden
 			if (my_q < nq_valid) {
 				const float tn = ord_float(tau_ahead);
