@@ -476,7 +476,8 @@ typedef struct {
 	uint32_t tc_kernel;         /* 1 = knn_tc_filter (wgmma, queries in shared memory) */
 } rxgpu_search_stats;
 void rxgpu_last_search_stats(rxgpu_search_stats* out);
-/* large query batches: bf16 tensor-core filter + exact fp32 re-rank (results identical to the exact scan).
+/* large query batches: int8 tensor-core filter (exact integer dot products of per-row scaled codes, certified by per-row
+ * residual norms) + exact fp32 re-rank (results identical to the exact scan).
  * mode 0 = automatic (batches >= 64 queries on >= 100k rows, k <= 127), 1 = whenever possible, 2 = never;
  * 3 / 4 = as 1 with single CTAs (the default) / clusters of up to two CTAs sharing every row tile; all give the same bits. */
 int rxgpu_set_tensor_core_filter(rxgpu_index*, int mode);

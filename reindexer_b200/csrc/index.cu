@@ -222,12 +222,13 @@ EncodeTiledFn encodeTiled() {  // libcuda is never linked: resolve the one drive
 	}();
 	return fn;
 }
-int makeBf16Map(CUtensorMap* m, void* base, uint64_t cols, uint64_t rows, uint64_t pitchBytes, uint32_t boxRows) {
-	const cuuint64_t gdim[2] = {cols, rows};
+// int8 query codes [rows][pitchBytes]: boxes of 128 bytes x boxRows, written to shared memory in the SWIZZLE_128B pattern
+int makeCodeMap(CUtensorMap* m, void* base, uint64_t pitchBytes, uint64_t rows, uint32_t boxRows) {
+	const cuuint64_t gdim[2] = {pitchBytes, rows};
 	const cuuint64_t gstr[1] = {pitchBytes};
 	const cuuint32_t box[2] = {uint32_t(kTcChunkK), boxRows};
 	const cuuint32_t estr[2] = {1, 1};
-	const CUresult r = encodeTiled()(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+	const CUresult r = encodeTiled()(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, base, gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
 									  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 	if (r != CUDA_SUCCESS) {
 		return fail(RXGPU_ERR_SYSTEM, "rxgpu: cuTensorMapEncodeTiled failed (" + std::to_string(int(r)) + ")");
@@ -236,7 +237,10 @@ int makeBf16Map(CUtensorMap* m, void* base, uint64_t cols, uint64_t rows, uint64
 }
 
 constexpr size_t kTcSmemLimit = 227 * 1024;  // the per-block opt-in maximum of sm_90
-constexpr uint32_t kTcCandCap = 4096;
+// per-query candidate list entries: the rows within the bound's window of the k1-th distance grow about in proportion to k1
+// (config 1, int8 filter, candidates per query: k = 10: 1 620, k = 30: 3 820, k = 63: 6 880, k = 127: 12 000); 4096 is also the floor, so masses of near-duplicates still overflow to the
+// exact scan instead of being re-ranked one list entry at a time
+uint32_t tcCandCap(uint32_t k1) { return std::max<uint32_t>(4096u, 256u * k1); }
 
 // knn_tc_filter<query block, cluster size>: one instantiation per wgmma N and per cluster shape
 using TcKernel = void (*)(const CUtensorMap, const TcArgs);
@@ -267,24 +271,22 @@ bool tcEligible(const rxgpu_index* ix, uint32_t nq, uint32_t k1, int mode) {
 	if (tcQueryBlock(nq, (ix->dim + kTcChunkK - 1) / kTcChunkK) == 0) {
 		return false;
 	}
-	// the error coefficient kTcErrCoef = 0.0042 certifies |q~.v~ - q.v| <= c ||q|| ||v|| only while
-	// 2^-8 + 2^-18 + dim * 2^-23 <= 0.0042 (two bf16 roundings + fp32 accumulation): dim <= 2400; beyond 2048 dims the exact scan answers
+	// the s32 accumulator holds the exact code dot product while dim * 127^2 < 2^31; beyond 2048 dims the exact scan answers
 	if (ix->dim > 2048) {
 		return false;
 	}
 	return ix->tc_mode == 1 || (nq >= 64 && ix->size >= 100000);
 }
 
-// bf16 shadow + row norms, rebuilt when the rows changed since the last large-batch search (10M x 768: ~7 ms)
+// int8 shadow + per-row constants, brought up to date when the rows changed since the last large-batch search
 int ensureShadow(const rxgpu_index* ix, cudaStream_t st) {
 	std::lock_guard<std::mutex> lck(ix->tc_mtx);
-	const uint32_t pitchBf = (ix->dim + kTcChunkK - 1) / kTcChunkK * kTcChunkK;
+	const uint32_t pitchQ = (ix->dim + kTcChunkK - 1) / kTcChunkK * kTcChunkK;
 	if (!ix->d_shadow) {
 		const size_t cap = (size_t(ix->capacity ? ix->capacity : 1) + kTcTileRows - 1) / kTcTileRows * kTcTileRows;  // whole tiles
-		RX_CUDA(cudaMalloc(&ix->d_shadow, cap * pitchBf * 2));
-		RX_CUDA(cudaMalloc(reinterpret_cast<void**>(&ix->d_vnorm), cap * sizeof(float)));
-		RX_CUDA(cudaMalloc(reinterpret_cast<void**>(&ix->d_vw), cap * sizeof(float2)));
-		ix->pitch_bf = pitchBf;
+		RX_CUDA(cudaMalloc(&ix->d_shadow, cap * pitchQ));
+		RX_CUDA(cudaMalloc(reinterpret_cast<void**>(&ix->d_rowc), cap * sizeof(float4)));
+		ix->pitch_q = pitchQ;
 		ix->shadow_version = ~0ull;
 		ix->shadow_dirty_all = true;
 		ix->shadow_dirty.clear();
@@ -293,8 +295,8 @@ int ensureShadow(const rxgpu_index* ix, cudaStream_t st) {
 		// only the rows the mutations since the last search rewrote (an upsert, a swap-remove, an appended run), unless the log gave up
 		auto convert = [&](uint32_t b, uint32_t e) {
 			const unsigned blocks = unsigned((uint64_t(e - b) * 32 + 255) / 256);
-			tc_convert_rows<<<blocks, 256, 0, st>>>(ix->d_rows, ix->pitch, ix->dim, b, e, static_cast<__nv_bfloat16*>(ix->d_shadow),
-													pitchBf / kTcChunkK, ix->d_vnorm);
+			tc_convert_rows<<<blocks, 256, 0, st>>>(ix->d_rows, ix->pitch, ix->dim, b, e, static_cast<unsigned char*>(ix->d_shadow),
+													pitchQ / kTcChunkK, ix->metric == RXGPU_COS ? ix->d_norms : nullptr, ix->d_rowc);
 		};
 		if (ix->shadow_dirty_all) {
 			if (ix->size) {
@@ -310,8 +312,9 @@ int ensureShadow(const rxgpu_index* ix, cudaStream_t st) {
 		}
 		ix->shadow_dirty_all = false;
 		ix->shadow_dirty.clear();
-		const uint32_t padded = uint32_t((ix->size + kTcTileRows - 1) / kTcTileRows * kTcTileRows);
-		tc_make_vw<<<(padded + 255) / 256, 256, 0, st>>>(ix->d_vnorm, uint32_t(ix->size), padded, ix->metric, ix->d_vw);
+		// rows past the end, up to whole tiles, have all-zero constants (their codes are never tested: the kernel masks rows >= n)
+		const uint64_t padded = (ix->size + kTcTileRows - 1) / kTcTileRows * kTcTileRows;
+		RX_CUDA(cudaMemsetAsync(ix->d_rowc + ix->size, 0, size_t(padded - ix->size) * sizeof(float4), st));
 		RX_CUDA(cudaGetLastError());
 		RX_CUDA(cudaStreamSynchronize(st));
 		ix->shadow_version = ix->version;
@@ -323,34 +326,34 @@ int ensureShadow(const rxgpu_index* ix, cudaStream_t st) {
 int scanTopKExact(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1, int mode,
 				  float bound, float* d_out_dist, uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count);
 
-// Large batches: approximate bf16 tensor-core scores with a certified error bound select the candidates, the exact fp32 routine
+// Large batches: approximate int8 tensor-core scores with a certified error bound select the candidates, the exact fp32 routine
 // re-ranks them.  Output = the same top-k1 under (dist, internal index) as scanTopKExact, bit for bit.
 int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1,
 					   float* d_out_dist, uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count) {
 	if (int rc = ensureShadow(ix, st)) {
 		return rc;
 	}
-	const uint32_t pitchBf = ix->pitch_bf, kchunks = pitchBf / kTcChunkK;
+	const uint32_t pitchQ = ix->pitch_q, kchunks = pitchQ / kTcChunkK;
 	const uint32_t nqb = tcQueryBlock(nq, kchunks);
 	const uint32_t ntiles = uint32_t((ix->size + kTcTileRows - 1) / kTcTileRows);
-	// single CTAs by default: measured on an H100 80GB HBM3 (700 W limit) at config 1, 25.0 k queries/s against 8.2 k with clusters of
+	// single CTAs by default: measured on an H100 80GB HBM3 (400 W limit) at config 1, 34.8 k queries/s against 19.9 k with clusters of
 	// two -- a multicast stage waits for the slowest consumer of the cluster, while CTAs that share row tiles through L2 never wait
 	const uint32_t clusterMax = ix->tc_cluster_max ? ix->tc_cluster_max : 1u;
 	// a cluster of two owns two consecutive query blocks; an odd block count is padded with a block of no valid queries
 	const uint32_t cluster = clusterMax >= 2 && nq > nqb && ntiles >= 2 ? 2u : 1u;
 	const uint32_t ngroups = ((nq + nqb - 1) / nqb + cluster - 1) / cluster;
 	const uint32_t nqPad = ngroups * cluster * nqb;
-	RX_CUDA(ws.d_qbf.ensure(size_t(nqPad) * pitchBf));
-	RX_CUDA(ws.d_qnorm.ensure(nqPad));
+	RX_CUDA(ws.d_qcodes.ensure(size_t(nqPad) * pitchQ));
+	RX_CUDA(ws.d_qc.ensure(nqPad));
 	RX_CUDA(ws.d_tau.ensure(nqPad));
 	RX_CUDA(ws.d_ub_list.ensure(size_t(nqPad) * kTcMaxK1));
 	RX_CUDA(ws.d_ub_lock.ensure(nqPad));
 	RX_CUDA(ws.d_cand_count.ensure(nqPad));
-	RX_CUDA(ws.d_cand_rows.ensure(size_t(nqPad) * kTcCandCap));
+	const uint32_t candCap = tcCandCap(k1);
+	RX_CUDA(ws.d_cand_rows.ensure(size_t(nqPad) * candCap));
 	RX_CUDA(ws.h_cand_count.ensure(nqPad));
 	RX_CUDA(ws.d_lists.ensure(size_t(nq) * k1));
-	tc_prepare_queries<<<(nqPad * 32 + 255) / 256, 256, 0, st>>>(d_queries, nq, nqPad, ix->dim, pitchBf,
-																 reinterpret_cast<__nv_bfloat16*>(ws.d_qbf.p), ws.d_qnorm.p);
+	tc_prepare_queries<<<(nqPad * 32 + 255) / 256, 256, 0, st>>>(d_queries, nq, nqPad, ix->dim, pitchQ, ws.d_qcodes.p, ws.d_qc.p);
 	RX_CUDA(raiseSmemCeilingOnce(tc_init_tau, ix->device, int(tc_init_smem_bytes(2048))));
 	tc_init_tau<<<(nq + kTcInitQ - 1) / kTcInitQ, 256, tc_init_smem_bytes(ix->pitch), st>>>(
 		ix->d_rows, ix->pitch, ix->dim, ix->metric == RXGPU_COS ? ix->d_norms : nullptr, uint32_t(std::min<uint64_t>(ix->size, kTcInitRows)),
@@ -359,7 +362,7 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	RX_CUDA(cudaGetLastError());
 	g_stats.launches += 2;
 	CUtensorMap mapQ;
-	if (int rc = makeBf16Map(&mapQ, ws.d_qbf.p, pitchBf, nqPad, uint64_t(pitchBf) * 2, nqb)) {
+	if (int rc = makeCodeMap(&mapQ, ws.d_qcodes.p, pitchQ, nqPad, nqb)) {
 		return rc;
 	}
 	const TcKernel kfn = tcKernel(nqb, cluster);
@@ -383,22 +386,23 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	}
 	TcArgs a{};
 	a.shadow = static_cast<const unsigned char*>(ix->d_shadow);
-	a.vw = ix->d_vw;
-	a.qnorm = ws.d_qnorm.p;
+	a.rowc = ix->d_rowc;
+	a.qc = ws.d_qc.p;
 	a.tau = ws.d_tau.p;
 	a.ub_list = ws.d_ub_list.p;
 	a.ub_lock = ws.d_ub_lock.p;
 	a.init_rows = uint32_t(std::min<uint64_t>(ix->size, kTcInitRows));
 	a.cand_rows = ws.d_cand_rows.p;
 	a.cand_count = ws.d_cand_count.p;
-	a.cand_cap = kTcCandCap;
+	a.cand_cap = candCap;
 	a.n = uint32_t(ix->size);
+	a.dim = ix->dim;
 	a.kchunks = kchunks;
 	a.nq_total = nq;
 	a.k1 = k1;
 	a.metric = ix->metric;
 	// One launch serves G = min(groups left, resident) query groups with W = resident / G tile walkers each, so the G clusters of a
-	// walker read every row tile from HBM about once and from L2 otherwise (config 1: 11 blocks x 12 walkers = 132 CTAs, the shadow
+	// walker read every row tile from HBM about once and from L2 otherwise (config 1: 8 blocks x 16 walkers = 128 CTAs, the shadow
 	// streamed once per batch instead of once per block).  The grid never exceeds what is resident at once: a second wave would put
 	// the clusters of one walker far apart in time and lose the L2 reuse.  Larger batches take several such launches.
 	for (uint32_t g0 = 0; g0 < ngroups;) {
@@ -422,7 +426,7 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 		g_stats.launches += 1;
 		g_stats.passes += 1;
 		const uint32_t served = std::min(groups * cluster * nqb, nq - a.q0);  // queries of this launch, padding excluded
-		g_stats.algorithmic_bytes += uint64_t(ix->size) * pitchBf * 2 + uint64_t(ix->size) * 8 + uint64_t(served) * pitchBf * 2;
+		g_stats.algorithmic_bytes += uint64_t(ix->size) * pitchQ + uint64_t(ix->size) * sizeof(float4) + uint64_t(served) * pitchQ;
 		g0 += groups;
 	}
 	g_stats.tc_cluster = cluster;
@@ -434,11 +438,11 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	if (ix->metric == RXGPU_L2) {
 		RX_CUDA(raiseSmemCeilingOnce(knn_rerank<true>, ix->device, kScanSmemBudget));
 		knn_rerank<true><<<nq, kScanThreads, rsmem, st>>>(ix->d_rows, ix->pitch, ix->dim, norms, d_queries, ws.d_cand_rows.p,
-														   ws.d_cand_count.p, kTcCandCap, k1, ws.d_lists.p);
+														   ws.d_cand_count.p, candCap, k1, ws.d_lists.p);
 	} else {
 		RX_CUDA(raiseSmemCeilingOnce(knn_rerank<false>, ix->device, kScanSmemBudget));
 		knn_rerank<false><<<nq, kScanThreads, rsmem, st>>>(ix->d_rows, ix->pitch, ix->dim, norms, d_queries, ws.d_cand_rows.p,
-															ws.d_cand_count.p, kTcCandCap, k1, ws.d_lists.p);
+															ws.d_cand_count.p, candCap, k1, ws.d_lists.p);
 	}
 	MergeArgs m{};
 	m.lists = ws.d_lists.p;
@@ -462,8 +466,8 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	RX_CUDA(cudaStreamSynchronize(st));
 	uint64_t cands = 0;
 	for (uint32_t q = 0; q < nq; ++q) {
-		cands += std::min<unsigned>(ws.h_cand_count.p[q], kTcCandCap);
-		if (ws.h_cand_count.p[q] > kTcCandCap) {
+		cands += std::min<unsigned>(ws.h_cand_count.p[q], candCap);
+		if (ws.h_cand_count.p[q] > candCap) {
 			g_stats.tc_fallbacks += 1;
 			if (int rc = scanTopKExact(ix, ws, st, d_queries + size_t(q) * ix->dim, 1, k1, kModeTopK, 0.f, d_out_dist + size_t(q) * k1,
 									   d_out_idx + size_t(q) * k1, d_out_label ? d_out_label + size_t(q) * k1 : nullptr, d_out_count + q)) {
@@ -473,6 +477,7 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	}
 	ws.tc_lists_valid = true;
 	ws.tc_lists_nq = nq;
+	ws.tc_lists_cap = candCap;
 	ws.tc_lists_version = ix->version;
 	g_stats.tc_used = 1;
 	g_stats.tc_candidates = cands;
@@ -537,7 +542,7 @@ int tieRowsAfterScan(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, cons
 	}
 	bool fromLists = ws.tc_lists_valid && ws.tc_lists_version == ix->version && k <= kTcMaxK1;
 	for (uint32_t i = 0; fromLists && i < nsel; ++i) {  // a query whose list overflowed was answered by the exact scan: no list
-		fromLists = sel[i] < ws.tc_lists_nq && ws.h_cand_count.p[sel[i]] <= kTcCandCap;
+		fromLists = sel[i] < ws.tc_lists_nq && ws.h_cand_count.p[sel[i]] <= ws.tc_lists_cap;
 	}
 	if (!fromLists) {
 		for (uint32_t i = 0; i < nsel; ++i) {
@@ -559,11 +564,11 @@ int tieRowsAfterScan(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, cons
 	if (ix->metric == RXGPU_L2) {
 		RX_CUDA(raiseSmemCeilingOnce(knn_rerank<true>, ix->device, kScanSmemBudget));
 		knn_rerank<true><<<nsel, kScanThreads, rsmem, st>>>(ix->d_rows, ix->pitch, ix->dim, norms, d_queries, ws.d_cand_rows.p, ws.d_cand_count.p,
-															 kTcCandCap, k, ws.d_lists.p, ws.d_sel.p, ws.d_selbound.p);
+															 ws.tc_lists_cap, k, ws.d_lists.p, ws.d_sel.p, ws.d_selbound.p);
 	} else {
 		RX_CUDA(raiseSmemCeilingOnce(knn_rerank<false>, ix->device, kScanSmemBudget));
 		knn_rerank<false><<<nsel, kScanThreads, rsmem, st>>>(ix->d_rows, ix->pitch, ix->dim, norms, d_queries, ws.d_cand_rows.p, ws.d_cand_count.p,
-															  kTcCandCap, k, ws.d_lists.p, ws.d_sel.p, ws.d_selbound.p);
+															  ws.tc_lists_cap, k, ws.d_lists.p, ws.d_sel.p, ws.d_selbound.p);
 	}
 	MergeArgs m{};
 	m.lists = ws.d_lists.p;
@@ -733,11 +738,9 @@ int rxgpu_index_resize(rxgpu_index* ix, uint64_t new_capacity) {
 	ix->capacity = new_capacity;
 	if (ix->d_shadow) {  // rebuilt lazily at the new capacity
 		cudaFree(ix->d_shadow);
-		cudaFree(ix->d_vnorm);
-		cudaFree(ix->d_vw);
-		ix->d_vw = nullptr;
+		cudaFree(ix->d_rowc);
 		ix->d_shadow = nullptr;
-		ix->d_vnorm = nullptr;
+		ix->d_rowc = nullptr;
 	}
 	try {
 		if (ix->flags & RXGPU_FLAG_HOST_MIRROR) {

@@ -132,8 +132,8 @@ struct Workspace {
 	DevBuf<uint32_t> d_out_count;
 	DevBuf<uint64_t> d_range;
 	DevBuf<unsigned long long> d_range_count;
-	DevBuf<uint16_t> d_qbf;  // bf16 query block for the tensor-core filter
-	DevBuf<float> d_qnorm;
+	DevBuf<unsigned char> d_qcodes;  // int8 query codes for the tensor-core filter
+	DevBuf<float4> d_qc;             // their per-query constants (s_q, r_q, ||q||, 1 / k_q)
 	DevBuf<unsigned int> d_tau, d_cand_count, d_ub_lock;
 	DevBuf<float> d_ub_list;
 	DevBuf<uint32_t> d_cand_rows;
@@ -148,6 +148,7 @@ struct Workspace {
 	// (d_cand_rows / h_cand_count) hold every row at or below each query's k1-th distance -- tieRowsAfterScan reads them
 	bool tc_lists_valid = false;
 	uint32_t tc_lists_nq = 0;
+	uint32_t tc_lists_cap = 0;  // entries per query list of that call
 	uint64_t tc_lists_version = 0;
 	DevBuf<uint32_t> d_sel;
 	DevBuf<float> d_selbound;
@@ -202,12 +203,11 @@ struct rxgpu_index {
 	rxgpu_ivf_device* ivf = nullptr;    // centroids + list boundaries attached by rxgpu_ivf_import
 	rxgpu_sq8_device* sq8 = nullptr;    // SQ8 codes + corrective offsets attached by rxgpu_sq8_attach (sq8.cu)
 
-	// tensor-core filter state, built lazily by the first large-batch search: bf16 shadow of the rows + row norms
+	// tensor-core filter state, built lazily by the first large-batch search: int8 shadow of the rows + per-row constants
 	mutable std::mutex tc_mtx;
-	mutable void* d_shadow = nullptr;  // __nv_bfloat16 [capacity][pitch_bf]
-	mutable float* d_vnorm = nullptr;  // [capacity] ||row||_2
-	mutable float2* d_vw = nullptr;    // [capacity] per-row (max(||row||, tiny), w) pairs the filter epilogue consumes, 512 B per 64-row tile
-	mutable uint32_t pitch_bf = 0;
+	mutable void* d_shadow = nullptr;  // int8 codes, [capacity / 64 blocks][pitch_q / 128 chunks][64 x 128 B], knn_tc.cuh
+	mutable float4* d_rowc = nullptr;  // [capacity] (scale, residual norm, norm, Cosine coefficient) of every row
+	mutable uint32_t pitch_q = 0;      // bytes of codes per row, dim rounded up to 128
 	mutable uint64_t shadow_version = ~0ull;
 	// rows rewritten since the shadow was last brought up to date (the mutations log them beside `version`): ensureShadow converts
 	// only these; the log gives up (full rebuild) beyond kShadowLogMax ranges
@@ -255,11 +255,8 @@ struct rxgpu_index {
 		if (d_shadow) {
 			cudaFree(d_shadow);
 		}
-		if (d_vnorm) {
-			cudaFree(d_vnorm);
-		}
-		if (d_vw) {
-			cudaFree(d_vw);
+		if (d_rowc) {
+			cudaFree(d_rowc);
 		}
 		if (stream) {
 			cudaStreamDestroy(stream);

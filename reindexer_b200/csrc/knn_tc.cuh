@@ -1,37 +1,50 @@
 // Tensor-core candidate filter for large query batches (sm_90a: TMA + wgmma + mbarrier, thread-block clusters), exact results.
 //
 // knn_scan_warp is HBM-bound only while <= ~16 queries share a pass; a batch of 1024 queries is FMA-bound there.  This kernel
-// computes APPROXIMATE scores for a block of NQ queries against every row with bf16 operands on the tensor cores and keeps, per
-// query, only the rows that can still be among the k best under a CERTIFIED error bound; the survivors (a few hundred per query)
+// computes APPROXIMATE scores for a block of NQ queries against every row with int8 operands on the tensor cores and keeps, per
+// query, only the rows that can still be among the k best under a CERTIFIED error bound; the survivors (~1 600 per query at config 1)
 // are then re-ranked with the exact fp32 routine of knn_scan_warp, so the final result is identical to the exact scan.
 //
-//   error bound   |q~.v~ - q.v| <= c * ||q|| * ||v||,  c = 2^-8 + 2^-18 (two bf16 roundings, unit roundoff 2^-9 each)
-//                                                        + dim * 2^-23 (fp32 accumulation in the MMA); c = 0.0042 leaves 5% slack
-//                                                        at 768 dims and 1% at 2048 dims, the largest dimension the filter accepts
-//   lower bound   lb = d~ - e, upper bound ub = d~ + e in map space (smaller is better)
+// Quantisation (tc_quantize, the same for rows and queries; fp32 vector v of dimension D):
+//   scale     s_v = max|v_i| / 127 (fp32; 0 for an all-zero row)      codes  c_v = round(v / s_v), clamped to +-127
+//   residual  rho_v = v - s_v c_v                                       r_v >= ||rho_v||, n_v >= ||v||  (fp64 sums, rounded up to fp32)
+// The dot product of the codes I = c_q.c_v is EXACT in the s32 wgmma accumulator (|I| <= 2048 * 127^2 < 2^31 for every dimension the
+// filter accepts), and with p = s_q s_v I
+//   q.v = p + s_q c_q.rho_v + rho_q.v    =>   |q.v - p| <= (n_q + r_q) r_v + r_q n_v
+// The exact scan's own fp32 sum differs from q.v by at most D 2^-23 n_q n_v; 16 more units of 2^-23 n_q n_v and a relative 2^-8
+// cover the rearranged fp32 arithmetic of the test below, so
+//   e(q, v) = (1 + 2^-8) ((n_q + r_q) r_v + (r_q + (D + 16) 2^-23 n_q) n_v)
+//   IP      d~ = -p,                  lb/ub = d~ -+ e
+//   Cosine  d~ = -p c_v,              lb/ub = d~ -+ e c_v              (c_v = the exact scan's own norm coefficient)
+//   L2      d~ = n_q^2 + n_v^2 - 2p,  lb/ub = d~ -+ (2e + eps (n_q^2 + n_v^2)),  eps = kTcL2Eps + (D + 1) 2^-23 (the exact scan's sum
+//                                                                                  of squares and the rounding of d~ itself)
+// For sigma = 0.25 rows at 768 dims r_v / n_v is about 0.7 %, so e is about 0.015 n_q n_v.
 //   threshold     tau_q = k1-th smallest ub over all DISTINCT rows seen so far by any CTA (one small list per query in HBM,
 //                 updated under a per-query lock -- only O(k log n) successful inserts per query over a whole pass) => a valid
 //                 upper bound of the final k1-th best TRUE distance; a row is a candidate iff lb <= tau_q.  tau starts from an
 //                 exact scan of the first rows (tc_init_tau) and only decreases.
 //
 // Launch shape: one grid covers G query groups (a group = one query block of NQ queries per CTA of a cluster) with W tile walkers
-// each, G x W <= the clusters resident at once (config 1: 11 blocks x 12 walkers = 132 CTAs, one launch per batch).  Walker w visits
+// each, G x W <= the clusters resident at once (config 1: 8 blocks x 16 walkers = 128 CTAs, one launch per batch).  Walker w visits
 // the 128-row tiles w, w + W, w + 2W, ..., so every tile is visited once per query, and the G CTAs of one walker request the same
 // tiles at about the same time: the first read misses to HBM, the others hit L2, and nothing makes one CTA wait for another.
 //
 // Roles (384 threads = three warpgroups, 1 CTA per SM, persistent over 128-row tiles):
-//   warp 0       producer: the query block (NQ x dim bf16) once by TMA, then the bf16 shadow rows, 128 rows x 64 K (16 KB) per stage
-//                through a 4-stage mbarrier ring.  The shadow is stored TILED and PRE-SWIZZLED in HBM ([tile of 64 rows][K chunk]
-//                [64 x 128 B in the SWIZZLE_128B pattern]) so a stage is two contiguous 8 KB cp.async.bulk copies (row-major fp32
-//                stays the source of truth; the shadow is private, derived).  In a cluster of two CTAs (optional; single CTAs are
-//                faster on the H100) each CTA fetches half of every stage and multicasts it to both, which own consecutive query blocks.
-//   warpgroups 1, 2   consumers: warpgroup w multiplies rows [64 w, 64 w + 64) of every tile with the whole query block
-//                (wgmma.m64nNQk16, both operands from shared memory, fp32 accumulators in registers), releases each stage as soon
-//                as its MMAs retired, then applies the metric to its 64 x NQ scores, tests them against tau, appends candidates to
-//                per-query lists in HBM and tightens tau.
+//   warps 0, 1   producers: warp 0 loads the query block (NQ x dim int8 codes) once by TMA; warp w then streams the 64-row shadow
+//                blocks 2t + w of the walker's tiles t, one K chunk (64 rows x 128 codes = 8 KB) per stage, through the RING OF
+//                consumer warpgroup w (kTcStages stages each).  The shadow is stored TILED and PRE-SWIZZLED in HBM ([64-row block]
+//                [K chunk][64 x 128 B in the SWIZZLE_128B pattern]) so a stage is one contiguous 8 KB cp.async.bulk copy (row-major
+//                fp32 stays the source of truth; the shadow is private, derived).  In a cluster of two CTAs (optional; single CTAs
+//                are faster on the H100) each CTA fetches half of every stage and multicasts it to both, which own consecutive
+//                query blocks.
+//   warpgroups 1, 2   consumers: warpgroup w multiplies its 64-row blocks with the whole query block (wgmma.m64nNQk32.s32.s8.s8,
+//                both operands from shared memory, exact int32 accumulators in registers), releases each stage as soon as its MMAs
+//                retired, then tests its 64 x NQ scores against tau, appends candidates to per-query lists in HBM and tightens
+//                tau.  The two rings are independent, so one warpgroup's epilogue overlaps the other's MMAs.
 #pragma once
 #include <cuda.h>
-#include <cuda_bf16.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 #include "knn_scan.cuh"
@@ -39,20 +52,19 @@
 namespace rxgpu {
 
 constexpr int kTcThreads = 384;
-constexpr int kTcTileRows = 128;     // two wgmma M = 64 halves, one per consumer warpgroup
-constexpr int kTcChunkK = 64;        // bf16 elements per 128-byte swizzle row
-constexpr int kTcStages = 4;
-constexpr int kTcBlockBytes = 64 * kTcChunkK * 2;           // 8 KB: one 64-row shadow block of one K chunk
-constexpr int kTcStageBytes = 2 * kTcBlockBytes;            // 16 KB
+constexpr int kTcTileRows = 128;     // two 64-row blocks (wgmma M = 64), one per consumer warpgroup
+constexpr int kTcChunkK = 128;       // int8 codes per 128-byte swizzle row
+constexpr int kTcStages = 6;         // stages per consumer warpgroup ring
+constexpr int kTcBlockBytes = 64 * kTcChunkK;               // 8 KB: one 64-row shadow block of one K chunk = one stage
 constexpr uint32_t kTcMaxNq = 128;   // queries per CTA (wgmma N <= 128 keeps the accumulators at <= 64 registers per thread)
-constexpr uint32_t kTcMaxK1 = 128;  // k + 1 <= 128: the bound list is scanned linearly under the per-query lock and ~25-35 (k + 1) candidates
-                                    // per query must fit the 4096-entry lists (k = 10: 330; k = 63: 1600; an overflowing query takes the exact scan)
-constexpr float kTcErrCoef = 0.0042f;  // see header comment
+constexpr uint32_t kTcMaxK1 = 128;  // k + 1 <= 128: the bound list is scanned linearly under the per-query lock
+constexpr float kTcL2Eps = 1e-5f;
 
 struct TcArgs {
-	const unsigned char* shadow;  // bf16 shadow, [tile of 64 rows][K chunk][64 rows x 128 B, SWIZZLE_128B pattern pre-applied]
-	const float2* vw;          // tc_make_vw: [rows padded to whole tiles] (max(||v||, tiny), w)
-	const float* qnorm;        // [nq_total] ||q||_2
+	const unsigned char* shadow;  // int8 codes, [64-row block][K chunk][64 rows x 128 B, SWIZZLE_128B pattern pre-applied]
+	const float4* rowc;        // [rows padded to whole tiles] (s_v, r_v, n_v, c_v): scale, residual norm, norm, Cosine coefficient
+								// (1 for IP / L2); zero beyond n
+	const float4* qc;          // [nq_total] (s_q, r_q, n_q, 1 / max(s_q, tiny)) of tc_prepare_queries
 	unsigned int* tau;         // [nq_total] ordered-uint of the current threshold (map space), shared by all CTAs
 	float* ub_list;            // [nq_total][kTcMaxK1] the k1 smallest upper bounds over ALL rows seen by any CTA (guarded by ub_lock)
 	unsigned int* ub_lock;     // [nq_total]
@@ -61,7 +73,8 @@ struct TcArgs {
 	unsigned int* cand_count;  // [nq_total]
 	uint32_t cand_cap;
 	uint32_t n;                // rows
-	uint32_t kchunks;          // padded dim / 64
+	uint32_t dim;
+	uint32_t kchunks;          // padded dim / 128
 	uint32_t nq_total;         // queries in the whole batch
 	uint32_t q0;               // first query of this launch
 	uint32_t groups;           // G: query groups of this launch (a group = one query block per CTA of a cluster)
@@ -69,10 +82,10 @@ struct TcArgs {
 	int metric;                // kL2 / kIP / kCos
 };
 
-// shared memory: query block, stage ring, barriers, then per consumer warpgroup the (P, R) pairs and thresholds of the block
+// shared memory: query block, two stage rings, barriers, per-query constants, then per consumer warpgroup thresholds and (P, R)
 __host__ __device__ inline size_t tc_smem_bytes(uint32_t nq_block, uint32_t kchunks) {
-	return 1024 /*align slack*/ + size_t(nq_block) * kchunks * 128 + size_t(kTcStages) * kTcStageBytes + 256 /*barriers*/ +
-		   size_t(nq_block) * (4 /*qe*/ + 2 * (4 + 8) /*thr, pr per warpgroup*/) + 64;
+	return 1024 /*align slack*/ + size_t(nq_block) * kchunks * 128 + size_t(2 * kTcStages) * kTcBlockBytes + 256 /*barriers*/ +
+		   size_t(nq_block) * (16 /*qc*/ + 2 * (4 + 8) /*thr, pr per warpgroup*/) + 64;
 }
 
 // ---- PTX wrappers -------------------------------------------------------------------------------------------------------------
@@ -146,7 +159,7 @@ __device__ __forceinline__ void cluster_sync_all() {
 	asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 // wgmma shared-memory matrix descriptor, K-major, SWIZZLE_128B: 8-row groups are 1024 B apart (SBO), one swizzle atom along K
-// (LBO unused); the K step of 16 bf16 inside the atom advances the start address by 32 bytes
+// (LBO unused); the K step of 32 int8 inside the atom advances the start address by 32 bytes
 __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
 	uint64_t d = 0;
 	d |= uint64_t((smem_addr & 0x3FFFFu) >> 4);  // start address, bits [0,14)
@@ -161,127 +174,131 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() {
 	asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// D[64 rows x N queries] (+)= A[64 x 16] (smem) x B[N x 16]^T (smem), bf16 in, fp32 accumulate; d = the thread's N / 2 accumulators
-__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+// D[64 rows x N queries] (+)= A[64 x 32] (smem) x B[N x 32]^T (smem), s8 in, exact s32 accumulate; d = the thread's N / 2 accumulators
+__device__ __forceinline__ void wgmma_m64n32k32(int (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
 	asm volatile(
 		"{\n"
 		".reg .pred p;\n"
 		"setp.ne.b32 p, %18, 0;\n"
-		"wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+		"wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
 		"{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, "
-		"%16, %17, p, 1, 1, 0, 0;\n"
+		"%16, %17, p;\n"
 		"}\n"
-		: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-		  "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]),
+		  "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
 		: "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_m64n64k32(int (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
 	asm volatile(
 		"{\n"
 		".reg .pred p;\n"
 		"setp.ne.b32 p, %34, 0;\n"
-		"wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+		"wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
 		"{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
 		"%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
-		"%32, %33, p, 1, 1, 0, 0;\n"
+		"%32, %33, p;\n"
 		"}\n"
-		: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-		  "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-		  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]),
+		  "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+		  "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
 		: "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void wgmma_m64n96k16(float (&d)[48], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_m64n96k32(int (&d)[48], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
 	asm volatile(
 		"{\n"
 		".reg .pred p;\n"
 		"setp.ne.b32 p, %50, 0;\n"
-		"wgmma.mma_async.sync.aligned.m64n96k16.f32.bf16.bf16 "
+		"wgmma.mma_async.sync.aligned.m64n96k32.s32.s8.s8 "
 		"{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
 		"%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
 		"%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47}, "
-		"%48, %49, p, 1, 1, 0, 0;\n"
+		"%48, %49, p;\n"
 		"}\n"
-		: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-		  "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-		  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-		  "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]),
+		  "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+		  "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]),
+		  "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47])
 		: "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_m64n128k32(int (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
 	asm volatile(
 		"{\n"
 		".reg .pred p;\n"
 		"setp.ne.b32 p, %66, 0;\n"
-		"wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+		"wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
 		"{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
 		"%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
 		"%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
 		"%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
-		"%64, %65, p, 1, 1, 0, 0;\n"
+		"%64, %65, p;\n"
 		"}\n"
-		: "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-		  "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-		  "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-		  "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-		  "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-		  "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+		: "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]),
+		  "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+		  "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]),
+		  "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+		  "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]),
+		  "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
 		: "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 template <int N>
-__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_s8(int (&d)[N / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
 	if constexpr (N == 32) {
-		wgmma_m64n32k16(d, adesc, bdesc, accumulate);
+		wgmma_m64n32k32(d, adesc, bdesc, accumulate);
 	} else if constexpr (N == 64) {
-		wgmma_m64n64k16(d, adesc, bdesc, accumulate);
+		wgmma_m64n64k32(d, adesc, bdesc, accumulate);
 	} else if constexpr (N == 96) {
-		wgmma_m64n96k16(d, adesc, bdesc, accumulate);
+		wgmma_m64n96k32(d, adesc, bdesc, accumulate);
 	} else {
 		static_assert(N == 128, "query block of 32, 64, 96 or 128");
-		wgmma_m64n128k16(d, adesc, bdesc, accumulate);
+		wgmma_m64n128k32(d, adesc, bdesc, accumulate);
 	}
 }
 
-// The candidate test  lb = d~ - e <= tau  rewritten as ONE fused multiply-add and one compare on the raw accumulator s = q~.v~:
-//   IP      d = -s,               e = qe*vn            <=>  s >= -tau - qe*vn                       P = -qe        R = -tau      w = 0
-//   Cosine  d = -s/vn,            e = qe               <=>  s >= (-tau - qe) * vn                   P = -tau - qe  R = 0         w = 0
-//   L2      d = qn2 + vn2 - 2s,   e = 2qe*vn + eps*(qn2+vn2)
-//                                                      <=>  s - (1-eps)/2*vn2 >= -qe*vn + ((1-eps)*qn2 - tau)/2   (w = (1-eps)/2*vn2 per row)
-// The error coefficient carries 5% slack, which also covers the one-ulp differences of these rearrangements.
-constexpr float kTcL2Eps = 1e-5f;
-__device__ __forceinline__ float2 tc_make_pr(int metric, float tau, float qe) {
-	if (metric == kIP) {
-		return make_float2(-qe, -tau);
+// The candidate test lb <= tau on the raw accumulator I, for every score one int -> float conversion (I2FP.F32.S32, an ALU-pipe
+// instruction on sm_90), two (L2: three) FFMAs and one compare.  The block bound e <= n_q M_v, with
+//   M_v = c_v (a* r_v + b* n_v),   a* >= (1 + 2^-8) (n_q + r_q) / n_q,   b* >= (1 + 2^-8) (r_q + (D + 16) 2^-23 n_q) / n_q
+// (a*, b*: the largest over the CTA's query block, computed once per launch), makes the per-row and the per-query factors separate;
+// dividing the test by k_q = s_q (1 for an all-zero query, whose codes are zero) gives, with x = float(I) and S_v = s_v c_v,
+//   IP, Cosine  x S_v + P M_v + R >= 0               P = n_q / k_q   R = tau / k_q
+//   L2          x S_v + P M_v - Z W_v + R >= 0       Z = 1 / k_q     R = (tau - (1 - eps) n_q^2) / (2 k_q)    W_v = (1 - eps) n_v^2 / 2
+// The test is evaluated as "not below zero", so an overflow to NaN (magnitudes far outside the data the exact scan handles) lets
+// the row through to tc_candidate, which decides with the per-query bound e(q, v) and no division.
+__device__ __forceinline__ float tc_l2eps(uint32_t dim) { return kTcL2Eps + float(dim + 1) * 0x1p-23f; }
+__device__ __forceinline__ float2 tc_make_pr(int metric, float tau, float4 qc, float l2eps) {  // qc = (s_q, r_q, n_q, 1 / k_q)
+	const float p = qc.z * qc.w;
+	if (metric != kL2) {
+		return make_float2(p, tau * qc.w);
 	}
-	if (metric == kCos) {
-		return make_float2(-tau - qe, 0.f);
-	}
-	const float qn = qe * (1.f / kTcErrCoef);
-	return make_float2(-qe, 0.5f * ((1.f - kTcL2Eps) * qn * qn - tau));
+	return make_float2(p, 0.5f * (tau - (1.f - l2eps) * qc.z * qc.z) * qc.w);
 }
 
-// The rare path of the epilogue: row `row` passed the test for query `q` (raw accumulator s, row norm vn, qe = c * ||q||).  Appends
-// the candidate, and when its upper bound beats the query's current threshold, inserts it into the query's global bound list (under
-// the per-query lock; other CTAs contend) and tightens the global tau.  Returns the new threshold (+inf when it did not change).
+// The rare path of the epilogue: row `row` passed the block test for query `q` (x = float(I), qc and rc the query's and the row's
+// constants).  When the row's own bound lb = d~ - e(q, v) passes the threshold it is appended as a candidate, and when its upper
+// bound beats the query's current threshold, it is inserted into the query's global bound list (under the per-query lock; other
+// CTAs contend) and tightens the global tau.  Returns the new threshold (+inf when it did not change).
 // Kept out of line: it runs for a few hundred of 10M rows per query, and inlining it at every accumulator only costs instruction cache.
-__device__ __noinline__ float tc_candidate(const TcArgs& a, uint32_t q, uint32_t row, float s, float vn, float qe, float tau) {
-	float d, e;
+__device__ __noinline__ float tc_candidate(const TcArgs& a, uint32_t q, uint32_t row, float x, float4 qc, float4 rc, float tau) {
+	const float p = qc.x * rc.x * x;
+	const float e = (1.f + 0x1p-8f) * fmaf(qc.z + qc.y, rc.y, (qc.y + float(a.dim + 16) * 0x1p-23f * qc.z) * rc.z);
+	float d, err;
 	if (a.metric == kL2) {
-		const float qn = qe * (1.f / kTcErrCoef);
-		d = fmaf(-2.f, s, fmaf(qn, qn, vn * vn));
-		e = 2.f * qe * vn + kTcL2Eps * (qn * qn + vn * vn);
+		d = fmaf(-2.f, p, fmaf(qc.z, qc.z, rc.z * rc.z));
+		err = 2.f * e + tc_l2eps(a.dim) * (qc.z * qc.z + rc.z * rc.z);
 	} else if (a.metric == kCos) {
-		const float vinv = 1.f / vn;  // within 1e-5 of the stored coefficient (normalize.cc shortcut), inside the slack
-		d = -s * vinv;
-		e = qe * 1.0001f;
+		d = -p * rc.w;
+		err = e * rc.w;
 	} else {
-		d = -s;
-		e = qe * vn;
+		d = -p;
+		err = e;
+	}
+	if (d - err > tau) {  // the block test was looser than the row's own bound (NaN: keep the row)
+		return INFINITY;
 	}
 	const unsigned pos = atomicAdd(&a.cand_count[q], 1u);
 	if (pos < a.cand_cap) {
 		a.cand_rows[size_t(q) * a.cand_cap + pos] = row;
 	}
-	const float ub = d + e;
+	const float ub = d + err;
 	float tightened = INFINITY;
 	if (ub < tau && row >= a.init_rows) {
 		while (atomicCAS(&a.ub_lock[q], 0u, 1u) != 0u) {
@@ -326,14 +343,16 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 	unsigned char* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // offset arithmetic keeps the shared window
 	constexpr uint32_t kQchunkBytes = kNq * 128;                       // one K-chunk of the query block: kNq rows x 128 B
 	unsigned char* s_q = base;                                         // [kchunks][kNq][128 B], swizzled by TMA
-	unsigned char* s_rows = s_q + size_t(a.kchunks) * kQchunkBytes;    // [stages][2 blocks][64][128 B]   (1024-aligned: kNq % 8 == 0)
-	uint64_t* bars = reinterpret_cast<uint64_t*>(s_rows + size_t(kTcStages) * kTcStageBytes);
-	uint64_t* full_bar = bars;                   // [stages] TMA -> MMA
-	uint64_t* empty_bar = bars + kTcStages;      // [stages] MMA (every consumer warp of every CTA of the cluster) -> TMA
-	uint64_t* q_bar = bars + 2 * kTcStages;      // queries resident
-	float* s_qe = reinterpret_cast<float*>(bars + 32);                 // [kNq] c * ||q||
-	float* s_thr = s_qe + kNq;                                         // [2][kNq] current tau (map space), per consumer warpgroup
-	float2* s_pr = reinterpret_cast<float2*>(s_thr + 2 * kNq);         // [2][kNq] (P, R): candidate iff s - w_row >= fma(P, ||v||, R)
+	unsigned char* s_rows = s_q + size_t(a.kchunks) * kQchunkBytes;    // [2 rings][stages][64][128 B]   (1024-aligned: kNq % 8 == 0)
+	uint64_t* bars = reinterpret_cast<uint64_t*>(s_rows + size_t(2 * kTcStages) * kTcBlockBytes);
+	uint64_t* full_bar = bars;                       // [2][stages] TMA -> MMA
+	uint64_t* empty_bar = bars + 2 * kTcStages;      // [2][stages] MMA (the consumer warps of the ring in every CTA of the cluster) -> TMA
+	uint64_t* q_bar = bars + 4 * kTcStages;          // queries resident
+	float* s_ab = reinterpret_cast<float*>(q_bar + 1);                 // (a*, b*) of the block bound
+	float4* s_qc = reinterpret_cast<float4*>(bars + 32);               // [kNq] (s_q, r_q, n_q, 1 / k_q)
+	float* s_thr = reinterpret_cast<float*>(s_qc + kNq);               // [2][kNq] current tau (map space), per consumer warpgroup
+	float2* s_pr = reinterpret_cast<float2*>(s_thr + 2 * kNq);         // [2][kNq] (P, R) of the candidate test
+	static_assert(4 * kTcStages + 2 <= 32, "barriers and (a*, b*) fit in front of the per-query constants");
 
 	const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;  // provably warp-uniform
 	const uint32_t ntiles = (a.n + kTcTileRows - 1) / kTcTileRows;
@@ -343,20 +362,29 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 	const uint32_t walker = cid / a.groups, walkers = ncl / a.groups;
 	const uint32_t q0 = a.q0 + ((cid % a.groups) * kCluster + crank) * kNq;
 	const uint32_t nq_valid = q0 < a.nq_total ? min(uint32_t(kNq), a.nq_total - q0) : 0u;
+	const float l2eps = tc_l2eps(a.dim);
 
 	if (threadIdx.x == 0) {
-		for (int s = 0; s < kTcStages; ++s) {
+		for (int s = 0; s < 2 * kTcStages; ++s) {
 			mbar_init(&full_bar[s], 1);
-			mbar_init(&empty_bar[s], 8 * kCluster);  // the eight consumer warps of every CTA that reads the stage's bytes
+			mbar_init(&empty_bar[s], 4 * kCluster);  // the four consumer warps of the ring's warpgroup in every CTA that reads the stage
 		}
 		mbar_init(q_bar, 1);
 		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+		s_ab[0] = s_ab[1] = 0.f;
 	}
+	__syncthreads();
+	const float delta = float(a.dim + 16) * 0x1p-23f;
 	for (uint32_t i = threadIdx.x; i < kNq; i += blockDim.x) {
 		const bool valid = i < nq_valid;
 		const float thr = valid ? ord_float(a.tau[q0 + i]) : -INFINITY;
-		s_qe[i] = valid ? kTcErrCoef * a.qnorm[q0 + i] : 0.f;
-		const float2 pr = valid ? tc_make_pr(a.metric, thr, s_qe[i]) : make_float2(0.f, INFINITY);  // padding queries never match
+		const float4 qc = valid ? a.qc[q0 + i] : make_float4(0.f, 0.f, 0.f, 0.f);
+		if (qc.z > 0.f) {  // non-negative floats order like their bit patterns
+			atomicMax(reinterpret_cast<unsigned int*>(&s_ab[0]), __float_as_uint((qc.z + qc.y) / qc.z));
+			atomicMax(reinterpret_cast<unsigned int*>(&s_ab[1]), __float_as_uint(qc.y / qc.z + delta));
+		}
+		s_qc[i] = qc;
+		const float2 pr = valid ? tc_make_pr(a.metric, thr, qc, l2eps) : make_float2(0.f, -INFINITY);  // padding queries never match
 		s_thr[i] = s_thr[kNq + i] = thr;
 		s_pr[i] = s_pr[kNq + i] = pr;
 	}
@@ -365,31 +393,33 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		cluster_sync_all();  // the peers' barriers exist before anything of ours can signal them
 	}
 
-	if (warp == 0) {
-		// ===== TMA producer: the whole warp walks the loop, one elected lane issues (operands stay in uniform registers) =====
-		if (elect_one_sync()) {
+	if (warp < 2) {
+		// ===== TMA producer of ring `warp`: the whole warp walks the loop, one elected lane issues (operands stay in uniform registers)
+		const uint32_t ring = uint32_t(warp);
+		if (ring == 0 && elect_one_sync()) {
 			mbar_expect_tx(q_bar, a.kchunks * kQchunkBytes);
 			for (uint32_t kc = 0; kc < a.kchunks; ++kc) {
 				tma_load_2d(s_q + size_t(kc) * kQchunkBytes, &map_queries, q_bar, int32_t(kc * kTcChunkK), int32_t(q0));
 			}
 		}
 		__syncwarp();
+		uint64_t* full = full_bar + ring * kTcStages;
+		uint64_t* empty = empty_bar + ring * kTcStages;
+		unsigned char* ring_smem = s_rows + size_t(ring) * kTcStages * kTcBlockBytes;
 		uint32_t stage = 0, phase = 0;
 		for (uint32_t t = walker; t < ntiles; t += walkers) {
+			// the 64-row shadow block 2t + ring, its K chunks 8 KB apart in HBM
+			const unsigned char* src = a.shadow + size_t(2 * t + ring) * a.kchunks * kTcBlockBytes;
 			for (uint32_t kc = 0; kc < a.kchunks; ++kc) {
-				mbar_wait(&empty_bar[stage], phase ^ 1);
-				// a 128-row stage = the 64-row shadow blocks 2t and 2t+1 of this K chunk, 8 KB each, kchunks * 8 KB apart in HBM
-				const unsigned char* src = a.shadow + (size_t(2 * t) * a.kchunks + kc) * kTcBlockBytes;
-				unsigned char* dst = s_rows + size_t(stage) * kTcStageBytes;
+				mbar_wait(&empty[stage], phase ^ 1);
+				unsigned char* dst = ring_smem + size_t(stage) * kTcBlockBytes;
 				if (elect_one_sync()) {
-					mbar_expect_tx(&full_bar[stage], kTcStageBytes);
+					mbar_expect_tx(&full[stage], kTcBlockBytes);
 					if constexpr (kCluster == 1) {
-						bulk_load(dst, src, kTcBlockBytes, &full_bar[stage]);
-						bulk_load(dst + kTcBlockBytes, src + size_t(a.kchunks) * kTcBlockBytes, kTcBlockBytes, &full_bar[stage]);
+						bulk_load(dst, src + size_t(kc) * kTcBlockBytes, kTcBlockBytes, &full[stage]);
 					} else {  // my 1/C of the stage, delivered to every CTA of the cluster
-						constexpr uint32_t kPart = kTcStageBytes / kCluster;
-						const uint32_t blk = crank * kPart / kTcBlockBytes, off = crank * kPart % kTcBlockBytes;
-						bulk_load_mc(dst + blk * kTcBlockBytes + off, src + size_t(blk) * a.kchunks * kTcBlockBytes + off, kPart, &full_bar[stage],
+						constexpr uint32_t kPart = kTcBlockBytes / kCluster;
+						bulk_load_mc(dst + crank * kPart, src + size_t(kc) * kTcBlockBytes + crank * kPart, kPart, &full[stage],
 									 uint16_t((1u << kCluster) - 1u));
 					}
 				}
@@ -401,20 +431,25 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 			}
 		}
 	} else if (warp >= 4) {
-		// ===== consumer warpgroup wg: rows [64 wg, 64 wg + 64) of every tile =====
+		// ===== consumer warpgroup wg: the 64-row blocks 2t + wg of the walker's tiles t, through ring wg =====
 		const uint32_t wg = uint32_t(warp) / 4 - 1, wtid = threadIdx.x - 128 * (wg + 1);
 		float* thr = s_thr + wg * kNq;
 		float2* pr = s_pr + wg * kNq;
+		uint64_t* full = full_bar + wg * kTcStages;
+		uint64_t* empty = empty_bar + wg * kTcStages;
+		const unsigned char* ring_smem = s_rows + size_t(wg) * kTcStages * kTcBlockBytes;
 		// accumulator fragment of wgmma.m64nN: d[4j + {0,1}] = (row r0, query 8j + 2c + {0,1}), d[4j + {2,3}] = the same for row r0 + 8
 		const uint32_t r0 = (wtid >> 5) * 16 + (lane >> 2), c2 = 2 * (lane & 3);
 		const uint32_t my_q = wtid;  // the query whose threshold this thread refreshes from the global list
 		unsigned int tau_ahead = my_q < nq_valid ? a.tau[q0 + my_q] : 0u;
+		const bool l2 = a.metric == kL2;
+		const float ka = (1.f + 0x1p-7f) * s_ab[0], kb = (1.f + 0x1p-7f) * s_ab[1];  // 2^-8 of e, and 2^-8 for the rounding of M_v
 		auto release = [&](uint32_t st) {  // this warp is done with stage st in every CTA that reads it
 			if constexpr (kCluster == 1) {
-				mbar_arrive(&empty_bar[st]);
+				mbar_arrive(&empty[st]);
 			} else {
 				for (uint32_t c = 0; c < uint32_t(kCluster); ++c) {
-					mbar_arrive_cluster(&empty_bar[st], c);
+					mbar_arrive_cluster(&empty[st], c);
 				}
 			}
 		};
@@ -426,29 +461,29 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 				const float tn = ord_float(tau_ahead);
 				if (tn < thr[my_q]) {
 					thr[my_q] = tn;
-					pr[my_q] = tc_make_pr(a.metric, tn, s_qe[my_q]);
+					pr[my_q] = tc_make_pr(a.metric, tn, s_qc[my_q], l2eps);
 				}
 				tau_ahead = a.tau[q0 + my_q];
 			}
-			const uint32_t row0 = t * kTcTileRows + wg * 64 + r0, row1 = row0 + 8;
-			const float2 vw0 = a.vw[row0], vw1 = a.vw[row1];  // rows are padded to whole tiles; consumed after the MMAs
-			float acc[kNq / 2];
+			const uint32_t row0 = (2 * t + wg) * 64 + r0, row1 = row0 + 8;
+			const float4 rc0 = a.rowc[row0], rc1 = a.rowc[row1];  // rows are padded to whole tiles; consumed after the MMAs
+			int acc[kNq / 2];
 #pragma unroll
 			for (int i = 0; i < kNq / 2; ++i) {
-				acc[i] = 0.f;
+				acc[i] = 0;
 			}
 			uint32_t prev = 0;
 			for (uint32_t kc = 0; kc < a.kchunks; ++kc) {
-				mbar_wait(&full_bar[stage], phase);
-				const uint32_t a_addr = smem_u32(s_rows + size_t(stage) * kTcStageBytes + wg * kTcBlockBytes);
+				mbar_wait(&full[stage], phase);
+				const uint32_t a_addr = smem_u32(ring_smem + size_t(stage) * kTcBlockBytes);
 				const uint32_t b_addr = smem_u32(s_q + size_t(kc) * kQchunkBytes);
 				wgmma_fence();
 #pragma unroll
-				for (uint32_t k = 0; k < kTcChunkK / 16; ++k) {  // K = 16 bf16 = 32 bytes inside the 128-byte swizzle row
-					wgmma_bf16<kNq>(acc, wgmma_desc_sw128(a_addr + k * 32), wgmma_desc_sw128(b_addr + k * 32), (kc | k) != 0);
+				for (uint32_t k = 0; k < kTcChunkK / 32; ++k) {  // K = 32 int8 = 32 bytes inside the 128-byte swizzle row
+					wgmma_s8<kNq>(acc, wgmma_desc_sw128(a_addr + k * 32), wgmma_desc_sw128(b_addr + k * 32), (kc | k) != 0);
 				}
 				wgmma_commit();
-				if (kc > 0) {  // the previous chunk's MMAs have retired: its stage goes back to the producers
+				if (kc > 0) {  // the previous chunk's MMAs have retired: its stage goes back to the producer
 					wgmma_wait<1>();
 					if (lane == 0) {
 						release(prev);
@@ -470,25 +505,45 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 			auto tighten = [&](uint32_t qq, float nt) {
 				if (nt < thr[qq]) {
 					thr[qq] = nt;
-					pr[qq] = tc_make_pr(a.metric, nt, s_qe[qq]);
+					pr[qq] = tc_make_pr(a.metric, nt, s_qc[qq], l2eps);
 				}
 			};
-			// hot path: one broadcast LDS.128 per two queries, one FFMA and one compare per score
+			// per-row factors of the block test (rows beyond n have all-zero constants and are masked anyway)
+			const float S0 = rc0.x * rc0.w, S1 = rc1.x * rc1.w;
+			const float M0 = rc0.w * fmaf(ka, rc0.y, kb * rc0.z), M1 = rc1.w * fmaf(ka, rc1.y, kb * rc1.z);
+			const float W0 = l2 ? 0.5f * (1.f - l2eps) * rc0.z * rc0.z : 0.f, W1 = l2 ? 0.5f * (1.f - l2eps) * rc1.z * rc1.z : 0.f;
 			const bool ok0 = row0 < a.n, ok1 = row1 < a.n;
+			auto scan = [&](auto kL2Tag) {
+				constexpr bool kL2 = decltype(kL2Tag)::value;
 #pragma unroll
-			for (int j = 0; j < kNq / 8; ++j) {
-				const uint32_t q = 8 * j + c2;
-				const float4 p2 = *reinterpret_cast<const float4*>(&pr[q]);  // (P, R) of queries q and q + 1
-				const bool h0 = ok0 && acc[4 * j] - vw0.y >= fmaf(p2.x, vw0.x, p2.y);
-				const bool h1 = ok0 && acc[4 * j + 1] - vw0.y >= fmaf(p2.z, vw0.x, p2.w);
-				const bool h2 = ok1 && acc[4 * j + 2] - vw1.y >= fmaf(p2.x, vw1.x, p2.y);
-				const bool h3 = ok1 && acc[4 * j + 3] - vw1.y >= fmaf(p2.z, vw1.x, p2.w);
-				if (h0 | h1 | h2 | h3) {  // rare path: exact bounds, candidate append, threshold tightening
-					if (h0) tighten(q, tc_candidate(a, q0 + q, row0, acc[4 * j], vw0.x, s_qe[q], thr[q]));
-					if (h1) tighten(q + 1, tc_candidate(a, q0 + q + 1, row0, acc[4 * j + 1], vw0.x, s_qe[q + 1], thr[q + 1]));
-					if (h2) tighten(q, tc_candidate(a, q0 + q, row1, acc[4 * j + 2], vw1.x, s_qe[q], thr[q]));
-					if (h3) tighten(q + 1, tc_candidate(a, q0 + q + 1, row1, acc[4 * j + 3], vw1.x, s_qe[q + 1], thr[q + 1]));
+				for (int j = 0; j < kNq / 8; ++j) {
+					const uint32_t q = 8 * j + c2;
+					const float4 p2 = *reinterpret_cast<const float4*>(&pr[q]);  // (P, R) of queries q and q + 1
+					float Ra = p2.y, Rb = p2.w, Rc = p2.y, Rd = p2.w;
+					if constexpr (kL2) {
+						const float za = s_qc[q].w, zb = s_qc[q + 1].w;
+						Ra = fmaf(-za, W0, Ra);
+						Rb = fmaf(-zb, W0, Rb);
+						Rc = fmaf(-za, W1, Rc);
+						Rd = fmaf(-zb, W1, Rd);
+					}
+					const float x0 = float(acc[4 * j]), x1 = float(acc[4 * j + 1]), x2 = float(acc[4 * j + 2]), x3 = float(acc[4 * j + 3]);
+					const bool h0 = ok0 && !(fmaf(x0, S0, fmaf(p2.x, M0, Ra)) < 0.f);
+					const bool h1 = ok0 && !(fmaf(x1, S0, fmaf(p2.z, M0, Rb)) < 0.f);
+					const bool h2 = ok1 && !(fmaf(x2, S1, fmaf(p2.x, M1, Rc)) < 0.f);
+					const bool h3 = ok1 && !(fmaf(x3, S1, fmaf(p2.z, M1, Rd)) < 0.f);
+					if (h0 | h1 | h2 | h3) {  // rare path: the row's own bound, candidate append, threshold tightening
+						if (h0) tighten(q, tc_candidate(a, q0 + q, row0, x0, s_qc[q], rc0, thr[q]));
+						if (h1) tighten(q + 1, tc_candidate(a, q0 + q + 1, row0, x1, s_qc[q + 1], rc0, thr[q + 1]));
+						if (h2) tighten(q, tc_candidate(a, q0 + q, row1, x2, s_qc[q], rc1, thr[q]));
+						if (h3) tighten(q + 1, tc_candidate(a, q0 + q + 1, row1, x3, s_qc[q + 1], rc1, thr[q + 1]));
+					}
 				}
+			};
+			if (l2) {
+				scan(std::true_type{});
+			} else {
+				scan(std::false_type{});
 			}
 			__syncwarp();  // the rare path diverges (per-lane lock loops): reconverge before the .aligned wgmma of the next tile
 			asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // nobody still reads (P, R) when the next refresh writes them
@@ -613,42 +668,62 @@ __global__ void __launch_bounds__(kScanThreads) knn_rerank(const float* rows, ui
 	}
 }
 
-// per-row constants of the filter epilogue, one float2 per row: (max(||v||, tiny), w) with w = the row's share of the L2 expansion
-// (0 for IP / Cosine); rows beyond n are zero.  A 64-row tile's pairs are one contiguous 512-byte block (one cp.async.bulk).
-__global__ void tc_make_vw(const float* vnorm, uint32_t n, uint32_t padded, int metric, float2* vw) {
-	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i < padded) {
-		const float vn = i < n ? vnorm[i] : 0.f;
-		vw[i] = make_float2(fmaxf(vn, 1e-30f), metric == kL2 ? 0.5f * (1.f - kTcL2Eps) * vn * vn : 0.f);
+// ---- helpers: int8 shadow, query codes, threshold init ------------------------------------------------------------------------------
+// The quantiser of the header comment, one warp per vector p[0, dim): calls put(c, code4) for every group of four codes c .. c + 3 of
+// [0, padded) (zero beyond dim) and returns (s, r, n) -- r and n rounded up from fp64 sums, so they bound ||rho|| and ||v||.
+template <typename Put>
+__device__ __forceinline__ float3 tc_quantize(const float* p, uint32_t dim, uint32_t padded, int lane, Put put) {
+	float mx = 0.f;
+	double ss = 0.0;
+	for (uint32_t c = lane; c < dim; c += 32) {
+		const float v = p[c];
+		mx = fmaxf(mx, fabsf(v));
+		ss = fma(double(v), double(v), ss);
 	}
+	for (int off = 16; off > 0; off >>= 1) {
+		mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+		ss += __shfl_xor_sync(0xffffffffu, ss, off);
+	}
+	const float s = mx / 127.f;  // 0 for an all-zero vector (and for one whose largest entry is below 127 denormal steps)
+	double rr = 0.0;
+	for (uint32_t c = 4 * lane; c < padded; c += 128) {
+		uint32_t code4 = 0;
+#pragma unroll
+		for (uint32_t i = 0; i < 4; ++i) {
+			const float v = c + i < dim ? p[c + i] : 0.f;
+			const float code = s > 0.f ? fminf(fmaxf(rintf(v / s), -127.f), 127.f) : 0.f;
+			const double rho = double(v) - double(s) * double(code);  // exact: s * code has 32 significant bits
+			rr = fma(rho, rho, rr);
+			code4 |= (uint32_t(int(code)) & 0xFFu) << (8 * i);
+		}
+		put(c, code4);
+	}
+	for (int off = 16; off > 0; off >>= 1) {
+		rr += __shfl_xor_sync(0xffffffffu, rr, off);
+	}
+	// the fp64 sums are within dim * 2^-53 of the true ones: a relative 2^-40 and rounding up keep r and n upper bounds
+	return make_float3(s, __double2float_ru(sqrt(rr) * (1.0 + 0x1p-40)), __double2float_ru(sqrt(ss) * (1.0 + 0x1p-40)));
 }
 
-// ---- helpers: bf16 shadow, norms, query preparation, threshold init ---------------------------------------------------------------
-// rows fp32 [n][pitch] -> bf16 shadow + ||row||_2.  Shadow layout: [tile of 64 rows][K chunk of 64][64 rows x 128 bytes], and inside
-// every 8 KB block the 16-byte units of row r are XOR-permuted with (r % 8) -- the SWIZZLE_128B pattern wgmma expects in
-// shared memory -- so that a plain contiguous cp.async.bulk brings a ready-to-multiply operand tile.
-__global__ void tc_convert_rows(const float* rows, uint32_t pitch, uint32_t dim, uint32_t row_begin, uint32_t row_end, __nv_bfloat16* shadow,
-								uint32_t kchunks, float* vnorm) {
+// rows fp32 [n][pitch] -> int8 shadow + per-row constants (s_v, r_v, n_v, c_v), c_v = the Cosine norm coefficient (1 otherwise).
+// Shadow layout: [64-row block][K chunk of 128][64 rows x 128 bytes], and inside every 8 KB block the 16-byte units of row r are
+// XOR-permuted with (r % 8) -- the SWIZZLE_128B pattern wgmma expects in shared memory -- so that a plain contiguous cp.async.bulk
+// brings a ready-to-multiply operand tile.
+__global__ void tc_convert_rows(const float* rows, uint32_t pitch, uint32_t dim, uint32_t row_begin, uint32_t row_end, unsigned char* shadow,
+								uint32_t kchunks, const float* norm_coefs, float4* rowc) {
 	const uint32_t row = row_begin + (blockIdx.x * blockDim.x + threadIdx.x) / 32;
 	const int lane = threadIdx.x & 31;
 	if (row >= row_end) {
 		return;
 	}
-	const float* p = rows + size_t(row) * pitch;
-	const uint32_t tile = row / 64u, r = row % 64u;
-	float s = 0.f;
-	for (uint32_t c = lane; c < kchunks * kTcChunkK; c += 32) {
-		const float v = c < dim ? p[c] : 0.f;
-		s = fmaf(v, v, s);
+	const uint32_t blk = row / 64u, r = row % 64u;
+	const float3 srn = tc_quantize(rows + size_t(row) * pitch, dim, kchunks * kTcChunkK, lane, [&](uint32_t c, uint32_t code4) {
 		const uint32_t kc = c / kTcChunkK, cc = c % kTcChunkK;
-		const uint32_t unit = (cc >> 3) ^ (r & 7u);  // 16-byte unit = 8 bf16
-		shadow[(size_t(tile) * kchunks + kc) * 4096u + r * 64u + unit * 8u + (cc & 7u)] = __float2bfloat16_rn(v);
-	}
-	for (int off = 16; off > 0; off >>= 1) {
-		s += __shfl_xor_sync(0xffffffffu, s, off);
-	}
-	if (lane == 0 && vnorm) {
-		vnorm[row] = sqrtf(s);
+		const uint32_t unit = (cc >> 4) ^ (r & 7u);  // 16-byte unit = 16 codes
+		*reinterpret_cast<uint32_t*>(shadow + (size_t(blk) * kchunks + kc) * kTcBlockBytes + r * 128u + unit * 16u + (cc & 15u)) = code4;
+	});
+	if (lane == 0) {
+		rowc[row] = make_float4(srn.x, srn.y, srn.z, norm_coefs ? norm_coefs[row] : 1.f);
 	}
 }
 
@@ -775,25 +850,19 @@ __global__ void __launch_bounds__(256) tc_init_tau(const float* rows, uint32_t p
 	}
 }
 
-// queries fp32 [nq][dim] -> bf16 [nq_pad][pitch_bf] (zero padded) + ||q||
-__global__ void tc_prepare_queries(const float* queries, uint32_t nq, uint32_t nq_pad, uint32_t dim, uint32_t pitch_bf, __nv_bfloat16* out,
-								   float* qnorm) {
+// queries fp32 [nq][dim] -> int8 codes [nq_pad][pitch] (zero padded) + (s_q, r_q, n_q, 1 / k_q), k_q = s_q (1 when s_q = 0)
+__global__ void tc_prepare_queries(const float* queries, uint32_t nq, uint32_t nq_pad, uint32_t dim, uint32_t pitch, unsigned char* codes,
+								   float4* qc) {
 	const uint32_t q = (blockIdx.x * blockDim.x + threadIdx.x) / 32;
 	const int lane = threadIdx.x & 31;
 	if (q >= nq_pad) {
 		return;
 	}
-	float s = 0.f;
-	for (uint32_t c = lane; c < pitch_bf; c += 32) {
-		const float v = (q < nq && c < dim) ? queries[size_t(q) * dim + c] : 0.f;
-		s = fmaf(v, v, s);
-		out[size_t(q) * pitch_bf + c] = __float2bfloat16_rn(v);
-	}
-	for (int off = 16; off > 0; off >>= 1) {
-		s += __shfl_xor_sync(0xffffffffu, s, off);
-	}
+	unsigned char* out = codes + size_t(q) * pitch;
+	const float3 srn = tc_quantize(queries + size_t(q) * dim, q < nq ? dim : 0u, pitch, lane,
+								   [&](uint32_t c, uint32_t code4) { *reinterpret_cast<uint32_t*>(out + c) = code4; });
 	if (lane == 0 && q < nq) {
-		qnorm[q] = sqrtf(s);
+		qc[q] = make_float4(srn.x, srn.y, srn.z, srn.x > 0.f ? 1.f / srn.x : 1.f);
 	}
 }
 
