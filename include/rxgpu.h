@@ -86,6 +86,16 @@ int rxgpu_search_knn(const rxgpu_index*, uint32_t nq, const float* queries /* nq
  * writes the best min(*out_n, max_out) results best-first; *out_n = total number of matches (may exceed max_out). */
 int rxgpu_search_range(const rxgpu_index*, const float* query, float radius, uint64_t max_out, float* out_dist, uint64_t* out_label,
 					   uint64_t* out_n);
+/* BruteforceSearch::SearchRange for nq queries at once (our extension; the reference takes one query per call).
+ * radius[q] is in map space, exactly as for rxgpu_search_range.  Per query q the result is identical to
+ * rxgpu_search_range(queries + q*dim, radius[q], max_out, ...): out_n[q] = total matches, and the best
+ * min(out_n[q], max_out) matches go best-first into row q of out_dist / out_label (nq x max_out).
+ * A batch of >= 64 queries on >= 100k rows runs through the tensor-core candidate filter (rxgpu_set_tensor_core_filter), with up to
+ * max(4096, 2 * min(max_out, 131072)) candidates per query; a query with more is answered by the exact scan (tc_fallbacks).
+ * Does not change the result that rxgpu_last_range_results returns. */
+int rxgpu_search_range_batch(const rxgpu_index*, uint32_t nq, const float* queries /* nq x dim, host */,
+							 const float* radius /* nq */, uint64_t max_out,
+							 float* out_dist, uint64_t* out_label, uint64_t* out_n /* nq */);
 
 /* The result of this thread's last rxgpu_search_range stays retained in the library: entries [offset, offset + n) of it (best first),
  * so a caller that sized its buffers too small fetches the rest WITHOUT a second scan of the rows. */

@@ -118,6 +118,7 @@ _SIGNATURES = {
     "rxgpu_index_device": (C.c_int, [C.c_void_p]),
     "rxgpu_search_knn": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, C.c_uint32, _f32p, _u64p, _u32p]),
     "rxgpu_search_range": (C.c_int, [C.c_void_p, _f32p, C.c_float, C.c_uint64, _f32p, _u64p, _u64p]),
+    "rxgpu_search_range_batch": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, _f32p, C.c_uint64, _f32p, _u64p, _u64p]),
     "rxgpu_last_range_results": (C.c_int, [C.c_uint64, C.c_uint64, _f32p, _u64p]),
     "rxgpu_comm_unique_id": (C.c_int, [C.c_void_p]),
     "rxgpu_comm_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_void_p, C.c_int]),
@@ -313,6 +314,22 @@ class GpuBruteforceSearch:
         _check(self._lib.rxgpu_search_range(self._h, _p(q, _f32p), radius, max_out, _p(d, _f32p), _p(l, _u64p), C.byref(n)))
         m = min(n.value, max_out)
         return d[:m], l[:m], n.value
+
+    def search_range_batch(self, queries, radius, max_out: int | None = None):
+        """queries: [nq, dim]; radius: a scalar or [nq] (map space, as search_range).  Returns (dists [nq, max_out],
+        labels [nq, max_out], counts [nq]): row q holds the best min(counts[q], max_out) matches of query q, best-first, and
+        counts[q] is its total number of matches.  max_out defaults to the row count, at most 131072 (the largest that still
+        sizes the filter's candidate lists by it)."""
+        q = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, self.dim)
+        nq = q.shape[0]
+        r = np.ascontiguousarray(np.broadcast_to(np.asarray(radius, dtype=np.float32), (nq,)))
+        max_out = min(self.size(), 1 << 17) if max_out is None else max_out
+        d = np.zeros((nq, max(max_out, 1)), np.float32)
+        l = np.zeros((nq, max(max_out, 1)), np.uint64)
+        c = np.zeros(nq, np.uint64)
+        _check(self._lib.rxgpu_search_range_batch(self._h, nq, _p(q, _f32p), _p(r, _f32p), max_out, _p(d, _f32p), _p(l, _u64p),
+                                                  _p(c, _u64p)))
+        return d[:, :max_out], l[:, :max_out], c
 
     def select(self, query, k: int | None = None, radius: float | None = None, need_sort=True, is_array=False, raw=False,
                max_out: int | None = None):

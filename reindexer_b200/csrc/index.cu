@@ -241,6 +241,10 @@ constexpr size_t kTcSmemLimit = 227 * 1024;  // the per-block opt-in maximum of 
 // (config 1, int8 filter, candidates per query: k = 10: 1 620, k = 30: 3 820, k = 63: 6 880, k = 127: 12 000); 4096 is also the floor, so masses of near-duplicates still overflow to the
 // exact scan instead of being re-ranked one list entry at a time
 uint32_t tcCandCap(uint32_t k1) { return std::max<uint32_t>(4096u, 256u * k1); }
+// per-query candidate list entries of a range batch: twice the matches the caller asked for (the bound's window of candidates that
+// do not match), the KNN floor of 4096, and at most 2^18 (1 GiB of candidate rows for 1024 queries); a query with more candidates
+// is answered by the exact range scan
+uint32_t tcRangeCap(uint64_t max_out) { return uint32_t(std::max<uint64_t>(4096u, 2 * std::min<uint64_t>(max_out, 1u << 17))); }
 
 // knn_tc_filter<query block, cluster size>: one instantiation per wgmma N and per cluster shape
 using TcKernel = void (*)(const CUtensorMap, const TcArgs);
@@ -264,8 +268,9 @@ uint32_t tcQueryBlock(uint32_t nq, uint32_t kchunks) {
 	return std::min(nqb, (((nq + blocks - 1) / blocks) + 31u) & ~31u);  // even out the blocks
 }
 
-bool tcEligible(const rxgpu_index* ix, uint32_t nq, uint32_t k1, int mode) {
-	if (ix->tc_mode == 2 || mode != kModeTopK || k1 > kTcMaxK1 || !encodeTiled()) {
+// whether the filter serves a batch of nq queries at all (KNN and range search alike)
+bool tcServes(const rxgpu_index* ix, uint32_t nq) {
+	if (ix->tc_mode == 2 || !encodeTiled()) {
 		return false;
 	}
 	if (tcQueryBlock(nq, (ix->dim + kTcChunkK - 1) / kTcChunkK) == 0) {
@@ -276,6 +281,9 @@ bool tcEligible(const rxgpu_index* ix, uint32_t nq, uint32_t k1, int mode) {
 		return false;
 	}
 	return ix->tc_mode == 1 || (nq >= 64 && ix->size >= 100000);
+}
+bool tcEligible(const rxgpu_index* ix, uint32_t nq, uint32_t k1, int mode) {
+	return mode == kModeTopK && k1 <= kTcMaxK1 && tcServes(ix, nq);
 }
 
 // int8 shadow + per-row constants, brought up to date when the rows changed since the last large-batch search
@@ -326,10 +334,12 @@ int ensureShadow(const rxgpu_index* ix, cudaStream_t st) {
 int scanTopKExact(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1, int mode,
 				  float bound, float* d_out_dist, uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count);
 
-// Large batches: approximate int8 tensor-core scores with a certified error bound select the candidates, the exact fp32 routine
-// re-ranks them.  Output = the same top-k1 under (dist, internal index) as scanTopKExact, bit for bit.
-int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1,
-					   float* d_out_dist, uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count) {
+// The candidate filter over a batch: the rows whose certified lower bound is at or below the query's threshold tau go to
+// ws.d_cand_rows[q][candCap], and ws.d_cand_count[q] counts them all (also past candCap: an overflowed list).  KNN (h_tau == nullptr):
+// tau starts from tc_init_tau and tightens to the k1-th best upper bound.  Range search: h_tau[q] = float_ord(radius) fixes tau, and
+// init_rows = UINT32_MAX keeps every row out of the bound list (knn_tc.cuh header comment); k1 is not used.
+int tcFilter(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1, uint32_t candCap,
+			 const unsigned int* h_tau) {
 	if (int rc = ensureShadow(ix, st)) {
 		return rc;
 	}
@@ -346,21 +356,24 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	RX_CUDA(ws.d_qcodes.ensure(size_t(nqPad) * pitchQ));
 	RX_CUDA(ws.d_qc.ensure(nqPad));
 	RX_CUDA(ws.d_tau.ensure(nqPad));
-	RX_CUDA(ws.d_ub_list.ensure(size_t(nqPad) * kTcMaxK1));
-	RX_CUDA(ws.d_ub_lock.ensure(nqPad));
 	RX_CUDA(ws.d_cand_count.ensure(nqPad));
-	const uint32_t candCap = tcCandCap(k1);
 	RX_CUDA(ws.d_cand_rows.ensure(size_t(nqPad) * candCap));
 	RX_CUDA(ws.h_cand_count.ensure(nqPad));
-	RX_CUDA(ws.d_lists.ensure(size_t(nq) * k1));
 	tc_prepare_queries<<<(nqPad * 32 + 255) / 256, 256, 0, st>>>(d_queries, nq, nqPad, ix->dim, pitchQ, ws.d_qcodes.p, ws.d_qc.p);
-	RX_CUDA(raiseSmemCeilingOnce(tc_init_tau, ix->device, int(tc_init_smem_bytes(2048))));
-	tc_init_tau<<<(nq + kTcInitQ - 1) / kTcInitQ, 256, tc_init_smem_bytes(ix->pitch), st>>>(
-		ix->d_rows, ix->pitch, ix->dim, ix->metric == RXGPU_COS ? ix->d_norms : nullptr, uint32_t(std::min<uint64_t>(ix->size, kTcInitRows)),
-		d_queries, nq, k1, ix->metric, ws.d_tau.p, ws.d_ub_list.p, ws.d_ub_lock.p);
+	g_stats.launches += 1;
+	if (h_tau) {
+		RX_CUDA(cudaMemcpyAsync(ws.d_tau.p, h_tau, size_t(nq) * 4, cudaMemcpyHostToDevice, st));
+	} else {
+		RX_CUDA(ws.d_ub_list.ensure(size_t(nqPad) * kTcMaxK1));
+		RX_CUDA(ws.d_ub_lock.ensure(nqPad));
+		RX_CUDA(raiseSmemCeilingOnce(tc_init_tau, ix->device, int(tc_init_smem_bytes(2048))));
+		tc_init_tau<<<(nq + kTcInitQ - 1) / kTcInitQ, 256, tc_init_smem_bytes(ix->pitch), st>>>(
+			ix->d_rows, ix->pitch, ix->dim, ix->metric == RXGPU_COS ? ix->d_norms : nullptr, uint32_t(std::min<uint64_t>(ix->size, kTcInitRows)),
+			d_queries, nq, k1, ix->metric, ws.d_tau.p, ws.d_ub_list.p, ws.d_ub_lock.p);
+		g_stats.launches += 1;
+	}
 	RX_CUDA(cudaMemsetAsync(ws.d_cand_count.p, 0, size_t(nqPad) * 4, st));
 	RX_CUDA(cudaGetLastError());
-	g_stats.launches += 2;
 	CUtensorMap mapQ;
 	if (int rc = makeCodeMap(&mapQ, ws.d_qcodes.p, pitchQ, nqPad, nqb)) {
 		return rc;
@@ -389,9 +402,9 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	a.rowc = ix->d_rowc;
 	a.qc = ws.d_qc.p;
 	a.tau = ws.d_tau.p;
-	a.ub_list = ws.d_ub_list.p;
-	a.ub_lock = ws.d_ub_lock.p;
-	a.init_rows = uint32_t(std::min<uint64_t>(ix->size, kTcInitRows));
+	a.ub_list = h_tau ? nullptr : ws.d_ub_list.p;
+	a.ub_lock = h_tau ? nullptr : ws.d_ub_lock.p;
+	a.init_rows = h_tau ? UINT32_MAX : uint32_t(std::min<uint64_t>(ix->size, kTcInitRows));
 	a.cand_rows = ws.d_cand_rows.p;
 	a.cand_count = ws.d_cand_count.p;
 	a.cand_cap = candCap;
@@ -432,6 +445,18 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	g_stats.tc_cluster = cluster;
 	g_stats.tc_kernel = 1;
 	g_stats.query_tile = nqb * cluster;
+	return 0;
+}
+
+// Large batches: approximate int8 tensor-core scores with a certified error bound select the candidates, the exact fp32 routine
+// re-ranks them.  Output = the same top-k1 under (dist, internal index) as scanTopKExact, bit for bit.
+int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1,
+					   float* d_out_dist, uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count) {
+	const uint32_t candCap = tcCandCap(k1);
+	if (int rc = tcFilter(ix, ws, st, d_queries, nq, k1, candCap, nullptr)) {
+		return rc;
+	}
+	RX_CUDA(ws.d_lists.ensure(size_t(nq) * k1));
 	// exact re-rank of the candidates with the arithmetic of knn_scan_warp, then decode + labels
 	const size_t rsmem = size_t((ix->dim + 127) / 128) * 512 + size_t(kScanWarps) * (k1 + kCandBuf) * 8;
 	const float* norms = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
@@ -1201,21 +1226,10 @@ int rxgpu_search_knn(const rxgpu_index* ix, uint32_t nq, const float* queries, u
 	return 0;
 }
 
-static int searchRangeHost(const rxgpu_index* ix, const float* query, float radius, std::vector<Hit>& res) {
+// The exact range scan of one device-resident query: every row with dist < radius, in the order of hitLessByLabel.  Uses ws.d_range.
+static int scanRangeExact(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_query, float radius, std::vector<Hit>& res) {
 	res.clear();
-	g_stats = rxgpu_search_stats{};
-	if (ix->size == 0) {
-		return 0;
-	}
-	WsLease lease(ix);
-	Workspace& ws = *lease.ws;
-	if (!ws.stream) {
-		RX_CUDA(cudaStreamCreateWithFlags(&ws.stream, cudaStreamNonBlocking));
-	}
-	cudaStream_t st = ws.stream;
-	RX_CUDA(ws.d_queries.ensure(ix->dim));
 	RX_CUDA(ws.d_range_count.ensure(1));
-	RX_CUDA(cudaMemcpyAsync(ws.d_queries.p, query, ix->dim * sizeof(float), cudaMemcpyHostToDevice, st));
 	// result buffer: up to 4M matches (32 MB) without a rescan; a larger result grows the buffer and scans once more
 	uint64_t cap = std::max<uint64_t>(ws.d_range.n, std::min<uint64_t>(std::max<uint64_t>(ix->size, 1), 1u << 22));
 	for (;;) {
@@ -1224,7 +1238,7 @@ static int searchRangeHost(const rxgpu_index* ix, const float* query, float radi
 		ScanArgs a{};
 		a.rows = ix->d_rows;
 		a.norm_coefs = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
-		a.queries = ws.d_queries.p;
+		a.queries = d_query;
 		a.pitch = ix->pitch;
 		a.dim = ix->dim;
 		a.row_begin = 0;
@@ -1258,10 +1272,158 @@ static int searchRangeHost(const rxgpu_index* ix, const float* query, float radi
 		}
 		break;
 	}
-	g_stats.query_tile = 1;
-	g_stats.algorithmic_bytes = uint64_t(ix->size) * ix->dim * 4 + (ix->metric == RXGPU_COS ? uint64_t(ix->size) * 4 : 0) + ix->dim * 4 +
-								res.size() * 8;
+	g_stats.algorithmic_bytes += uint64_t(ix->size) * ix->dim * 4 + (ix->metric == RXGPU_COS ? uint64_t(ix->size) * 4 : 0) + ix->dim * 4 +
+								 res.size() * 8;
 	std::sort(res.begin(), res.end(), hitLessByLabel);  // the order in which the reference's heap drains backwards
+	return 0;
+}
+
+static int searchRangeHost(const rxgpu_index* ix, const float* query, float radius, std::vector<Hit>& res) {
+	res.clear();
+	g_stats = rxgpu_search_stats{};
+	if (ix->size == 0) {
+		return 0;
+	}
+	WsLease lease(ix);
+	Workspace& ws = *lease.ws;
+	if (!ws.stream) {
+		RX_CUDA(cudaStreamCreateWithFlags(&ws.stream, cudaStreamNonBlocking));
+	}
+	cudaStream_t st = ws.stream;
+	RX_CUDA(ws.d_queries.ensure(ix->dim));
+	RX_CUDA(cudaMemcpyAsync(ws.d_queries.p, query, ix->dim * sizeof(float), cudaMemcpyHostToDevice, st));
+	if (int rc = scanRangeExact(ix, ws, st, ws.d_queries.p, radius, res)) {
+		return rc;
+	}
+	g_stats.query_tile = 1;
+	return 0;
+}
+
+// Range search for a batch (rxgpu_search_range_batch).  A batch the filter serves (tcServes) runs one filter pass with tau = radius,
+// then the range mode of knn_rerank keeps the candidates with dist < radius -- the same set and distance bits as the exact range
+// scan, which answers every other query.
+static int searchRangeBatchHost(const rxgpu_index* ix, uint32_t nq, const float* queries, const float* radius, uint64_t max_out,
+								float* out_dist, uint64_t* out_label, uint64_t* out_n) {
+	g_stats = rxgpu_search_stats{};
+	std::vector<Hit> res;
+	auto emit = [&](uint32_t q, const std::vector<Hit>& hits) {  // hits in the order of hitLessByLabel
+		const uint64_t n = std::min<uint64_t>(hits.size(), max_out);
+		for (uint64_t i = 0; i < n; ++i) {
+			out_dist[q * max_out + i] = hits[i].dist;
+			out_label[q * max_out + i] = hits[i].label;
+		}
+		out_n[q] = hits.size();
+	};
+	// dist < radius never holds for a NaN or -inf radius: no matches, no scan.  A +inf radius matches every row: the exact scan.
+	auto filtered = [&](uint32_t q) { return radius[q] > -INFINITY && radius[q] < INFINITY; };
+	if (ix->size == 0) {
+		for (uint32_t q = 0; q < nq; ++q) {
+			emit(q, res);
+		}
+		return 0;
+	}
+	WsLease lease(ix);
+	Workspace& ws = *lease.ws;
+	if (!ws.stream) {
+		RX_CUDA(cudaStreamCreateWithFlags(&ws.stream, cudaStreamNonBlocking));
+	}
+	cudaStream_t st = ws.stream;
+	const size_t qn = size_t(nq) * ix->dim;
+	RX_CUDA(ws.d_queries.ensure(qn));
+	RX_CUDA(ws.h_queries.ensure(qn));
+	std::memcpy(ws.h_queries.p, queries, qn * sizeof(float));
+	RX_CUDA(cudaMemcpyAsync(ws.d_queries.p, ws.h_queries.p, qn * sizeof(float), cudaMemcpyHostToDevice, st));
+	std::vector<uint32_t> exact;  // queries the exact range scan answers
+	if (tcServes(ix, nq)) {
+		const uint32_t cap = tcRangeCap(max_out);
+		// the queries outside the filter get a radius of -inf: no candidate passes, and none would match
+		std::vector<float> rad(nq);
+		std::vector<unsigned int> tau(nq);
+		for (uint32_t q = 0; q < nq; ++q) {
+			rad[q] = filtered(q) ? radius[q] : -INFINITY;
+			tau[q] = float_ord(rad[q]);
+		}
+		if (int rc = tcFilter(ix, ws, st, ws.d_queries.p, nq, 0, cap, tau.data())) {
+			return rc;
+		}
+		ws.tc_lists_valid = false;  // the candidate lists now hold this batch's range candidates: no tie replay may read them
+		RX_CUDA(ws.d_radius.ensure(nq));
+		RX_CUDA(ws.d_range_n.ensure(nq));
+		RX_CUDA(ws.h_range_n.ensure(nq));
+		RX_CUDA(ws.d_range.ensure(size_t(nq) * cap));
+		RX_CUDA(cudaMemcpyAsync(ws.d_radius.p, rad.data(), size_t(nq) * 4, cudaMemcpyHostToDevice, st));
+		RX_CUDA(cudaMemsetAsync(ws.d_range_n.p, 0, size_t(nq) * 4, st));
+		const size_t rsmem = size_t((ix->dim + 127) / 128) * 512 + size_t(kScanWarps) * (1 + kCandBuf) * 8;
+		const float* norms = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
+		if (ix->metric == RXGPU_L2) {
+			RX_CUDA(raiseSmemCeilingOnce(knn_rerank<true>, ix->device, kScanSmemBudget));
+			knn_rerank<true><<<nq, kScanThreads, rsmem, st>>>(ix->d_rows, ix->pitch, ix->dim, norms, ws.d_queries.p, ws.d_cand_rows.p,
+															   ws.d_cand_count.p, cap, 1, nullptr, nullptr, nullptr, ws.d_radius.p,
+															   ws.d_range.p, ws.d_range_n.p);
+		} else {
+			RX_CUDA(raiseSmemCeilingOnce(knn_rerank<false>, ix->device, kScanSmemBudget));
+			knn_rerank<false><<<nq, kScanThreads, rsmem, st>>>(ix->d_rows, ix->pitch, ix->dim, norms, ws.d_queries.p, ws.d_cand_rows.p,
+																ws.d_cand_count.p, cap, 1, nullptr, nullptr, nullptr, ws.d_radius.p,
+																ws.d_range.p, ws.d_range_n.p);
+		}
+		RX_CUDA(cudaGetLastError());
+		g_stats.launches += 1;
+		RX_CUDA(cudaMemcpyAsync(ws.h_cand_count.p, ws.d_cand_count.p, size_t(nq) * 4, cudaMemcpyDeviceToHost, st));
+		RX_CUDA(cudaMemcpyAsync(ws.h_range_n.p, ws.d_range_n.p, size_t(nq) * 4, cudaMemcpyDeviceToHost, st));
+		RX_CUDA(cudaStreamSynchronize(st));
+		// copy back the first `width` keys of every query's region: as many as the largest answer the filter decided
+		uint64_t cands = 0;
+		uint32_t width = 0;
+		for (uint32_t q = 0; q < nq; ++q) {
+			if (!filtered(q)) {
+				continue;
+			}
+			cands += std::min(ws.h_cand_count.p[q], cap);
+			if (ws.h_cand_count.p[q] > cap) {  // an overflowed list (masses of rows near the radius): the exact scan answers it
+				g_stats.tc_fallbacks += 1;
+			} else {
+				width = std::max(width, ws.h_range_n.p[q]);
+			}
+		}
+		if (width) {
+			RX_CUDA(ws.h_range.ensure(size_t(nq) * width));
+			RX_CUDA(cudaMemcpy2DAsync(ws.h_range.p, size_t(width) * 8, ws.d_range.p, size_t(cap) * 8, size_t(width) * 8, nq,
+									  cudaMemcpyDeviceToHost, st));
+			RX_CUDA(cudaStreamSynchronize(st));
+		}
+		for (uint32_t q = 0; q < nq; ++q) {
+			if (!filtered(q) || ws.h_cand_count.p[q] > cap) {
+				exact.push_back(q);
+				continue;
+			}
+			res.clear();
+			const uint64_t* keys = ws.h_range.p + size_t(q) * width;
+			for (uint32_t i = 0; i < ws.h_range_n.p[q]; ++i) {
+				const uint32_t row = uint32_t(keys[i]);
+				res.push_back(Hit{ord_float(uint32_t(keys[i] >> 32)), row, ix->h_labels[row]});
+			}
+			std::sort(res.begin(), res.end(), hitLessByLabel);  // the order of the exact range scan
+			emit(q, res);
+		}
+		g_stats.tc_used = 1;
+		g_stats.tc_candidates = cands;
+		g_stats.algorithmic_bytes += cands * (uint64_t(ix->dim) * 4 + 4);
+	} else {
+		for (uint32_t q = 0; q < nq; ++q) {
+			exact.push_back(q);
+		}
+		g_stats.query_tile = 1;
+	}
+	for (const uint32_t q : exact) {
+		if (radius[q] == INFINITY || filtered(q)) {
+			if (int rc = scanRangeExact(ix, ws, st, ws.d_queries.p + size_t(q) * ix->dim, radius[q], res)) {
+				return rc;
+			}
+		} else {
+			res.clear();
+		}
+		emit(q, res);
+	}
 	return 0;
 }
 
@@ -1288,6 +1450,21 @@ int rxgpu_search_range(const rxgpu_index* ix, const float* query, float radius, 
 		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
 	}
 	return 0;
+}
+
+int rxgpu_search_range_batch(const rxgpu_index* ix, uint32_t nq, const float* queries, const float* radius, uint64_t max_out,
+							 float* out_dist, uint64_t* out_label, uint64_t* out_n) {
+	if (int rc = checkIndex(ix)) {
+		return rc;
+	}
+	if (nq && (!queries || !radius || !out_n || (max_out && (!out_dist || !out_label)))) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: null argument");
+	}
+	try {
+		return searchRangeBatchHost(ix, nq, queries, radius, max_out, out_dist, out_label, out_n);
+	} catch (const std::bad_alloc&) {
+		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
+	}
 }
 
 int rxgpu_last_range_results(uint64_t offset, uint64_t n, float* out_dist, uint64_t* out_label) {

@@ -130,8 +130,11 @@ struct Workspace {
 	DevBuf<uint32_t> d_out_idx;
 	DevBuf<uint64_t> d_out_label;
 	DevBuf<uint32_t> d_out_count;
-	DevBuf<uint64_t> d_range;
+	DevBuf<uint64_t> d_range;  // single-query range scan: its matches; range batch on the filter: [nq][cand cap] matches per query
 	DevBuf<unsigned long long> d_range_count;
+	DevBuf<float> d_radius;          // range batch on the filter: per-query radius, and its per-query match counts
+	DevBuf<unsigned int> d_range_n;
+	PinBuf<unsigned int> h_range_n;
 	DevBuf<unsigned char> d_qcodes;  // int8 query codes for the tensor-core filter
 	DevBuf<float4> d_qc;             // their per-query constants (s_q, r_q, ||q||, 1 / k_q)
 	DevBuf<unsigned int> d_tau, d_cand_count, d_ub_lock;

@@ -23,6 +23,11 @@
 //                 updated under a per-query lock -- only O(k log n) successful inserts per query over a whole pass) => a valid
 //                 upper bound of the final k1-th best TRUE distance; a row is a candidate iff lb <= tau_q.  tau starts from an
 //                 exact scan of the first rows (tc_init_tau) and only decreases.
+//   range search  tau_q = the query's radius, seeded by the host and never tightened (init_rows = UINT32_MAX: no row reaches the
+//                 bound list, so ub_list, ub_lock and k1 are never read).  A row matches iff its exact distance d < radius, and every
+//                 such row has lb <= d < tau_q, so it is a candidate; the exact re-rank (knn_rerank's range mode) then keeps the
+//                 candidates with d < radius, computed with the exact scan's arithmetic -- the same set and the same distance bits as
+//                 the exact range scan.  Certification needs no upper bound here, only that lb never exceeds d.
 //
 // Launch shape: one grid covers G query groups (a group = one query block of NQ queries per CTA of a cluster) with W tile walkers
 // each, G x W <= the clusters resident at once (config 1: 8 blocks x 16 walkers = 128 CTAs, one launch per batch).  Walker w visits
@@ -563,14 +568,21 @@ template <bool kIsL2>
 __global__ void __launch_bounds__(kScanThreads) knn_rerank(const float* rows, uint32_t pitch, uint32_t dim, const float* norm_coefs,
 															const float* queries, const uint32_t* cand_rows, const unsigned int* cand_count,
 															uint32_t cand_cap, uint32_t k1, uint64_t* lists /* [gridDim.x][k1] */,
-															const uint32_t* qsel = nullptr, const float* tie_bound = nullptr) {
+															const uint32_t* qsel = nullptr, const float* tie_bound = nullptr,
+															const float* radius = nullptr, uint64_t* range_keys = nullptr,
+															unsigned int* range_count = nullptr) {
 	// qsel: CTA b serves query qsel[b] (default: query b).  tie_bound != nullptr = tie mode (kModeTieRows): among the candidates
 	// with dist <= tie_bound[b], the first k1 in internal row order (key = row << 32 | ord(dist)) -- every row at or below the k-th
 	// distance is a candidate, so this replaces a second scan of the whole shard when the reference's tie rule must be replayed.
+	// radius != nullptr = range mode: every candidate with dist < radius[q] (strict, as the exact range scan) is appended, unordered,
+	// as make_key(dist, row) to range_keys[q][cand_cap] and counted in range_count[q]; lists and k1 are not used.  The matches are a
+	// subset of the query's candidates, so they never exceed cand_cap.
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const uint32_t q = qsel ? qsel[blockIdx.x] : blockIdx.x;
 	const bool tie = tie_bound != nullptr;
+	const bool range = radius != nullptr;
+	const float rad = range ? radius[q] : 0.f;
 	const float bound = tie ? tie_bound[blockIdx.x] : 0.f;
 	const uint32_t nch = (dim + 127u) / 128u, dp4 = nch * 32u, pitch4 = pitch >> 2;
 	const uint32_t m = k1 + kCandBuf;
@@ -624,6 +636,12 @@ __global__ void __launch_bounds__(kScanThreads) knn_rerank(const float* rows, ui
 		if (!kIsL2 && norm_coefs != nullptr) {
 			dist *= norm_coefs[row];
 		}
+		if (range) {
+			if (lane == 0 && dist < rad) {
+				range_keys[size_t(q) * cand_cap + atomicAdd(&range_count[q], 1u)] = make_key(dist, row);
+			}
+			continue;
+		}
 		const uint64_t key = !tie ? make_key(dist, row) : (dist <= bound ? ((uint64_t(row) << 32) | float_ord(dist)) : kKeyNone);
 		if (key < thr) {  // warp-uniform
 			if (lane == 0) {
@@ -637,6 +655,9 @@ __global__ void __launch_bounds__(kScanThreads) knn_rerank(const float* rows, ui
 				cnt = 0;
 			}
 		}
+	}
+	if (range) {
+		return;
 	}
 	if (cnt) {
 		warp_select(wkeys, k1 + cnt, k1, lane);
