@@ -488,7 +488,7 @@ typedef struct {
 void rxgpu_last_search_stats(rxgpu_search_stats* out);
 /* large query batches: int8 tensor-core filter (exact integer dot products of per-row scaled codes, certified by per-row
  * residual norms) + exact fp32 re-rank (results identical to the exact scan).
- * mode 0 = automatic (batches >= 64 queries on >= 100k rows, k <= 127), 1 = whenever possible, 2 = never;
+ * mode 0 = automatic (batches >= 64 queries on >= 100k rows, k <= 1023), 1 = whenever possible, 2 = never;
  * 3 / 4 = as 1 with single CTAs (the default) / clusters of up to two CTAs sharing every row tile; all give the same bits. */
 int rxgpu_set_tensor_core_filter(rxgpu_index*, int mode);
 /* process-wide switch: bracket every scan-kernel launch with CUDA events (used by bench.py for the roofline figure) */

@@ -127,9 +127,12 @@ int pickQueryTile(const rxgpu_index* ix, uint32_t nq) {
 }
 
 // Top-k1 rows per query under the total order (dist, internal index) -- or, in tie mode, the first k1 rows in internal
-// order with dist <= bound.  Everything stays on the device; results land in d_out_* ([nq][k1]).
+// order with dist <= bound.  Everything stays on the device; results land in d_out_* ([nq][k1]).  rowEnd < size: only the rows
+// [0, rowEnd) (the seed of the staged thresholds).
 int scanTopKExact(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1, int mode,
-				  float bound, float* d_out_dist, uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count) {
+				  float bound, float* d_out_dist, uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count,
+				  uint32_t rowEnd = UINT32_MAX) {
+	const uint32_t nrows = uint32_t(std::min<uint64_t>(rowEnd, ix->size));
 	// k1 > kMaxFusedK1: rounds of <= kMaxFusedK1 results; a round only admits keys above the previous round's last key, so the
 	// rounds concatenate to the top-k1 under the same total order (one pass over the rows per round)
 	const uint32_t kr = std::min<uint32_t>(k1, kMaxFusedK1);
@@ -147,7 +150,7 @@ int scanTopKExact(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const f
 	a.pitch = ix->pitch;
 	a.dim = ix->dim;
 	a.row_begin = 0;
-	a.row_end = uint32_t(ix->size);
+	a.row_end = nrows;
 	a.k1 = kr;
 	a.mode = mode;
 	a.bound = bound;
@@ -200,7 +203,7 @@ int scanTopKExact(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const f
 		}
 	}
 	g_stats.query_tile = uint32_t(qt);
-	const uint64_t perPass = uint64_t(ix->size) * ix->dim * 4 + (ix->metric == RXGPU_COS ? uint64_t(ix->size) * 4 : 0) +
+	const uint64_t perPass = uint64_t(nrows) * ix->dim * 4 + (ix->metric == RXGPU_COS ? uint64_t(nrows) * 4 : 0) +
 							 uint64_t(qt) * ix->dim * 4 + uint64_t(qt) * kr * 12;
 	g_stats.algorithmic_bytes += perPass * ((nq + qt - 1) / qt) * rounds;
 	return 0;
@@ -245,6 +248,15 @@ uint32_t tcCandCap(uint32_t k1) { return std::max<uint32_t>(4096u, 256u * k1); }
 // do not match), the KNN floor of 4096, and at most 2^18 (1 GiB of candidate rows for 1024 queries); a query with more candidates
 // is answered by the exact range scan
 uint32_t tcRangeCap(uint64_t max_out) { return uint32_t(std::max<uint64_t>(4096u, 2 * std::min<uint64_t>(max_out, 1u << 17))); }
+// Staged thresholds (k1 > kTcMaxK1, DESIGN 3.2): the seed is the exact top-k1 of the first kStageSeedPerK1 * k1 rows, each stage's
+// prefix is kStageRatio times the previous one, and a stage re-ranks about kStageRatio * k1 * (the bound's window factor) candidates
+// per query.  Lists of kStageCapPerK1 * k1 entries, at most 2^18.  Chosen at config 1 on an H100 (DESIGN 3.2): r = 4 against 8 and
+// 16, a seed of 2 k1 rows against 8 k1.
+constexpr uint32_t kStageRatio = 4;
+constexpr uint32_t kStageSeedPerK1 = 2;
+constexpr uint32_t kStageCapPerK1 = 64;
+uint32_t stageSeedRows(uint32_t k1) { return kStageSeedPerK1 * k1; }
+uint32_t stageCandCap(uint32_t k1) { return std::min<uint32_t>(1u << 18, std::max<uint32_t>(4096u, kStageCapPerK1 * k1)); }
 
 // knn_tc_filter<query block, cluster size>: one instantiation per wgmma N and per cluster shape
 using TcKernel = void (*)(const CUtensorMap, const TcArgs);
@@ -283,7 +295,7 @@ bool tcServes(const rxgpu_index* ix, uint32_t nq) {
 	return ix->tc_mode == 1 || (nq >= 64 && ix->size >= 100000);
 }
 bool tcEligible(const rxgpu_index* ix, uint32_t nq, uint32_t k1, int mode) {
-	return mode == kModeTopK && k1 <= kTcMaxK1 && tcServes(ix, nq);
+	return mode == kModeTopK && k1 <= kTcStagedMaxK1 && tcServes(ix, nq);
 }
 
 // int8 shadow + per-row constants, brought up to date when the rows changed since the last large-batch search
@@ -331,15 +343,15 @@ int ensureShadow(const rxgpu_index* ix, cudaStream_t st) {
 	return 0;
 }
 
-int scanTopKExact(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1, int mode,
-				  float bound, float* d_out_dist, uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count);
+// One batch of queries on the candidate filter: the int8 query codes and their tensor map, prepared once, and the launch shape.
+struct TcBatch {
+	uint32_t nq, nqb, cluster, ngroups, nqPad, kchunks;
+	int resident;
+	TcKernel kfn;
+	CUtensorMap mapQ;
+};
 
-// The candidate filter over a batch: the rows whose certified lower bound is at or below the query's threshold tau go to
-// ws.d_cand_rows[q][candCap], and ws.d_cand_count[q] counts them all (also past candCap: an overflowed list).  KNN (h_tau == nullptr):
-// tau starts from tc_init_tau and tightens to the k1-th best upper bound.  Range search: h_tau[q] = float_ord(radius) fixes tau, and
-// init_rows = UINT32_MAX keeps every row out of the bound list (knn_tc.cuh header comment); k1 is not used.
-int tcFilter(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1, uint32_t candCap,
-			 const unsigned int* h_tau) {
+int tcPrepare(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t candCap, TcBatch& b) {
 	if (int rc = ensureShadow(ix, st)) {
 		return rc;
 	}
@@ -361,27 +373,50 @@ int tcFilter(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float*
 	RX_CUDA(ws.h_cand_count.ensure(nqPad));
 	tc_prepare_queries<<<(nqPad * 32 + 255) / 256, 256, 0, st>>>(d_queries, nq, nqPad, ix->dim, pitchQ, ws.d_qcodes.p, ws.d_qc.p);
 	g_stats.launches += 1;
-	if (h_tau) {
-		RX_CUDA(cudaMemcpyAsync(ws.d_tau.p, h_tau, size_t(nq) * 4, cudaMemcpyHostToDevice, st));
-	} else {
-		RX_CUDA(ws.d_ub_list.ensure(size_t(nqPad) * kTcMaxK1));
-		RX_CUDA(ws.d_ub_lock.ensure(nqPad));
-		RX_CUDA(raiseSmemCeilingOnce(tc_init_tau, ix->device, int(tc_init_smem_bytes(2048))));
-		tc_init_tau<<<(nq + kTcInitQ - 1) / kTcInitQ, 256, tc_init_smem_bytes(ix->pitch), st>>>(
-			ix->d_rows, ix->pitch, ix->dim, ix->metric == RXGPU_COS ? ix->d_norms : nullptr, uint32_t(std::min<uint64_t>(ix->size, kTcInitRows)),
-			d_queries, nq, k1, ix->metric, ws.d_tau.p, ws.d_ub_list.p, ws.d_ub_lock.p);
-		g_stats.launches += 1;
-	}
-	RX_CUDA(cudaMemsetAsync(ws.d_cand_count.p, 0, size_t(nqPad) * 4, st));
 	RX_CUDA(cudaGetLastError());
-	CUtensorMap mapQ;
-	if (int rc = makeCodeMap(&mapQ, ws.d_qcodes.p, pitchQ, nqPad, nqb)) {
+	if (int rc = makeCodeMap(&b.mapQ, ws.d_qcodes.p, pitchQ, nqPad, nqb)) {
 		return rc;
 	}
-	const TcKernel kfn = tcKernel(nqb, cluster);
-	RX_CUDA(raiseSmemCeilingOnce(kfn, ix->device, int(kTcSmemLimit)));
+	b.kfn = tcKernel(nqb, cluster);
+	RX_CUDA(raiseSmemCeilingOnce(b.kfn, ix->device, int(kTcSmemLimit)));
 	cudaLaunchConfig_t cfg{};
 	cfg.gridDim = dim3(unsigned(ix->sm_count) / cluster * cluster);
+	cfg.blockDim = dim3(kTcThreads);
+	cfg.dynamicSmemBytes = tc_smem_bytes(nqb, kchunks);
+	cudaLaunchAttribute attr[1];
+	attr[0].id = cudaLaunchAttributeClusterDimension;
+	attr[0].val.clusterDim.x = cluster;
+	attr[0].val.clusterDim.y = 1;
+	attr[0].val.clusterDim.z = 1;
+	cfg.attrs = attr;
+	cfg.numAttrs = 1;
+	b.resident = 0;  // GPC boundaries can strand SMs for clusters: ask how many fit at once
+	RX_CUDA(cudaOccupancyMaxActiveClusters(&b.resident, b.kfn, &cfg));
+	if (b.resident < 1) {
+		return fail(RXGPU_ERR_SYSTEM, "rxgpu: tensor-core filter kernel cannot be made resident");
+	}
+	b.nq = nq;
+	b.nqb = nqb;
+	b.cluster = cluster;
+	b.ngroups = ngroups;
+	b.nqPad = nqPad;
+	b.kchunks = kchunks;
+	return 0;
+}
+
+// The filter launches of a prepared batch over the rows [0, nrows), with the thresholds already in ws.d_tau: the rows whose certified
+// lower bound is at or below the query's threshold tau go to ws.d_cand_rows[q][candCap], and ws.d_cand_count[q] counts them all (also
+// past candCap: an overflowed list).  fixedTau: init_rows = UINT32_MAX keeps every row out of the bound list, so tau never moves
+// (knn_tc.cuh header comment) and k1 is not used; otherwise tau tightens to the k1-th best upper bound from tc_init_tau's list.
+int tcLaunch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const TcBatch& b, uint32_t k1, uint32_t candCap, uint32_t nrows, bool fixedTau) {
+	const uint32_t nq = b.nq, nqb = b.nqb, cluster = b.cluster, ngroups = b.ngroups, kchunks = b.kchunks, pitchQ = ix->pitch_q;
+	const uint32_t ntiles = (nrows + kTcTileRows - 1) / kTcTileRows;
+	const int resident = b.resident;
+	const TcKernel kfn = b.kfn;
+	const CUtensorMap mapQ = b.mapQ;
+	RX_CUDA(cudaMemsetAsync(ws.d_cand_count.p, 0, size_t(b.nqPad) * 4, st));
+	RX_CUDA(cudaGetLastError());
+	cudaLaunchConfig_t cfg{};
 	cfg.blockDim = dim3(kTcThreads);
 	cfg.dynamicSmemBytes = tc_smem_bytes(nqb, kchunks);
 	cfg.stream = st;
@@ -392,23 +427,18 @@ int tcFilter(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float*
 	attr[0].val.clusterDim.z = 1;
 	cfg.attrs = attr;
 	cfg.numAttrs = 1;
-	int resident = 0;  // GPC boundaries can strand SMs for clusters: ask how many fit at once
-	RX_CUDA(cudaOccupancyMaxActiveClusters(&resident, kfn, &cfg));
-	if (resident < 1) {
-		return fail(RXGPU_ERR_SYSTEM, "rxgpu: tensor-core filter kernel cannot be made resident");
-	}
 	TcArgs a{};
 	a.shadow = static_cast<const unsigned char*>(ix->d_shadow);
 	a.rowc = ix->d_rowc;
 	a.qc = ws.d_qc.p;
 	a.tau = ws.d_tau.p;
-	a.ub_list = h_tau ? nullptr : ws.d_ub_list.p;
-	a.ub_lock = h_tau ? nullptr : ws.d_ub_lock.p;
-	a.init_rows = h_tau ? UINT32_MAX : uint32_t(std::min<uint64_t>(ix->size, kTcInitRows));
+	a.ub_list = fixedTau ? nullptr : ws.d_ub_list.p;
+	a.ub_lock = fixedTau ? nullptr : ws.d_ub_lock.p;
+	a.init_rows = fixedTau ? UINT32_MAX : uint32_t(std::min<uint64_t>(ix->size, kTcInitRows));
 	a.cand_rows = ws.d_cand_rows.p;
 	a.cand_count = ws.d_cand_count.p;
 	a.cand_cap = candCap;
-	a.n = uint32_t(ix->size);
+	a.n = nrows;
 	a.dim = ix->dim;
 	a.kchunks = kchunks;
 	a.nq_total = nq;
@@ -439,12 +469,135 @@ int tcFilter(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float*
 		g_stats.launches += 1;
 		g_stats.passes += 1;
 		const uint32_t served = std::min(groups * cluster * nqb, nq - a.q0);  // queries of this launch, padding excluded
-		g_stats.algorithmic_bytes += uint64_t(ix->size) * pitchQ + uint64_t(ix->size) * sizeof(float4) + uint64_t(served) * pitchQ;
+		g_stats.algorithmic_bytes += uint64_t(nrows) * pitchQ + uint64_t(nrows) * sizeof(float4) + uint64_t(served) * pitchQ;
 		g0 += groups;
 	}
 	g_stats.tc_cluster = cluster;
 	g_stats.tc_kernel = 1;
 	g_stats.query_tile = nqb * cluster;
+	return 0;
+}
+
+// The candidate filter over a whole batch and all rows.  KNN (h_tau == nullptr): tau starts from tc_init_tau and tightens to the k1-th
+// best upper bound.  Range search: h_tau[q] = float_ord(radius) fixes tau.
+int tcFilter(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1, uint32_t candCap,
+			 const unsigned int* h_tau) {
+	TcBatch b;
+	if (int rc = tcPrepare(ix, ws, st, d_queries, nq, candCap, b)) {
+		return rc;
+	}
+	if (h_tau) {
+		RX_CUDA(cudaMemcpyAsync(ws.d_tau.p, h_tau, size_t(nq) * 4, cudaMemcpyHostToDevice, st));
+	} else {
+		RX_CUDA(ws.d_ub_list.ensure(size_t(b.nqPad) * kTcMaxK1));
+		RX_CUDA(ws.d_ub_lock.ensure(b.nqPad));
+		RX_CUDA(raiseSmemCeilingOnce(tc_init_tau, ix->device, int(tc_init_smem_bytes(2048))));
+		tc_init_tau<<<(nq + kTcInitQ - 1) / kTcInitQ, 256, tc_init_smem_bytes(ix->pitch), st>>>(
+			ix->d_rows, ix->pitch, ix->dim, ix->metric == RXGPU_COS ? ix->d_norms : nullptr, uint32_t(std::min<uint64_t>(ix->size, kTcInitRows)),
+			d_queries, nq, k1, ix->metric, ws.d_tau.p, ws.d_ub_list.p, ws.d_ub_lock.p);
+		g_stats.launches += 1;
+	}
+	return tcLaunch(ix, ws, st, b, k1, candCap, uint32_t(ix->size), h_tau != nullptr);
+}
+
+// knn_rerank's range mode over the candidate lists: CTA b keeps the candidates of query q = qsel[b] (b without qsel) with
+// dist < radius[q] as make_key(dist, row) in keys[q][cap], counted in nkeys[q] (zeroed here)
+int rerankRange(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t nctas, const uint32_t* d_qsel,
+				uint32_t cap, const float* d_radius, uint64_t* d_keys, unsigned int* d_nkeys) {
+	RX_CUDA(cudaMemsetAsync(d_nkeys, 0, size_t(nq) * 4, st));
+	const size_t rsmem = size_t((ix->dim + 127) / 128) * 512 + size_t(kScanWarps) * (1 + kCandBuf) * 8;
+	const float* norms = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
+	if (ix->metric == RXGPU_L2) {
+		RX_CUDA(raiseSmemCeilingOnce(knn_rerank<true>, ix->device, kScanSmemBudget));
+		knn_rerank<true><<<nctas, kScanThreads, rsmem, st>>>(ix->d_rows, ix->pitch, ix->dim, norms, d_queries, ws.d_cand_rows.p, ws.d_cand_count.p,
+															  cap, 1, nullptr, d_qsel, nullptr, d_radius, d_keys, d_nkeys);
+	} else {
+		RX_CUDA(raiseSmemCeilingOnce(knn_rerank<false>, ix->device, kScanSmemBudget));
+		knn_rerank<false><<<nctas, kScanThreads, rsmem, st>>>(ix->d_rows, ix->pitch, ix->dim, norms, d_queries, ws.d_cand_rows.p, ws.d_cand_count.p,
+															   cap, 1, nullptr, d_qsel, nullptr, d_radius, d_keys, d_nkeys);
+	}
+	RX_CUDA(cudaGetLastError());
+	g_stats.launches += 1;
+	return 0;
+}
+
+// KNN with k1 in (kTcMaxK1, kTcStagedMaxK1] on the filter, by staged exact thresholds (knn_tc.cuh, DESIGN 3.2).  Output = the same
+// top-k1 under (dist, internal index) as scanTopKExact, bit for bit.  The thresholds stay on the device between the stages; the batch
+// synchronises with the host once, at the end.
+int scanTopKStaged(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1,
+				   float* d_out_dist, uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count) {
+	const uint32_t cap = stageCandCap(k1);
+	const uint32_t size = uint32_t(ix->size);
+	TcBatch b;
+	if (int rc = tcPrepare(ix, ws, st, d_queries, nq, cap, b)) {
+		return rc;
+	}
+	RX_CUDA(ws.d_radius.ensure(nq));
+	RX_CUDA(ws.d_range_n.ensure(nq));
+	RX_CUDA(ws.d_range.ensure(size_t(nq) * cap));
+	RX_CUDA(ws.d_stage_status.ensure(nq));
+	RX_CUDA(ws.h_stage_status.ensure(nq));
+	RX_CUDA(ws.d_reranked.ensure(1));
+	RX_CUDA(ws.h_reranked.ensure(1));
+	RX_CUDA(cudaMemsetAsync(ws.d_reranked.p, 0, sizeof(unsigned long long), st));
+	// the seed: the exact top-k1 of a prefix, in the output arrays (the last stage or the exact scan overwrites every query's)
+	uint32_t rows = std::min(size, stageSeedRows(k1));
+	if (int rc = scanTopKExact(ix, ws, st, d_queries, nq, k1, kModeTopK, 0.f, d_out_dist, d_out_idx, d_out_label, d_out_count, rows)) {
+		return rc;
+	}
+	knn_seed_tau<<<(nq + 255) / 256, 256, 0, st>>>(d_out_dist, d_out_count, k1, nq, ws.d_tau.p, ws.d_radius.p, ws.d_stage_status.p);
+	RX_CUDA(cudaGetLastError());
+	g_stats.launches += 1;
+	SelectArgs s{};
+	s.keys = ws.d_range.p;
+	s.nkeys = ws.d_range_n.p;
+	s.cand_count = ws.d_cand_count.p;
+	s.labels = ix->d_labels;
+	s.cap = cap;
+	s.k1 = k1;
+	s.mode = kModeTopK;
+	s.tau = ws.d_tau.p;
+	s.radius = ws.d_radius.p;
+	s.status = ws.d_stage_status.p;
+	s.reranked = ws.d_reranked.p;
+	s.out_dist = d_out_dist;
+	s.out_idx = d_out_idx;
+	s.out_label = d_out_label;
+	s.out_count = d_out_count;
+	do {
+		rows = uint32_t(std::min<uint64_t>(size, uint64_t(rows) * kStageRatio));
+		if (int rc = tcLaunch(ix, ws, st, b, k1, cap, rows, true)) {
+			return rc;
+		}
+		if (int rc = rerankRange(ix, ws, st, d_queries, nq, nq, nullptr, cap, ws.d_radius.p, ws.d_range.p, ws.d_range_n.p)) {
+			return rc;
+		}
+		s.last = rows == size;
+		knn_select_topk<<<nq, kSelThreads, 0, st>>>(s);
+		RX_CUDA(cudaGetLastError());
+		g_stats.launches += 1;
+	} while (rows < size);
+	RX_CUDA(cudaMemcpyAsync(ws.h_cand_count.p, ws.d_cand_count.p, size_t(nq) * 4, cudaMemcpyDeviceToHost, st));
+	RX_CUDA(cudaMemcpyAsync(ws.h_stage_status.p, ws.d_stage_status.p, size_t(nq) * 4, cudaMemcpyDeviceToHost, st));
+	RX_CUDA(cudaMemcpyAsync(ws.h_reranked.p, ws.d_reranked.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+	RX_CUDA(cudaStreamSynchronize(st));
+	for (uint32_t q = 0; q < nq; ++q) {
+		if (ws.h_stage_status.p[q]) {  // an overflowed last list, a non-finite threshold or too few survivors: the exact scan answers
+			g_stats.tc_fallbacks += 1;
+			ws.h_cand_count.p[q] = UINT32_MAX;  // and no tie replay reads its list
+			if (int rc = scanTopKExact(ix, ws, st, d_queries + size_t(q) * ix->dim, 1, k1, kModeTopK, 0.f, d_out_dist + size_t(q) * k1,
+									   d_out_idx + size_t(q) * k1, d_out_label ? d_out_label + size_t(q) * k1 : nullptr, d_out_count + q)) {
+				return rc;
+			}
+		}
+	}
+	ws.tc_lists_valid = true;
+	ws.tc_lists_nq = nq;
+	ws.tc_lists_cap = cap;
+	ws.tc_lists_version = ix->version;
+	g_stats.tc_used = 1;
+	g_stats.tc_candidates = *ws.h_reranked.p;
+	g_stats.algorithmic_bytes += *ws.h_reranked.p * (uint64_t(ix->dim) * 4 + 4);
 	return 0;
 }
 
@@ -515,6 +668,9 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 namespace rxgpu {
 int scanTopK(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1, int mode, float bound,
 			 float* d_out_dist, uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count) {
+	if (tcEligible(ix, nq, k1, mode) && k1 > kTcMaxK1) {
+		return scanTopKStaged(ix, ws, st, d_queries, nq, k1, d_out_dist, d_out_idx, d_out_label, d_out_count);
+	}
 	if (tcEligible(ix, nq, k1, mode)) {
 		return scanTopKTensorCore(ix, ws, st, d_queries, nq, k1, d_out_dist, d_out_idx, d_out_label, d_out_count);
 	}
@@ -565,7 +721,7 @@ int tieRowsAfterScan(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, cons
 	if (nsel == 0) {
 		return 0;
 	}
-	bool fromLists = ws.tc_lists_valid && ws.tc_lists_version == ix->version && k <= kTcMaxK1;
+	bool fromLists = ws.tc_lists_valid && ws.tc_lists_version == ix->version && k < kTcStagedMaxK1;
 	for (uint32_t i = 0; fromLists && i < nsel; ++i) {  // a query whose list overflowed was answered by the exact scan: no list
 		fromLists = sel[i] < ws.tc_lists_nq && ws.h_cand_count.p[sel[i]] <= ws.tc_lists_cap;
 	}
@@ -580,9 +736,44 @@ int tieRowsAfterScan(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, cons
 		return 0;
 	}
 	RX_CUDA(ws.d_sel.ensure(nsel));
+	RX_CUDA(cudaMemcpyAsync(ws.d_sel.p, sel, size_t(nsel) * 4, cudaMemcpyHostToDevice, st));
+	if (k > kTcMaxK1) {
+		// the lists of staged thresholds: the candidates with dist <= d* (range mode, radius = the next float above d*), then the first k
+		// of them in internal order (knn_select_topk on row-major keys)
+		const uint32_t nq = ws.tc_lists_nq, cap = ws.tc_lists_cap;
+		std::vector<float> rad(nq, -INFINITY);
+		for (uint32_t i = 0; i < nsel; ++i) {
+			rad[sel[i]] = nextafterf(dstar[i], INFINITY);
+		}
+		RX_CUDA(ws.d_radius.ensure(nq));
+		RX_CUDA(ws.d_range_n.ensure(nq));
+		RX_CUDA(ws.d_range.ensure(size_t(nq) * cap));
+		RX_CUDA(cudaMemcpyAsync(ws.d_radius.p, rad.data(), size_t(nq) * 4, cudaMemcpyHostToDevice, st));
+		if (int rc = rerankRange(ix, ws, st, d_queries, nq, nsel, ws.d_sel.p, cap, ws.d_radius.p, ws.d_range.p, ws.d_range_n.p)) {
+			return rc;
+		}
+		SelectArgs s{};
+		s.keys = ws.d_range.p;
+		s.nkeys = ws.d_range_n.p;
+		s.cand_count = ws.d_cand_count.p;
+		s.qsel = ws.d_sel.p;
+		s.labels = ix->d_labels;
+		s.cap = cap;
+		s.k1 = k;
+		s.mode = kModeTieRows;
+		s.out_dist = d_out_dist;
+		s.out_idx = d_out_idx;
+		s.out_label = d_out_label;
+		s.out_count = d_out_count;
+		knn_select_topk<<<nsel, kSelThreads, 0, st>>>(s);
+		RX_CUDA(cudaGetLastError());
+		g_stats.launches += 1;
+		g_stats.tie_replays += nsel;
+		g_stats.tie_from_lists += nsel;
+		return 0;
+	}
 	RX_CUDA(ws.d_selbound.ensure(nsel));
 	RX_CUDA(ws.d_lists.ensure(size_t(nsel) * k));
-	RX_CUDA(cudaMemcpyAsync(ws.d_sel.p, sel, size_t(nsel) * 4, cudaMemcpyHostToDevice, st));
 	RX_CUDA(cudaMemcpyAsync(ws.d_selbound.p, dstar, size_t(nsel) * 4, cudaMemcpyHostToDevice, st));
 	const size_t rsmem = size_t((ix->dim + 127) / 128) * 512 + size_t(kScanWarps) * (k + kCandBuf) * 8;
 	const float* norms = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
@@ -1352,22 +1543,9 @@ static int searchRangeBatchHost(const rxgpu_index* ix, uint32_t nq, const float*
 		RX_CUDA(ws.h_range_n.ensure(nq));
 		RX_CUDA(ws.d_range.ensure(size_t(nq) * cap));
 		RX_CUDA(cudaMemcpyAsync(ws.d_radius.p, rad.data(), size_t(nq) * 4, cudaMemcpyHostToDevice, st));
-		RX_CUDA(cudaMemsetAsync(ws.d_range_n.p, 0, size_t(nq) * 4, st));
-		const size_t rsmem = size_t((ix->dim + 127) / 128) * 512 + size_t(kScanWarps) * (1 + kCandBuf) * 8;
-		const float* norms = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
-		if (ix->metric == RXGPU_L2) {
-			RX_CUDA(raiseSmemCeilingOnce(knn_rerank<true>, ix->device, kScanSmemBudget));
-			knn_rerank<true><<<nq, kScanThreads, rsmem, st>>>(ix->d_rows, ix->pitch, ix->dim, norms, ws.d_queries.p, ws.d_cand_rows.p,
-															   ws.d_cand_count.p, cap, 1, nullptr, nullptr, nullptr, ws.d_radius.p,
-															   ws.d_range.p, ws.d_range_n.p);
-		} else {
-			RX_CUDA(raiseSmemCeilingOnce(knn_rerank<false>, ix->device, kScanSmemBudget));
-			knn_rerank<false><<<nq, kScanThreads, rsmem, st>>>(ix->d_rows, ix->pitch, ix->dim, norms, ws.d_queries.p, ws.d_cand_rows.p,
-																ws.d_cand_count.p, cap, 1, nullptr, nullptr, nullptr, ws.d_radius.p,
-																ws.d_range.p, ws.d_range_n.p);
+		if (int rc = rerankRange(ix, ws, st, ws.d_queries.p, nq, nq, nullptr, cap, ws.d_radius.p, ws.d_range.p, ws.d_range_n.p)) {
+			return rc;
 		}
-		RX_CUDA(cudaGetLastError());
-		g_stats.launches += 1;
 		RX_CUDA(cudaMemcpyAsync(ws.h_cand_count.p, ws.d_cand_count.p, size_t(nq) * 4, cudaMemcpyDeviceToHost, st));
 		RX_CUDA(cudaMemcpyAsync(ws.h_range_n.p, ws.d_range_n.p, size_t(nq) * 4, cudaMemcpyDeviceToHost, st));
 		RX_CUDA(cudaStreamSynchronize(st));

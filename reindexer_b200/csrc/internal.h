@@ -141,6 +141,10 @@ struct Workspace {
 	DevBuf<float> d_ub_list;
 	DevBuf<uint32_t> d_cand_rows;
 	PinBuf<unsigned int> h_cand_count;
+	DevBuf<unsigned int> d_stage_status;  // KNN with staged thresholds: per-query fallback status, and the candidates re-ranked
+	PinBuf<unsigned int> h_stage_status;
+	DevBuf<unsigned long long> d_reranked;
+	PinBuf<unsigned long long> h_reranked;
 	PinBuf<float> h_queries;
 	PinBuf<float> h_out_dist;
 	PinBuf<uint32_t> h_out_idx;
@@ -148,7 +152,8 @@ struct Workspace {
 	PinBuf<uint32_t> h_out_count;
 	PinBuf<uint64_t> h_range;
 	// state of the last scanTopK on this workspace: when the tensor-core filter answered it, the per-query candidate lists
-	// (d_cand_rows / h_cand_count) hold every row at or below each query's k1-th distance -- tieRowsAfterScan reads them
+	// (d_cand_rows / h_cand_count; the last stage's with staged thresholds) hold every row at or below each query's k1-th distance --
+	// tieRowsAfterScan reads them
 	bool tc_lists_valid = false;
 	uint32_t tc_lists_nq = 0;
 	uint32_t tc_lists_cap = 0;  // entries per query list of that call

@@ -62,7 +62,7 @@ constexpr int kTcChunkK = 128;       // int8 codes per 128-byte swizzle row
 constexpr int kTcStages = 6;         // stages per consumer warpgroup ring
 constexpr int kTcBlockBytes = 64 * kTcChunkK;               // 8 KB: one 64-row shadow block of one K chunk = one stage
 constexpr uint32_t kTcMaxNq = 128;   // queries per CTA (wgmma N <= 128 keeps the accumulators at <= 64 registers per thread)
-constexpr uint32_t kTcMaxK1 = 128;  // k + 1 <= 128: the bound list is scanned linearly under the per-query lock
+constexpr uint32_t kTcMaxK1 = 128;  // k + 1 <= 128: the bound list is scanned linearly under the per-query lock (larger k: staged)
 constexpr float kTcL2Eps = 1e-5f;
 
 struct TcArgs {
@@ -686,6 +686,195 @@ __global__ void __launch_bounds__(kScanThreads) knn_rerank(const float* rows, ui
 			last = best;
 			first = false;
 		}
+	}
+}
+
+// ---- staged exact thresholds (k1 > kTcMaxK1) ---------------------------------------------------------------------------------------
+// Any k1 rows give a valid threshold: their k1-th best exact distance is at least the k1-th best over all rows.  The seed is the exact
+// top-k1 over a short prefix of the rows; stage s then runs the filter with that fixed threshold over a prefix r times longer, re-ranks
+// the candidates with knn_rerank's range mode (radius = the next float above tau: it keeps exactly dist <= tau) and takes the k1-th
+// best survivor as the next threshold.  The last stage covers every row; its k1 best survivors are the exact answer.
+constexpr uint32_t kTcStagedMaxK1 = 1024;  // k + 1 <= 1024: the staged path's limit
+constexpr int kSelThreads = 512;
+constexpr uint32_t kSelSort = 4096;        // keys sorted in shared memory by knn_select_topk
+
+// per-query stage status: 0 = the filter decides the query, 1 = it falls back to the exact scan (and admits nothing in later stages)
+__global__ void knn_seed_tau(const float* seed_dist, const uint32_t* seed_count, uint32_t k1, uint32_t nq, unsigned int* tau, float* radius,
+							 unsigned int* status) {
+	const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+	if (q >= nq) {
+		return;
+	}
+	// a non-finite k1-th distance of the prefix (rows of infinite or NaN distance) would admit every row: the exact scan answers
+	const float t = seed_count[q] >= k1 ? seed_dist[size_t(q) * k1 + k1 - 1] : NAN;
+	const bool ok = isfinite(t);
+	tau[q] = float_ord(ok ? t : -INFINITY);
+	radius[q] = ok ? nextafterf(t, INFINITY) : -INFINITY;
+	status[q] = ok ? 0u : 1u;
+}
+
+struct SelectArgs {
+	const uint64_t* keys;          // [nq][cap] unordered make_key(dist, row) of knn_rerank's range mode
+	const unsigned int* nkeys;     // [nq] keys per region
+	const unsigned int* cand_count;  // [nq] the filter's candidate counts (> cap: the list overflowed)
+	const uint32_t* qsel;          // CTA b serves query qsel[b], or nullptr (CTA b serves query b)
+	const uint64_t* labels;
+	uint32_t cap;
+	uint32_t k1;
+	int mode;                      // kModeTopK: the k1 smallest (dist, row); kModeTieRows: the k1 first rows in internal order
+	int last;                      // kModeTopK: the last stage writes the results and decides the fallbacks
+	unsigned int* tau;             // kModeTopK: [nq] the next stage's threshold (ordered uint) and radius
+	float* radius;
+	unsigned int* status;          // kModeTopK: [nq] knn_seed_tau's status
+	unsigned long long* reranked;  // kModeTopK: += the candidates re-ranked
+	float* out_dist;               // [CTA][k1] (kModeTopK: written by the last stage)
+	uint32_t* out_idx;
+	uint64_t* out_label;           // may be null
+	uint32_t* out_count;
+};
+
+// One CTA per query: the k1 smallest of the query's unordered key region, ascending, in time linear in the region.  A radix select on
+// 8-bit digits from the top narrows the keys at or below the k1-th to at most kSelSort (keys are unique, so the last digit always
+// does), a bitonic sort in shared memory orders them.  Tie mode selects on row-major keys (row << 32 | ord(dist)).
+__global__ void __launch_bounds__(kSelThreads) knn_select_topk(const SelectArgs a) {
+	__shared__ uint64_t s_keys[kSelSort];
+	__shared__ uint32_t s_hist[256];
+	__shared__ uint64_t s_prefix, s_bound;
+	__shared__ uint32_t s_below, s_n;
+	const uint32_t b = blockIdx.x, q = a.qsel ? a.qsel[b] : b;
+	const bool tie = a.mode == kModeTieRows;
+	const int lane = threadIdx.x & 31;
+	if (!tie) {
+		if (threadIdx.x == 0) {
+			atomicAdd(a.reranked, (unsigned long long)min(a.cand_count[q], a.cap));
+		}
+		if (a.status[q]) {  // settled as a fallback: admits nothing from now on
+			if (threadIdx.x == 0) {
+				a.tau[q] = float_ord(-INFINITY);
+				a.radius[q] = -INFINITY;
+			}
+			return;
+		}
+	}
+	const uint32_t n = min(a.nkeys[q], a.cap);
+	const uint64_t* src = a.keys + size_t(q) * a.cap;
+	auto load = [&](uint32_t i) {
+		const uint64_t k = src[i];
+		return tie ? (k << 32) | (k >> 32) : k;
+	};
+	// whole warps walk the region (the histogram aggregates equal digits of a warp with one shared atomic)
+	const uint32_t span = (n + kSelThreads - 1) / kSelThreads * kSelThreads;
+	if (threadIdx.x == 0) {
+		s_bound = kKeyNone;
+		s_prefix = 0;
+		s_below = 0;
+		s_n = 0;
+	}
+	__syncthreads();
+	if (n > kSelSort) {
+		for (int sh = 56; sh >= 0; sh -= 8) {
+			const uint64_t hi = sh == 56 ? 0ull : ~0ull << (sh + 8);  // the digits already fixed
+			const uint64_t prefix = s_prefix;
+			for (uint32_t i = threadIdx.x; i < 256; i += kSelThreads) {
+				s_hist[i] = 0;
+			}
+			__syncthreads();
+			for (uint32_t i = threadIdx.x; i < span; i += kSelThreads) {
+				const uint64_t k = i < n ? load(i) : 0ull;
+				const bool in = i < n && (k & hi) == prefix;
+				const uint32_t d = in ? uint32_t(k >> sh) & 0xFFu : 0x100u;
+				const unsigned peers = __match_any_sync(0xffffffffu, d);
+				if (in && lane == __ffs(peers) - 1) {
+					atomicAdd(&s_hist[d], uint32_t(__popc(peers)));
+				}
+			}
+			__syncthreads();
+			if (threadIdx.x == 0) {  // the digit of the k1-th key: below + (keys of smaller digits) < k1 <= ... + (keys of this digit)
+				const uint32_t need = a.k1 - s_below;
+				uint32_t cum = 0, d = 0;
+				while (cum + s_hist[d] < need) {
+					cum += s_hist[d++];
+				}
+				s_prefix = prefix | (uint64_t(d) << sh);
+				s_below += cum;
+				if (s_below + s_hist[d] <= kSelSort) {
+					s_bound = s_prefix | ((1ull << sh) - 1ull);
+				}
+			}
+			__syncthreads();
+			if (s_bound != kKeyNone) {
+				break;
+			}
+		}
+	}
+	const uint64_t bound = s_bound;
+	for (uint32_t i = threadIdx.x; i < span; i += kSelThreads) {  // gather the keys at or below the bound
+		const uint64_t k = i < n ? load(i) : kKeyNone;
+		const bool take = i < n && k <= bound;
+		const unsigned m = __ballot_sync(0xffffffffu, take);
+		uint32_t base = 0;
+		if (lane == 0 && m) {
+			base = atomicAdd(&s_n, uint32_t(__popc(m)));
+		}
+		base = __shfl_sync(0xffffffffu, base, 0);
+		if (take) {
+			s_keys[base + __popc(m & ((1u << lane) - 1u))] = k;
+		}
+	}
+	__syncthreads();
+	const uint32_t cnt = s_n;
+	uint32_t p2 = 1;
+	while (p2 < cnt) {
+		p2 <<= 1;
+	}
+	for (uint32_t i = cnt + threadIdx.x; i < p2; i += kSelThreads) {
+		s_keys[i] = kKeyNone;
+	}
+	__syncthreads();
+	for (uint32_t size = 2; size <= p2; size <<= 1) {  // bitonic sort, ascending
+		for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+			for (uint32_t t = threadIdx.x; t < p2 / 2; t += kSelThreads) {
+				const uint32_t i = 2 * t - (t & (stride - 1)), j = i + stride;
+				const bool up = (i & size) == 0;
+				const uint64_t x = s_keys[i], y = s_keys[j];
+				if ((x > y) == up) {
+					s_keys[i] = y;
+					s_keys[j] = x;
+				}
+			}
+			__syncthreads();
+		}
+	}
+	const uint32_t m = min(cnt, a.k1);
+	if (!tie) {
+		// fewer than k1 survivors (an overflowed list of an earlier stage): the threshold stays, it is still valid
+		if (!a.last) {
+			if (threadIdx.x == 0 && m == a.k1) {
+				const float t = ord_float(uint32_t(s_keys[m - 1] >> 32));
+				a.tau[q] = float_ord(t);
+				a.radius[q] = nextafterf(t, INFINITY);
+			}
+			return;
+		}
+		if (m < a.k1 || a.cand_count[q] > a.cap) {
+			if (threadIdx.x == 0) {
+				a.status[q] = 1u;
+			}
+			return;
+		}
+	}
+	const size_t ob = size_t(b) * a.k1;
+	for (uint32_t r = threadIdx.x; r < m; r += kSelThreads) {
+		const uint64_t k = s_keys[r];
+		const uint32_t idx = tie ? uint32_t(k >> 32) : uint32_t(k);
+		a.out_dist[ob + r] = ord_float(tie ? uint32_t(k) : uint32_t(k >> 32));
+		a.out_idx[ob + r] = idx;
+		if (a.out_label) {
+			a.out_label[ob + r] = a.labels[idx];
+		}
+	}
+	if (threadIdx.x == 0) {
+		a.out_count[b] = m;
 	}
 }
 
