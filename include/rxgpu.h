@@ -145,7 +145,7 @@ int rxgpu_comm_create(rxgpu_comm** out, int nranks, int rank, const void* id /* 
 /* the ranks of ONE process (a reindexer process that drives several GPUs: one host thread per rank; the devices may repeat, which is
  * how a one-GPU box exercises the cross-shard paths): out[0..nranks) receive the communicators, rank r on devices[r] (NULL = all on
  * device 0).  Their exchanges go through host memory behind a rendezvous; every rank must make the same collective calls, each from its
- * own thread.  Serves rxgpu_sharded_ft_select; rxgpu_sharded_search_knn exchanges over NCCL only. */
+ * own thread.  Serves rxgpu_sharded_search_knn, rxgpu_sharded_search_range_batch and rxgpu_sharded_ft_select. */
 int rxgpu_comm_create_local(rxgpu_comm** out, int nranks, const int* devices);
 void rxgpu_comm_destroy(rxgpu_comm*);
 int rxgpu_comm_rank(const rxgpu_comm*);
@@ -155,6 +155,15 @@ int rxgpu_comm_size(const rxgpu_comm*);
  * applied globally; out_count[q] = min(k, total rows). */
 int rxgpu_sharded_search_knn(rxgpu_comm*, const rxgpu_index* shard, uint32_t nq, const float* queries, int queries_on_device, uint32_t k,
 							 float* out_dist, uint64_t* out_label, uint32_t* out_count);
+/* collective: every rank calls it with its own shard and the SAME queries / radius / max_out.  Per query q the result on EVERY rank is
+ * identical to rxgpu_search_range_batch on one index holding the rows of all shards: out_n[q] = total matches over all shards, and the
+ * best min(out_n[q], max_out) matches, best first in the order of hitLessByLabel (distance, then label), go into row q of
+ * out_dist / out_label (nq x max_out, host); the rest of a row may be overwritten.  queries: host (queries_on_device == 0) or device
+ * pointer on the shard's GPU; radius: host, map space.  Labels must be unique across the shards (they are the rows of one namespace).
+ * Each shard runs rxgpu_search_range_batch's local part (filter or exact scan, its own choice); the ranks then all-reduce the totals,
+ * all-gather up to min(matches, max_out) best matches per query and shard, and merge them on the device (DESIGN.md §7). */
+int rxgpu_sharded_search_range_batch(rxgpu_comm*, const rxgpu_index* shard, uint32_t nq, const float* queries, int queries_on_device,
+									 const float* radius /* nq */, uint64_t max_out, float* out_dist, uint64_t* out_label, uint64_t* out_n);
 /* the device-side merge alone: d_payloads = nshards contributions of rxgpu_shard_payload_bytes(nq, k1) bytes each, laid out as
  * [dist f32 nq*k1][idx u32 nq*k1][label u64 nq*k1][count u32 nq][shard size u64] (sections 16-byte aligned) -- what
  * rxgpu_search_knn_device writes; outputs (device) as rxgpu_merge_shards, ties NOT yet ordered by label. */

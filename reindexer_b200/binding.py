@@ -126,6 +126,8 @@ _SIGNATURES = {
     "rxgpu_comm_rank": (C.c_int, [C.c_void_p]),
     "rxgpu_comm_size": (C.c_int, [C.c_void_p]),
     "rxgpu_sharded_search_knn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_int, C.c_uint32, _f32p, _u64p, _u32p]),
+    "rxgpu_sharded_search_range_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_int, _f32p, C.c_uint64, _f32p, _u64p,
+                                                   _u64p]),
     "rxgpu_shard_payload_bytes": (C.c_uint64, [C.c_uint32, C.c_uint32]),
     "rxgpu_merge_shards_device": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -561,7 +563,8 @@ def comm_unique_id() -> bytes:
 
 
 class ShardComm:
-    """rxgpu_comm: this rank's end of the NCCL communicator the sharded search exchanges its per-shard lists over."""
+    """rxgpu_comm: this rank's end of the communicator the sharded searches exchange their per-shard lists over (NCCL between
+    processes, or a host rendezvous between the threads of one process: local_group)."""
 
     def __init__(self, nranks: int, rank: int, comm_id: bytes | None, device: int, _handle=None):
         self._lib = lib()
@@ -604,6 +607,23 @@ class ShardComm:
         oc = np.zeros(nq, np.uint32)
         _check(self._lib.rxgpu_sharded_search_knn(self._h, shard._h, nq, qp, on_dev, k, _p(od, _f32p), _p(ol, _u64p), _p(oc, _u32p)))
         return od, ol, oc
+
+    def search_range_batch(self, shard: "GpuBruteforceSearch", queries, radius, max_out: int, nq: int | None = None):
+        """rxgpu_sharded_search_range_batch.  queries: host ndarray [nq, dim] or a device pointer (int) with nq given; radius: a
+        scalar or [nq] (map space).  Returns (dists [nq, max_out], labels [nq, max_out], counts [nq]) as
+        GpuBruteforceSearch.search_range_batch returns them for one index holding every shard's rows.  Collective: every rank calls it."""
+        if isinstance(queries, np.ndarray):
+            q = np.ascontiguousarray(queries, np.float32)
+            nq, qp, on_dev = q.shape[0], q.ctypes.data_as(C.c_void_p), 0
+        else:
+            qp, on_dev = C.c_void_p(int(queries)), 1
+        r = np.ascontiguousarray(np.broadcast_to(np.asarray(radius, dtype=np.float32), (nq,)))
+        od = np.zeros((nq, max(max_out, 1)), np.float32)
+        ol = np.zeros((nq, max(max_out, 1)), np.uint64)
+        oc = np.zeros(nq, np.uint64)
+        _check(self._lib.rxgpu_sharded_search_range_batch(self._h, shard._h, nq, qp, on_dev, _p(r, _f32p), max_out, _p(od, _f32p),
+                                                          _p(ol, _u64p), _p(oc, _u64p)))
+        return od[:, :max_out], ol[:, :max_out], oc
 
 
 def select_postprocess(metric, dist, label, k=None, has_radius=False, need_sort=True, is_array=False, raw=False):

@@ -1490,40 +1490,17 @@ static int searchRangeHost(const rxgpu_index* ix, const float* query, float radi
 	return 0;
 }
 
-// Range search for a batch (rxgpu_search_range_batch).  A batch the filter serves (tcServes) runs one filter pass with tau = radius,
-// then the range mode of knn_rerank keeps the candidates with dist < radius -- the same set and distance bits as the exact range
-// scan, which answers every other query.
-static int searchRangeBatchHost(const rxgpu_index* ix, uint32_t nq, const float* queries, const float* radius, uint64_t max_out,
-								float* out_dist, uint64_t* out_label, uint64_t* out_n) {
-	g_stats = rxgpu_search_stats{};
+}  // extern "C"
+
+namespace rxgpu {
+// Range search for a batch of device-resident queries on a non-empty index, enqueued on `st`.  A batch the filter serves (tcServes)
+// runs one filter pass with tau = radius, then the range mode of knn_rerank keeps the candidates with dist < radius -- the same set and
+// distance bits as the exact range scan, which answers every other query.  Adds to g_stats.
+int rangeBatch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, const float* radius,
+			   uint64_t max_out, const RangeEmit& emit) {
 	std::vector<Hit> res;
-	auto emit = [&](uint32_t q, const std::vector<Hit>& hits) {  // hits in the order of hitLessByLabel
-		const uint64_t n = std::min<uint64_t>(hits.size(), max_out);
-		for (uint64_t i = 0; i < n; ++i) {
-			out_dist[q * max_out + i] = hits[i].dist;
-			out_label[q * max_out + i] = hits[i].label;
-		}
-		out_n[q] = hits.size();
-	};
 	// dist < radius never holds for a NaN or -inf radius: no matches, no scan.  A +inf radius matches every row: the exact scan.
 	auto filtered = [&](uint32_t q) { return radius[q] > -INFINITY && radius[q] < INFINITY; };
-	if (ix->size == 0) {
-		for (uint32_t q = 0; q < nq; ++q) {
-			emit(q, res);
-		}
-		return 0;
-	}
-	WsLease lease(ix);
-	Workspace& ws = *lease.ws;
-	if (!ws.stream) {
-		RX_CUDA(cudaStreamCreateWithFlags(&ws.stream, cudaStreamNonBlocking));
-	}
-	cudaStream_t st = ws.stream;
-	const size_t qn = size_t(nq) * ix->dim;
-	RX_CUDA(ws.d_queries.ensure(qn));
-	RX_CUDA(ws.h_queries.ensure(qn));
-	std::memcpy(ws.h_queries.p, queries, qn * sizeof(float));
-	RX_CUDA(cudaMemcpyAsync(ws.d_queries.p, ws.h_queries.p, qn * sizeof(float), cudaMemcpyHostToDevice, st));
 	std::vector<uint32_t> exact;  // queries the exact range scan answers
 	if (tcServes(ix, nq)) {
 		const uint32_t cap = tcRangeCap(max_out);
@@ -1534,7 +1511,7 @@ static int searchRangeBatchHost(const rxgpu_index* ix, uint32_t nq, const float*
 			rad[q] = filtered(q) ? radius[q] : -INFINITY;
 			tau[q] = float_ord(rad[q]);
 		}
-		if (int rc = tcFilter(ix, ws, st, ws.d_queries.p, nq, 0, cap, tau.data())) {
+		if (int rc = tcFilter(ix, ws, st, d_queries, nq, 0, cap, tau.data())) {
 			return rc;
 		}
 		ws.tc_lists_valid = false;  // the candidate lists now hold this batch's range candidates: no tie replay may read them
@@ -1543,7 +1520,7 @@ static int searchRangeBatchHost(const rxgpu_index* ix, uint32_t nq, const float*
 		RX_CUDA(ws.h_range_n.ensure(nq));
 		RX_CUDA(ws.d_range.ensure(size_t(nq) * cap));
 		RX_CUDA(cudaMemcpyAsync(ws.d_radius.p, rad.data(), size_t(nq) * 4, cudaMemcpyHostToDevice, st));
-		if (int rc = rerankRange(ix, ws, st, ws.d_queries.p, nq, nq, nullptr, cap, ws.d_radius.p, ws.d_range.p, ws.d_range_n.p)) {
+		if (int rc = rerankRange(ix, ws, st, d_queries, nq, nq, nullptr, cap, ws.d_radius.p, ws.d_range.p, ws.d_range_n.p)) {
 			return rc;
 		}
 		RX_CUDA(cudaMemcpyAsync(ws.h_cand_count.p, ws.d_cand_count.p, size_t(nq) * 4, cudaMemcpyDeviceToHost, st));
@@ -1594,7 +1571,7 @@ static int searchRangeBatchHost(const rxgpu_index* ix, uint32_t nq, const float*
 	}
 	for (const uint32_t q : exact) {
 		if (radius[q] == INFINITY || filtered(q)) {
-			if (int rc = scanRangeExact(ix, ws, st, ws.d_queries.p + size_t(q) * ix->dim, radius[q], res)) {
+			if (int rc = scanRangeExact(ix, ws, st, d_queries + size_t(q) * ix->dim, radius[q], res)) {
 				return rc;
 			}
 		} else {
@@ -1603,6 +1580,42 @@ static int searchRangeBatchHost(const rxgpu_index* ix, uint32_t nq, const float*
 		emit(q, res);
 	}
 	return 0;
+}
+}  // namespace rxgpu
+
+extern "C" {
+
+// rxgpu_search_range_batch: the host queries go to the device, rangeBatch answers them, row q of the output gets query q's answer
+static int searchRangeBatchHost(const rxgpu_index* ix, uint32_t nq, const float* queries, const float* radius, uint64_t max_out,
+								float* out_dist, uint64_t* out_label, uint64_t* out_n) {
+	g_stats = rxgpu_search_stats{};
+	auto emit = [&](uint32_t q, const std::vector<Hit>& hits) {  // hits in the order of hitLessByLabel
+		const uint64_t n = std::min<uint64_t>(hits.size(), max_out);
+		for (uint64_t i = 0; i < n; ++i) {
+			out_dist[q * max_out + i] = hits[i].dist;
+			out_label[q * max_out + i] = hits[i].label;
+		}
+		out_n[q] = hits.size();
+	};
+	if (ix->size == 0) {
+		const std::vector<Hit> none;
+		for (uint32_t q = 0; q < nq; ++q) {
+			emit(q, none);
+		}
+		return 0;
+	}
+	WsLease lease(ix);
+	Workspace& ws = *lease.ws;
+	if (!ws.stream) {
+		RX_CUDA(cudaStreamCreateWithFlags(&ws.stream, cudaStreamNonBlocking));
+	}
+	cudaStream_t st = ws.stream;
+	const size_t qn = size_t(nq) * ix->dim;
+	RX_CUDA(ws.d_queries.ensure(qn));
+	RX_CUDA(ws.h_queries.ensure(qn));
+	std::memcpy(ws.h_queries.p, queries, qn * sizeof(float));
+	RX_CUDA(cudaMemcpyAsync(ws.d_queries.p, ws.h_queries.p, qn * sizeof(float), cudaMemcpyHostToDevice, st));
+	return rangeBatch(ix, ws, st, ws.d_queries.p, nq, radius, max_out, emit);
 }
 
 int rxgpu_search_range(const rxgpu_index* ix, const float* query, float radius, uint64_t max_out, float* out_dist, uint64_t* out_label,

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include <atomic>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -305,6 +306,14 @@ int scanTopK(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float*
 // filter's candidate lists when they exist (no second pass over the rows), else by one kModeTieRows scan per selected query.
 int tieRowsAfterScan(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nsel, const uint32_t* sel,
 					 const float* dstar, uint32_t k, float* d_out_dist, uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count);
+
+// Range search of nq device-resident queries on a non-empty index (the core of rxgpu_search_range_batch, and each shard's part of
+// rxgpu_sharded_search_range_batch).  emit(q, hits) is called once per query with ALL its matches (dist < radius[q], radius on the host)
+// in the order of hitLessByLabel; only the first min(hits, max_out) are ever returned, which sizes the filter's candidate lists.
+struct Hit;  // host/knn_select.h
+using RangeEmit = std::function<void(uint32_t q, const std::vector<Hit>& hits)>;
+int rangeBatch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, const float* radius,
+			   uint64_t max_out, const RangeEmit& emit);
 
 // writes row `idx` (== size: appends) with a new vector and label, keeping the label dictionary consistent (index.cu)
 int setRowAt(rxgpu_index* ix, uint32_t idx, uint64_t label, const float* vec);

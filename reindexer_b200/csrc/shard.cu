@@ -3,6 +3,9 @@
 // device-side k-way merge under the reference's comparator, and -- only when bit-equal distances straddle the k-th place -- the
 // reference's heap tie rule (bruteforce.cc:103-127) replayed globally from the filter's per-query candidate lists (every row at or
 // below the k-th distance is in them, so no shard is scanned a second time) with a second, tiny all-gather.
+// Range batches: each shard answers its part with rxgpu_search_range_batch's core, two all-reduces agree on the totals and on a payload
+// width, one all-gather ships every shard's best min(matches, max_out) per query, and a warp per query merges them under hitLessByLabel.
+// The exchanges go through commAllGather / commAllReduce: NCCL between processes, a host rendezvous between the threads of one process.
 // NCCL is resolved with dlopen at the first rxgpu_comm_* call: librxgpu.so itself keeps loading on a box without NCCL or a GPU.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -144,6 +147,73 @@ __global__ void shard_merge_kernel(const unsigned char* all, uint32_t nshards, u
 	}
 }
 
+// Layout of one rank's contribution to the range exchange (all sections 16-byte aligned), w entries per query:
+//   [dist f32 nq*w][label u64 nq*w][kept u32 nq]
+struct RangeLayout {
+	size_t off_dist, off_label, off_kept, bytes;
+	RangeLayout(uint32_t nq, uint32_t w) {
+		auto up = [](size_t x) { return (x + 15) & ~size_t(15); };
+		const size_t n = size_t(nq) * w;
+		off_dist = 0;
+		off_label = up(n * 4);
+		off_kept = up(off_label + n * 8);
+		bytes = up(off_kept + size_t(nq) * 4);
+	}
+};
+
+// One warp per query: lane s walks shard s's matches, already best first under hitLessByLabel.  Each round writes the warp-wide minimum
+// under that same comparator -- a float compare of the distances (-0 == +0), then the label, which is unique across the shards -- and the
+// owning lane advances, until `width` entries are out or every list is drained.  Row q of the output holds `width` entries; the ones
+// after the answer are zeroed.
+__global__ void range_merge_kernel(const unsigned char* all, uint32_t nshards, uint32_t nq, uint32_t w, RangeLayout lay, uint32_t width,
+								   float* out_dist, uint64_t* out_label) {
+	const uint32_t q = (blockIdx.x * blockDim.x + threadIdx.x) / 32;
+	const int lane = threadIdx.x & 31;
+	if (q >= nq) {
+		return;
+	}
+	const unsigned char* mine = all + size_t(lane) * lay.bytes;
+	const bool have = uint32_t(lane) < nshards;
+	const uint32_t cnt = have ? min(reinterpret_cast<const uint32_t*>(mine + lay.off_kept)[q], w) : 0u;
+	const float* d = reinterpret_cast<const float*>(mine + lay.off_dist) + size_t(q) * w;
+	const uint64_t* lb = reinterpret_cast<const uint64_t*>(mine + lay.off_label) + size_t(q) * w;
+	float* od_row = out_dist + size_t(q) * width;
+	uint64_t* ol_row = out_label + size_t(q) * width;
+	uint32_t head = 0, r = 0;
+	for (; r < width; ++r) {
+		bool valid = head < cnt;
+		float hd = valid ? d[head] : INFINITY;
+		uint64_t hl = valid ? lb[head] : ~0ull;
+		int owner = lane;
+#pragma unroll
+		for (int off = 16; off > 0; off >>= 1) {
+			const float od = __shfl_xor_sync(0xffffffffu, hd, off);
+			const uint64_t ol = __shfl_xor_sync(0xffffffffu, hl, off);
+			const bool ov = __shfl_xor_sync(0xffffffffu, valid, off);
+			const int oo = __shfl_xor_sync(0xffffffffu, owner, off);
+			const bool better = ov && (!valid || od < hd || (!(hd < od) && ol < hl));
+			if (better) {
+				hd = od;
+				hl = ol;
+				valid = ov;
+				owner = oo;
+			}
+		}
+		if (!valid) {
+			break;
+		}
+		if (lane == owner) {
+			od_row[r] = hd;  // the winner's own bits: -0 stays -0
+			ol_row[r] = hl;
+			++head;
+		}
+	}
+	for (uint32_t j = r + uint32_t(lane); j < width; j += 32) {
+		od_row[j] = 0.f;
+		ol_row[j] = 0;
+	}
+}
+
 }  // namespace
 
 // Ranks that live in ONE process (one host thread per rank; the GPUs may differ or be the same): the exchange goes through pinned host
@@ -190,6 +260,9 @@ struct rxgpu_comm {
 	PinBuf<uint8_t> h_m_tie;
 	PinBuf<unsigned char> h_tie_recv;
 	PinBuf<uint64_t> h_size;
+	DevBuf<uint64_t> d_r_n;  // range batch: the per-query totals, then the agreed width (as u32)
+	PinBuf<uint64_t> h_r_n;
+	PinBuf<unsigned char> h_r_send;  // this rank's range payload, staged for the copy to the device
 	~rxgpu_comm() {
 		cudaSetDevice(device);
 		if (comm && nccl().ok) {
@@ -383,9 +456,6 @@ int rxgpu_sharded_search_knn(rxgpu_comm* c, const rxgpu_index* ix, uint32_t nq, 
 	if (ix->device != c->device) {
 		return fail(RXGPU_ERR_PARAMS, "rxgpu: the shard lives on another device than its communicator");
 	}
-	if (c->local && c->nranks > 1) {
-		return fail(RXGPU_ERR_LOGIC, "rxgpu: the sharded KNN search exchanges over NCCL (one process per GPU); in-process rank groups serve the ft_fast merge");
-	}
 	if (nq && (!queries || !out_count || (k && (!out_dist || !out_label)))) {
 		return fail(RXGPU_ERR_PARAMS, "rxgpu: null argument");
 	}
@@ -435,7 +505,9 @@ int rxgpu_sharded_search_knn(rxgpu_comm* c, const rxgpu_index* ix, uint32_t nq, 
 		const rxgpu_search_stats scanStats = g_stats;  // what the roofline figure describes: the shard scan, not the rare tie pass
 		// ---- 2. one all-gather, 3. device merge
 		if (R > 1) {
-			RX_NCCL(nccl().AllGather(c->d_send.p, c->d_recv.p, lay.bytes, ncclChar, c->comm, st));
+			if (int rc = commAllGather(c, c->d_send.p, c->d_recv.p, lay.bytes, st)) {
+				return rc;
+			}
 		}
 		const size_t on = size_t(nq) * k;
 		RX_CUDA(c->d_m_dist.ensure(on));
@@ -500,7 +572,9 @@ int rxgpu_sharded_search_knn(rxgpu_comm* c, const rxgpu_index* ix, uint32_t nq, 
 				return rc;
 			}
 			if (R > 1) {
-				RX_NCCL(nccl().AllGather(c->d_send.p, c->d_recv.p, tlay.bytes, ncclChar, c->comm, st));
+				if (int rc = commAllGather(c, c->d_send.p, c->d_recv.p, tlay.bytes, st)) {
+					return rc;
+				}
 			}
 			RX_CUDA(c->h_tie_recv.ensure(tlay.bytes * R));
 			RX_CUDA(cudaMemcpyAsync(c->h_tie_recv.p, c->d_recv.p, tlay.bytes * R, cudaMemcpyDeviceToHost, st));
@@ -545,6 +619,119 @@ int rxgpu_sharded_search_knn(rxgpu_comm* c, const rxgpu_index* ix, uint32_t nq, 
 		g_stats.tc_fallbacks = scanStats.tc_fallbacks;
 		g_stats.launches = after.launches + 1 + (tieQ.empty() ? 0 : 0);
 		g_stats.tie_replays = uint32_t(tieQ.size());
+	} catch (const std::bad_alloc&) {
+		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
+	}
+	return 0;
+}
+
+int rxgpu_sharded_search_range_batch(rxgpu_comm* c, const rxgpu_index* ix, uint32_t nq, const float* queries, int queries_on_device,
+									 const float* radius, uint64_t max_out, float* out_dist, uint64_t* out_label, uint64_t* out_n) {
+	if (!c) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: null communicator");
+	}
+	if (int rc = checkIndex(ix)) {
+		return rc;
+	}
+	if (ix->device != c->device) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: the shard lives on another device than its communicator");
+	}
+	if (nq && (!queries || !radius || !out_n || (max_out && (!out_dist || !out_label)))) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: null argument");
+	}
+	g_stats = rxgpu_search_stats{};
+	if (nq == 0) {
+		return 0;
+	}
+	std::lock_guard<std::mutex> lck(c->mtx);
+	try {
+		cudaStream_t st = c->stream;
+		const uint32_t R = uint32_t(c->nranks);
+		// ---- 1. this shard's matches; the best min(n, max_out) of every query are kept, best first (a global top-max_out never needs more)
+		RX_CUDA(c->h_r_n.ensure(nq));
+		std::vector<uint32_t> kept(nq, 0);
+		std::vector<size_t> first(nq, 0);
+		std::vector<float> kd;
+		std::vector<uint64_t> kl;
+		if (ix->size == 0) {
+			std::memset(c->h_r_n.p, 0, size_t(nq) * 8);
+		} else {
+			const float* d_q = queries;
+			if (!queries_on_device) {
+				RX_CUDA(c->d_queries.ensure(size_t(nq) * ix->dim));
+				RX_CUDA(cudaMemcpyAsync(c->d_queries.p, queries, size_t(nq) * ix->dim * 4, cudaMemcpyHostToDevice, st));
+				d_q = c->d_queries.p;
+			}
+			WsLease lease(ix);
+			const RangeEmit emit = [&](uint32_t q, const std::vector<Hit>& hits) {
+				c->h_r_n.p[q] = hits.size();
+				kept[q] = uint32_t(std::min<uint64_t>(hits.size(), max_out));
+				first[q] = kd.size();
+				for (uint32_t i = 0; i < kept[q]; ++i) {
+					kd.push_back(hits[i].dist);
+					kl.push_back(hits[i].label);
+				}
+			};
+			if (int rc = rangeBatch(ix, *lease.ws, st, d_q, nq, radius, max_out, emit)) {
+				return rc;
+			}
+		}
+		// ---- 2. the totals over all shards, and the width every rank sends
+		RX_CUDA(c->d_r_n.ensure(size_t(nq) + 1));
+		RX_CUDA(cudaMemcpyAsync(c->d_r_n.p, c->h_r_n.p, size_t(nq) * 8, cudaMemcpyHostToDevice, st));
+		if (int rc = commAllReduce(c, c->d_r_n.p, nq, CommOp::SumU64, st)) {
+			return rc;
+		}
+		RX_CUDA(cudaMemcpyAsync(c->h_r_n.p, c->d_r_n.p, size_t(nq) * 8, cudaMemcpyDeviceToHost, st));
+		RX_CUDA(cudaStreamSynchronize(st));
+		std::memcpy(out_n, c->h_r_n.p, size_t(nq) * 8);
+		if (max_out == 0) {
+			return 0;
+		}
+		uint32_t* d_w = reinterpret_cast<uint32_t*>(c->d_r_n.p + nq);
+		c->h_r_n.p[0] = *std::max_element(kept.begin(), kept.end());
+		RX_CUDA(cudaMemcpyAsync(d_w, c->h_r_n.p, 4, cudaMemcpyHostToDevice, st));
+		if (int rc = commAllReduce(c, d_w, 1, CommOp::MaxU32, st)) {
+			return rc;
+		}
+		RX_CUDA(cudaMemcpyAsync(c->h_r_n.p, d_w, 4, cudaMemcpyDeviceToHost, st));
+		RX_CUDA(cudaStreamSynchronize(st));
+		const uint32_t W = *reinterpret_cast<const uint32_t*>(c->h_r_n.p);
+		if (W == 0) {  // no match on any shard
+			return 0;
+		}
+		// ---- 3. one all-gather of the padded payloads, 4. device merge, and only the merged rows cross to the host
+		const RangeLayout lay(nq, W);
+		RX_CUDA(c->h_r_send.ensure(lay.bytes));
+		float* h_dist = reinterpret_cast<float*>(c->h_r_send.p + lay.off_dist);
+		uint64_t* h_label = reinterpret_cast<uint64_t*>(c->h_r_send.p + lay.off_label);
+		for (uint32_t q = 0; q < nq; ++q) {
+			std::memcpy(h_dist + size_t(q) * W, kd.data() + first[q], size_t(kept[q]) * 4);
+			std::memcpy(h_label + size_t(q) * W, kl.data() + first[q], size_t(kept[q]) * 8);
+		}
+		std::memcpy(c->h_r_send.p + lay.off_kept, kept.data(), size_t(nq) * 4);
+		RX_CUDA(c->d_send.ensure(lay.bytes));
+		RX_CUDA(c->d_recv.ensure(lay.bytes * R));
+		unsigned char* snd = R > 1 ? c->d_send.p : c->d_recv.p;  // a single shard merges its own payload in place
+		RX_CUDA(cudaMemcpyAsync(snd, c->h_r_send.p, lay.bytes, cudaMemcpyHostToDevice, st));
+		if (R > 1) {
+			if (int rc = commAllGather(c, c->d_send.p, c->d_recv.p, lay.bytes, st)) {
+				return rc;
+			}
+		}
+		const uint32_t width = uint32_t(std::min<uint64_t>(max_out, uint64_t(R) * W));
+		const size_t on = size_t(nq) * width;
+		RX_CUDA(c->d_m_dist.ensure(on));
+		RX_CUDA(c->d_m_label.ensure(on));
+		const unsigned blocks = unsigned((uint64_t(nq) * 32 + 255) / 256);
+		range_merge_kernel<<<blocks, 256, 0, st>>>(c->d_recv.p, R, nq, W, lay, width, c->d_m_dist.p, c->d_m_label.p);
+		RX_CUDA(cudaGetLastError());
+		g_stats.launches += 1;
+		RX_CUDA(cudaMemcpy2DAsync(out_dist, size_t(max_out) * 4, c->d_m_dist.p, size_t(width) * 4, size_t(width) * 4, nq,
+								  cudaMemcpyDeviceToHost, st));
+		RX_CUDA(cudaMemcpy2DAsync(out_label, size_t(max_out) * 8, c->d_m_label.p, size_t(width) * 8, size_t(width) * 8, nq,
+								  cudaMemcpyDeviceToHost, st));
+		RX_CUDA(cudaStreamSynchronize(st));
 	} catch (const std::bad_alloc&) {
 		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
 	}

@@ -135,6 +135,18 @@ class ShardedBruteforceSearch:
             out_d[q, :len(td2)], out_l[q, :len(td2)] = td2, tl2
         return out_d, out_l, rc
 
+    def search_range_batch(self, queries, radius, max_out: int):
+        """queries: host ndarray [nq, dim] or device tensor (identical on every rank); radius: a scalar or [nq], map space.  Returns
+        (dist [nq, max_out], label [nq, max_out], count [nq]) on every rank, as GpuBruteforceSearch.search_range_batch returns them for
+        one index holding all rows.  One C-ABI call per rank (rxgpu_sharded_search_range_batch); there is no CPU exchange for it."""
+        if self.comm is None:
+            raise NotImplementedError("sharded range search runs on the GPUs only (rxgpu_sharded_search_range_batch)")
+        if isinstance(queries, np.ndarray):
+            return self.comm.search_range_batch(self.idx, queries, radius, max_out)
+        assert queries.is_cuda and queries.dtype == torch.float32 and queries.is_contiguous()
+        torch.cuda.current_stream().synchronize()  # the library runs on its own stream: the queries must be complete
+        return self.comm.search_range_batch(self.idx, queries.data_ptr(), radius, max_out, nq=queries.shape[0])
+
 
 class ShardedHnswSearch(ShardedBruteforceSearch):
     """Multi-GPU HNSW (SURVEY.md §8e): every GPU holds an independent sub-graph over its row range (built by the reference's
