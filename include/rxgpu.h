@@ -79,7 +79,10 @@ int rxgpu_index_device(const rxgpu_index*);
  * nq independent queries (the reference API is one query per call; nq > 1 is our extension, results identical to nq
  * calls).  Per query: rows sorted best->worst exactly as HnswIndexBase::select drains the reference's max-heap
  * (hnsw_index.cc:258-276), including the reference's tie rule (which of several bit-equal distances survive depends on
- * insertion order and label, SURVEY.md §8a rule 2).  out_count[q] = min(k, size). */
+ * insertion order and label, SURVEY.md §8a rule 2).  out_count[q] = min(k, size).
+ * The exact scan holds one query, zero padded to a multiple of 128 floats, and eight warp lists of min(k + 1, 256) + 32 keys in at
+ * most 100 KB of shared memory: a search whose dimension and k exceed that fails with RXGPU_ERR_PARAMS.  At k = 10 the largest
+ * dimension served is 24832; a larger k lowers it.  The tensor-core filter serves dimensions up to 2048 only. */
 int rxgpu_search_knn(const rxgpu_index*, uint32_t nq, const float* queries /* nq x dim, host */, uint32_t k,
 					 float* out_dist /* nq x k */, uint64_t* out_label /* nq x k */, uint32_t* out_count /* nq */);
 /* BruteforceSearch::SearchRange (strict dist < radius)        hnswlib/bruteforce.cc:129-143
