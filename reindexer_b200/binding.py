@@ -505,16 +505,17 @@ class GpuBruteforceSearch:
     def sq8_search_knn(self, queries, k: int, query_norms=None):
         return self._sq8_search(self._lib.rxgpu_sq8_search_knn, queries, k, query_norms, ())
 
-    def hnsw_search_knn_sq8(self, queries, k: int, ef: int = 0, query_norms=None):
+    def hnsw_search_knn_sq8(self, queries, k: int, ef: int = 0, query_norms=None, with_stats=False):
         q = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, self.dim)
         nq = q.shape[0]
         qn = None if query_norms is None else np.ascontiguousarray(query_norms, np.float32)
         d = np.zeros((nq, max(k, 1)), np.float32)
         l = np.zeros((nq, max(k, 1)), np.uint64)
         c = np.zeros(nq, np.uint32)
+        st = np.zeros((nq, 2), np.uint32)
         _check(self._lib.rxgpu_hnsw_search_knn_sq8(self._h, nq, _p(q, _f32p), None if qn is None else _p(qn, _f32p), k, ef, _p(d, _f32p),
-                                                   _p(l, _u64p), _p(c, _u32p), None))
-        return d, l, c
+                                                   _p(l, _u64p), _p(c, _u32p), _p(st, _u32p)))
+        return (d, l, c, st) if with_stats else (d, l, c)
 
     # -- IVF (lists trained and assigned by the reference's FAISS; rows of this index grouped by list) -------------------
     def ivf_import(self, centroids, list_sizes):

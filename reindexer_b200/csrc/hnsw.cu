@@ -973,7 +973,7 @@ int rxgpu_hnsw_import(rxgpu_index* ix, const rxgpu_hnsw_graph* g) {
 		return fail(RXGPU_ERR_LOGIC, "rxgpu: HNSW graph size differs from the number of rows in the index");
 	}
 	if (g->maxM0 > uint32_t(kMaxNeighbours) || g->M > uint32_t(kMaxNeighbours) || g->n == 0 || g->enterpoint >= g->n) {
-		return fail(RXGPU_ERR_PARAMS, "rxgpu: unsupported HNSW graph (M must be <= 32, graph must be non-empty)");
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: unsupported HNSW graph (M and maxM0 must be <= 64, graph must be non-empty)");
 	}
 	if (g->upper_slots && !g->upper) {
 		return fail(RXGPU_ERR_PARAMS, "rxgpu: null graph");
@@ -1033,11 +1033,14 @@ int rxgpu_hnsw_import(rxgpu_index* ix, const rxgpu_hnsw_graph* g) {
 	h->upper_slots = g->upper_slots;
 	h->h_upper_off.assign(g->upper_offsets, g->upper_offsets + g->n);
 	h->h_levels.assign(g->levels, g->levels + g->n);
-	RX_CUDA(cudaMemcpy(h->level0.p, g->level0, l0 * 4, cudaMemcpyHostToDevice));
-	RX_CUDA(cudaMemcpy(h->levels.p, g->levels, size_t(g->n) * 4, cudaMemcpyHostToDevice));
-	RX_CUDA(cudaMemcpy(h->upper_off.p, g->upper_offsets, (size_t(g->n) + 1) * 8, cudaMemcpyHostToDevice));
+	// every upload goes through the index's stream, which is non-blocking: a plain cudaMemcpy runs on the legacy stream, is not
+	// ordered before the search kernels and may return before a pageable copy has landed
+	cudaStream_t st = ix->stream;
+	RX_CUDA(cudaMemcpyAsync(h->level0.p, g->level0, l0 * 4, cudaMemcpyHostToDevice, st));
+	RX_CUDA(cudaMemcpyAsync(h->levels.p, g->levels, size_t(g->n) * 4, cudaMemcpyHostToDevice, st));
+	RX_CUDA(cudaMemcpyAsync(h->upper_off.p, g->upper_offsets, (size_t(g->n) + 1) * 8, cudaMemcpyHostToDevice, st));
 	if (g->upper_slots) {
-		RX_CUDA(cudaMemcpy(h->upper.p, g->upper, size_t(g->upper_slots) * (1 + g->M) * 4, cudaMemcpyHostToDevice));
+		RX_CUDA(cudaMemcpyAsync(h->upper.p, g->upper, size_t(g->upper_slots) * (1 + g->M) * 4, cudaMemcpyHostToDevice, st));
 	}
 	{  // resident warps: the search is a chain of dependent gathers, so occupancy hides its latency; 64 registers per thread allow
 		// 8 CTAs (32 warps) per SM.  RXGPU_HNSW_CTAS_PER_SM is a tuning aid.
@@ -1049,9 +1052,10 @@ int rxgpu_hnsw_import(rxgpu_index* ix, const rxgpu_hnsw_graph* g) {
 	RX_CUDA(h->visited.ensure(size_t(h->slots) * h->words));
 	RX_CUDA(h->vlog.ensure(size_t(h->slots) * kVlogCap));
 	RX_CUDA(h->counter.ensure(1));
-	RX_CUDA(cudaMemset(h->visited.p, 0, size_t(h->slots) * h->words * 4));
+	RX_CUDA(cudaMemsetAsync(h->visited.p, 0, size_t(h->slots) * h->words * 4, st));
 	RX_CUDA(h->deleted.ensure(h->words));
-	RX_CUDA(cudaMemset(h->deleted.p, 0, size_t(h->words) * 4));
+	RX_CUDA(cudaMemsetAsync(h->deleted.p, 0, size_t(h->words) * 4, st));
+	RX_CUDA(cudaStreamSynchronize(st));  // the caller's graph arrays may go away after the return
 	h->h_deleted.assign(h->words, 0u);
 	h->index_version = ix->version;
 	if (ix->hnsw) {
@@ -1235,9 +1239,10 @@ int rxgpu_hnsw_search_knn_sq8(const rxgpu_index* ix, uint32_t nq, const float* q
 		RX_CUDA(di.ensure(size_t(nq) * kEff));
 		RX_CUDA(dc.ensure(nq));
 		RX_CUDA(ds.ensure(size_t(nq) * 2));
-		RX_CUDA(cudaMemcpy(s8->d_q.p, hq.data(), hq.size(), cudaMemcpyHostToDevice));
-		RX_CUDA(cudaMemcpy(s8->d_qcorr.p, hcorr.data(), size_t(nq) * 4, cudaMemcpyHostToDevice));
-		RX_CUDA(cudaMemcpy(s8->d_qcoef.p, hcoef.data(), size_t(nq) * 4, cudaMemcpyHostToDevice));
+		// on the stream the search runs on (hnswSearchDevice synchronises it before returning, so the host vectors outlive the copies)
+		RX_CUDA(cudaMemcpyAsync(s8->d_q.p, hq.data(), hq.size(), cudaMemcpyHostToDevice, ix->stream));
+		RX_CUDA(cudaMemcpyAsync(s8->d_qcorr.p, hcorr.data(), size_t(nq) * 4, cudaMemcpyHostToDevice, ix->stream));
+		RX_CUDA(cudaMemcpyAsync(s8->d_qcoef.p, hcoef.data(), size_t(nq) * 4, cudaMemcpyHostToDevice, ix->stream));
 		const Sq8Query sq{s8->d_q.p, s8->d_qcorr.p, s8->d_qcoef.p};
 		if (int rc = hnswSearchDevice(ix, nq, nullptr, kEff, ef, dd.p, di.p, dc.p, ds.p, nullptr, &sq)) {
 			return rc;
@@ -1300,7 +1305,7 @@ int rxgpu_hnsw_search_knn(const rxgpu_index* ix, uint32_t nq, const float* queri
 	RX_CUDA(di.ensure(size_t(nq) * kEff));
 	RX_CUDA(dc.ensure(nq));
 	RX_CUDA(ds.ensure(size_t(nq) * 2));
-	RX_CUDA(cudaMemcpy(dq.p, queries, size_t(nq) * ix->dim * 4, cudaMemcpyHostToDevice));
+	RX_CUDA(cudaMemcpyAsync(dq.p, queries, size_t(nq) * ix->dim * 4, cudaMemcpyHostToDevice, ix->stream));  // ordered before the search
 	if (int rc = rxgpu_hnsw_search_knn_device(ix, nq, dq.p, kEff, ef, dd.p, di.p, dc.p, ds.p, nullptr)) {
 		return rc;
 	}
@@ -1353,7 +1358,7 @@ int rxgpu_hnsw_search_range(const rxgpu_index* ix, const float* query, float rad
 	RX_CUDA(dd.ensure(kSeed));
 	RX_CUDA(di.ensure(kSeed));
 	RX_CUDA(dc.ensure(1));
-	RX_CUDA(cudaMemcpy(dq.p, query, size_t(ix->dim) * 4, cudaMemcpyHostToDevice));
+	RX_CUDA(cudaMemcpyAsync(dq.p, query, size_t(ix->dim) * 4, cudaMemcpyHostToDevice, ix->stream));  // ordered before the search
 	// search(): the whole top_candidates heap of the ef-search = its ef best nodes (SearchKnn with k = ef on the same routine)
 	if (int rc = rxgpu_hnsw_search_knn_device(ix, 1, dq.p, kSeed, ef, dd.p, di.p, dc.p, nullptr, nullptr)) {
 		return rc;
@@ -1870,7 +1875,8 @@ int rxgpu_hnsw_mark_deleted(rxgpu_index* ix, uint64_t label) {
 		return fail(RXGPU_ERR_LOGIC, "The requested to delete element is already deleted");  // hnswalg.h:1335
 	}
 	h->h_deleted[idx >> 5] |= bit;
-	RX_CUDA(cudaMemcpy(h->deleted.p + (idx >> 5), &h->h_deleted[idx >> 5], 4, cudaMemcpyHostToDevice));
+	RX_CUDA(cudaMemcpyAsync(h->deleted.p + (idx >> 5), &h->h_deleted[idx >> 5], 4, cudaMemcpyHostToDevice, ix->stream));
+	RX_CUDA(cudaStreamSynchronize(ix->stream));
 	h->num_deleted += 1;
 	return 0;
 }

@@ -1878,10 +1878,12 @@ int rxgpu_ivf_import(rxgpu_index* ix, uint32_t nlist, const float* centroids, co
 		h->nlist = nlist;
 		RX_CUDA(h->centroids.ensure(size_t(nlist) * ix->pitch));
 		RX_CUDA(h->list_begin.ensure(size_t(nlist) + 1));
-		RX_CUDA(cudaMemset(h->centroids.p, 0, size_t(nlist) * ix->pitch * sizeof(float)));
-		RX_CUDA(cudaMemcpy2D(h->centroids.p, size_t(ix->pitch) * 4, centroids, size_t(ix->dim) * 4, size_t(ix->dim) * 4, nlist,
-							 cudaMemcpyHostToDevice));
-		RX_CUDA(cudaMemcpy(h->list_begin.p, begin.data(), begin.size() * 4, cudaMemcpyHostToDevice));
+		// on the index's stream, which the IVF kernels use: a legacy-stream copy would not be ordered before them
+		RX_CUDA(cudaMemsetAsync(h->centroids.p, 0, size_t(nlist) * ix->pitch * sizeof(float), ix->stream));
+		RX_CUDA(cudaMemcpy2DAsync(h->centroids.p, size_t(ix->pitch) * 4, centroids, size_t(ix->dim) * 4, size_t(ix->dim) * 4, nlist,
+								  cudaMemcpyHostToDevice, ix->stream));
+		RX_CUDA(cudaMemcpyAsync(h->list_begin.p, begin.data(), begin.size() * 4, cudaMemcpyHostToDevice, ix->stream));
+		RX_CUDA(cudaStreamSynchronize(ix->stream));
 		if (ix->metric == RXGPU_COS) {
 			RX_CUDA(h->cnorm.ensure(nlist));
 			norm_coef_kernel<<<(nlist * 32 + 255) / 256, 256, 0, ix->stream>>>(h->centroids.p, ix->pitch, ix->dim, 0, nlist, h->cnorm.p);

@@ -345,9 +345,11 @@ int rxgpu_sq8_attach(rxgpu_index* ix, const rxgpu_sq8_params* p, const uint8_t* 
 	RX_CUDA(s->codes.ensure(n * s->code_pitch));
 	RX_CUDA(s->corr.ensure(n));
 	if (codes) {  // the reference's own codes and offsets (HierarchicalNSWImpl<uint8_t>, by internal id = row)
-		RX_CUDA(cudaMemset(s->codes.p, 0, n * s->code_pitch));
-		RX_CUDA(cudaMemcpy2D(s->codes.p, s->code_pitch, codes, ix->dim, ix->dim, ix->size, cudaMemcpyHostToDevice));
-		RX_CUDA(cudaMemcpy(s->corr.p, offsets, size_t(ix->size) * 4, cudaMemcpyHostToDevice));
+		// on the index's stream, which the scans use: a legacy-stream copy would not be ordered before them
+		RX_CUDA(cudaMemsetAsync(s->codes.p, 0, n * s->code_pitch, ix->stream));
+		RX_CUDA(cudaMemcpy2DAsync(s->codes.p, s->code_pitch, codes, ix->dim, ix->dim, ix->size, cudaMemcpyHostToDevice, ix->stream));
+		RX_CUDA(cudaMemcpyAsync(s->corr.p, offsets, size_t(ix->size) * 4, cudaMemcpyHostToDevice, ix->stream));
+		RX_CUDA(cudaStreamSynchronize(ix->stream));
 	} else if (ix->size) {
 		sq8_quantize_rows<<<unsigned((ix->size + 127) / 128), 128, 0, ix->stream>>>(ix->d_rows, ix->pitch, ix->dim, uint32_t(ix->size), p->min_q, p->alpha,
 																					 p->delta, ix->metric == RXGPU_L2, s->codes.p, s->code_pitch, s->corr.p);
@@ -437,7 +439,12 @@ int rxgpu_sq8_search_knn(const rxgpu_index* ix, uint32_t nq, const float* querie
 		RX_CUDA(cudaMemcpyAsync(s->d_q.p, hq.data(), hq.size(), cudaMemcpyHostToDevice, st));
 		RX_CUDA(cudaMemcpyAsync(s->d_qcorr.p, hcorr.data(), size_t(nq) * 4, cudaMemcpyHostToDevice, st));
 		RX_CUDA(cudaMemcpyAsync(s->d_qcoef.p, hcoef.data(), size_t(nq) * 4, cudaMemcpyHostToDevice, st));
-		const int qt = nq >= 4 ? 4 : (nq >= 2 ? 2 : 1);
+		// the widest query tile the batch fills whose staged codes and key lists fit the budget: at k = 256, qt = 4 holds up to 7056
+		// dims, qt = 2 up to 32656 and qt = 1 every dimension the index accepts, so the refusal below is only a guard
+		int qt = nq >= 4 ? 4 : (nq >= 2 ? 2 : 1);
+		while (qt > 1 && sqScanSmem(qt, cp, kEff) > 100 * 1024) {
+			qt /= 2;
+		}
 		const unsigned grid = unsigned(std::min<uint64_t>(uint64_t(ix->sm_count) * 2, std::max<uint64_t>(1, (ix->size + 2 * kSqWarps - 1) / (2 * kSqWarps))));
 		const size_t smem = sqScanSmem(qt, cp, kEff);
 		if (smem > 100 * 1024) {
