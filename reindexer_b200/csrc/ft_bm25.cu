@@ -258,6 +258,13 @@ __global__ void ft_popcount(const uint32_t* mask, uint32_t words, unsigned long 
 		atomicAdd(out, s_sum);
 	}
 }
+// static_cast<uint16_t>(proc) of calcTermScores as the reference's x86-64 build executes it: cvttss2si truncates to int32, NaN and
+// values outside [-2^31, 2^31) give INT32_MIN, and the low 16 bits are kept.  A negative boost thus scores up to 16383 there and a
+// proc >= 65536 wraps; the device's own float -> u16 conversion saturates instead, so the conversion is written out.
+__device__ __forceinline__ uint32_t proc_to_u16(float proc) {
+	const int32_t i = proc >= -2147483648.f && proc < 2147483648.f ? __float2int_rz(proc) : INT32_MIN;
+	return uint32_t(i) & 0xFFFFu;
+}
 // calcTermScores (mergerimpl.h:289-324): one pass per subterm; a document scores once per term (tmask)
 __global__ void ft_score_pass(DevList l, TermParams t, int all_same, const uint32_t* mask, uint32_t* tmask, uint16_t* score, const uint32_t* enabled) {
 	if (enabled && !*enabled) {  // preselect decided on the device (ft_decide_preselect): the host enqueues the whole query ahead
@@ -279,7 +286,7 @@ __global__ void ft_score_pass(DevList l, TermParams t, int all_same, const uint3
 		if (maxBoost > 0.f) {
 			if (!(atomicOr(&tmask[d >> 5], bit) & bit)) {  // docs are unique inside one list: exactly one thread scores d in this pass
 				const float proc = __fmul_rn(__fmul_rn(t.proc, maxBoost), t.boost);
-				uint32_t p16 = uint32_t(uint16_t(proc));
+				uint32_t p16 = proc_to_u16(proc);
 				p16 = min(p16, 65535u / 4u);
 				p16 = min(p16, 65535u - uint32_t(score[d]));
 				score[d] = uint16_t(score[d] + p16);

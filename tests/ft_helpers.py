@@ -128,6 +128,178 @@ def corpus_problem(seed, total_docs=600, nfields=2, vocab=24, merge_limit=20000,
     return p
 
 
+def bulk_list(p, rng, docs, npos=1, max_pos=40, nfields=None, fields=None, first_pos=None):
+    """add_list without a per-document Python loop: docs ascending and unique, npos positions per document (a scalar or one count per
+    document) in random fields below nfields (or the given per-document `fields`) at word positions below max_pos, duplicates merged.
+    first_pos (per document) moves the positions of a document up by that much and adds first_pos itself in the document's first
+    field (field 0, or fields[i]), so it is that field's first position."""
+    docs = np.ascontiguousarray(docs, np.uint32)
+    nfields = p.nfields if nfields is None else nfields
+    cnt = np.broadcast_to(np.asarray(npos, np.int64), docs.shape)
+    assert (cnt >= 1).all()
+    owner = np.repeat(np.arange(len(docs)), cnt)
+    f = rng.integers(0, nfields, size=len(owner)) if fields is None else np.asarray(fields, np.int64)[owner]
+    pos = rng.integers(0, max_pos, size=len(owner))
+    if first_pos is not None:
+        pos = np.minimum(pos + np.asarray(first_pos, np.int64)[owner], (1 << 24) - 1)
+    packed = (f.astype(np.uint64) << 24) | pos.astype(np.uint64)
+    if first_pos is not None:
+        f0 = np.zeros(len(docs), np.int64) if fields is None else np.asarray(fields, np.int64)
+        owner = np.concatenate([owner, np.arange(len(docs))])
+        packed = np.concatenate([packed, (f0.astype(np.uint64) << 24) | np.asarray(first_pos, np.uint64)])
+    order = np.lexsort((packed, owner))
+    owner, packed = owner[order], packed[order]
+    keep = np.ones(len(owner), bool)
+    keep[1:] = (owner[1:] != owner[:-1]) | (packed[1:] != packed[:-1])
+    owner, packed = owner[keep], packed[keep].astype(np.uint32)
+    begin = np.zeros(len(docs) + 1, np.uint32)
+    begin[1:] = np.cumsum(np.bincount(owner, minlength=len(docs)))
+    return p.add_list_arrays(docs, begin, packed)
+
+
+def random_words(rng, total_docs, nfields, lo=3, hi=40):
+    words = rng.integers(lo, hi, size=(total_docs, nfields)).astype(np.uint32)
+    words[0] = 0
+    return words
+
+
+def score_problem(scores, saturated=None, seed=0, nfields=1, merge_limit=20000, excluded=None, removed=None, max_pos=40):
+    """OR terms whose preselect scores are chosen per document (scores[d] in 0..65535).  Term b (b = 0..13) holds the documents whose
+    remainder has bit b set, with subterm proc 1 and term boost 2^b; up to four more terms of boost 16384 add 65535 / 4 = 16383 each
+    (the per-subterm cap).  So calcTermScores (mergerimpl.h:289-324) gives document d exactly scores[d].  Documents marked `saturated`
+    are put into five capped terms instead: 5 x 16383 saturates the u16 sum at 65535."""
+    scores = np.asarray(scores, np.int64)
+    total_docs = len(scores)
+    assert scores[0] == 0 and (scores >= 0).all() and (scores <= 65535).all()
+    caps = np.minimum(scores // 16383, 4)
+    target = scores - caps * 16383
+    if saturated is not None:
+        caps = np.where(saturated, 5, caps)
+        target = np.where(saturated, 0, target)
+    rng = np.random.default_rng(seed)
+    p = F.FtProblem(total_docs, random_words(rng, total_docs, nfields), removed=removed, excluded=excluded)
+    p.cfg["merge_limit"] = merge_limit
+    assert (target < 16384).all()
+    for b in range(14):
+        docs = np.nonzero((target >> b) & 1)[0]
+        if len(docs):
+            p.add_term([(bulk_list(p, rng, docs, npos=rng.integers(1, 3, size=len(docs)), max_pos=max_pos), 1.0)], boost=float(1 << b))
+    for c in range(int(caps.max())):
+        docs = np.nonzero(caps > c)[0]
+        p.add_term([(bulk_list(p, rng, docs, max_pos=max_pos), 1.0)], boost=16384.0)
+    return p
+
+
+def planted_scores(n, seed, top, thr, run_start, run_len, frac=0.3, above=0.02):
+    """preselect scores for score_problem: a fraction of the documents below thr, a few in (thr, top], document 1 at top and a run
+    of run_len consecutive documents from run_start at exactly thr (so the threshold's documents fill whole mask words)"""
+    rng = np.random.default_rng(seed)
+    s = np.zeros(n, np.int64)
+    lo = rng.random(n) < frac
+    s[lo] = rng.integers(1, max(thr, 2), size=int(lo.sum()))
+    if top > thr:
+        hi = rng.random(n) < above
+        s[hi] = rng.integers(thr + 1, top + 1, size=int(hi.sum()))
+    s[run_start:run_start + run_len] = thr
+    s[1] = top
+    s[0] = 0
+    return s
+
+
+def cut_limit(scores, thr, cut_id):
+    """the merge_limit that makes thr the threshold score and keeps the threshold's documents up to and including cut_id"""
+    eq = np.nonzero(scores == thr)[0]
+    assert cut_id in eq
+    return int((scores > thr).sum()) + int(np.searchsorted(eq, cut_id, side="right"))
+
+
+def ref_u16(proc):
+    """static_cast<uint16_t>(float) as the reference's x86-64 build executes it: cvttss2si truncates to int32 (NaN and values outside
+    [-2^31, 2^31) give INT32_MIN), then the low 16 bits are kept"""
+    x = np.asarray(proc, np.float32).astype(np.float64)
+    ok = (x >= -2.0 ** 31) & (x < 2.0 ** 31)
+    i = np.where(ok, np.trunc(np.where(ok, x, 0.0)), -2.0 ** 31).astype(np.int64)
+    return (i & 0xFFFF).astype(np.int64)
+
+
+def _per_doc(lst, fb, any_nonzero):
+    """per document of a list: whether a position lies in a field of non-zero boost (calcTermBitmask), or the largest field boost
+    over its positions, starting from 0 (maxFieldsBoost)"""
+    d, b, q = lst
+    assert (np.diff(b.astype(np.int64)) > 0).all()
+    if not len(d):
+        return np.zeros(0, bool if any_nonzero else np.float32)
+    v = np.asarray(fb, np.float32)[q >> 24]
+    if any_nonzero:
+        return np.logical_or.reduceat(v != 0, b[:-1].astype(np.int64))
+    return np.maximum(np.maximum.reduceat(v, b[:-1].astype(np.int64)), np.float32(0))
+
+
+def preselect_plan(p, to_u16=None):
+    """numpy restatement of buildRestrictingBitmask, estimateNumDocsInMerge, calcTermScores and the threshold walk of
+    preselectMostRelevantDocs (mergerimpl.h:289-464, merger.h:239-267) for plain OR / AND / NOT terms.  Used to prove that a
+    problem reaches a boundary of the device's preselect: the top score, the threshold (minScore) and the budget of documents kept
+    at the threshold, and which documents hold that score.  to_u16 replaces the reference's float -> u16 conversion (ref_u16)."""
+    assert not p.synonyms and not any(t.get("phrase_num", 0) for t in p.terms)
+    N = p.total_docs
+    mask = np.ones(N, bool) if p.excluded is None else p.excluded == 0
+    for t in p.terms:
+        if t["op"] == F.OP_AND:
+            tm = np.zeros(N, bool)
+            for li in t["postings"]:
+                d = p.lists[int(li)][0]
+                tm[d if (t["field_boosts"] != 0).all() else d[_per_doc(p.lists[int(li)], t["field_boosts"], True)]] = True
+            mask &= tm
+    for t in p.terms:
+        if t["op"] == F.OP_NOT:
+            for li in t["postings"]:
+                mask[p.lists[int(li)][0]] = False
+    est_or, est_and = 0, None
+    for t in p.terms:
+        if t["op"] == F.OP_NOT:
+            continue
+        nd = sum(len(p.lists[int(li)][0]) for li in t["postings"])
+        if t["op"] == F.OP_AND:
+            est_and = nd if est_and is None else min(est_and, nd)
+        else:
+            est_or += nd
+    est = min(est_or if est_and is None else min(est_or, est_and), N)
+    total_or = sum(len(p.lists[int(li)][0]) for t in p.terms for li in t["postings"])
+    ml = p.cfg["merge_limit"]
+    max_merged = min(ml, total_or)
+    popcount = int(mask.sum())
+    simple = len(p.terms) == 1 and p.terms[0]["op"] != F.OP_NOT
+    score = np.zeros(N, np.int64)
+    for t in p.terms:
+        if t["op"] == F.OP_NOT:
+            continue
+        fb = np.asarray(t["field_boosts"], np.float32)
+        tmask = np.zeros(N, bool)
+        for li, sp in zip(t["postings"], t["procs"]):
+            d = p.lists[int(li)][0].astype(np.int64)
+            mb = np.full(len(d), fb[0], np.float32) if (fb == fb[0]).all() else _per_doc(p.lists[int(li)], fb, False)
+            sel = mask[d] & (mb > 0) & ~tmask[d]
+            proc = (np.float32(sp) * mb[sel]).astype(np.float32) * np.float32(t["boost"])
+            p16 = np.minimum((to_u16 or ref_u16)(proc), 65535 // 4)
+            dd = d[sel]
+            score[dd] += np.minimum(p16, 65535 - score[dd])
+            tmask[dd] = True
+    if p.removed is not None:
+        score[p.removed != 0] = 0
+    score[~mask] = 0
+    hist = np.bincount(score, minlength=65536)
+    min_score, budget, taken = 65535, 0, 0
+    for sc in range(65535, 0, -1):
+        if taken >= max_merged:
+            break
+        min_score, budget = sc, max_merged - taken
+        taken += int(hist[sc])
+    eq = np.nonzero(mask & (score == min_score))[0]
+    return dict(preselect=(not simple) and est > ml and N > ml and popcount > ml, popcount=popcount, estimate=est, max_merged=max_merged,
+                score=score, top=int(score.max()), min_score=min_score, budget=budget, eq=eq, positive=int((score > 0).sum()),
+                kept=int((score > min_score).sum()) + min(budget, len(eq)))
+
+
 def assert_same_merge(a, b, rank_sort_type, ctx=""):
     """a, b: MERGE_INFO arrays.  RankAndID / IDOnly keep the merge order (deterministic); RankOnly / IDAndPositions are sorted by an
     unstable sort, so equal ranks compare as sets."""
