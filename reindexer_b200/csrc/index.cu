@@ -1770,14 +1770,17 @@ int rxgpu_index_append_synth(rxgpu_index* ix, uint64_t seed, uint64_t first_row,
 	if (n == 0) {
 		return 0;
 	}
+	// refuse before touching the dictionary: a refused call leaves the index exactly as it was
+	for (uint64_t r = 0; r < n; ++r) {
+		if (ix->dict.find((first_row + r) << 32) != LabelMap::kNotFound) {
+			return fail(RXGPU_ERR_LOGIC, "rxgpu: synthetic rows must have fresh labels");
+		}
+	}
 	try {
 		ix->h_labels.reserve(ix->size + n);
 		ix->dict.reserve(ix->size + n);
 		for (uint64_t r = 0; r < n; ++r) {
 			const uint64_t label = (first_row + r) << 32;
-			if (ix->dict.find(label) != LabelMap::kNotFound) {
-				return fail(RXGPU_ERR_LOGIC, "rxgpu: synthetic rows must have fresh labels");
-			}
 			ix->dict.put(label, uint32_t(ix->size + r));
 			ix->h_labels.push_back(label);
 		}

@@ -113,8 +113,14 @@ class Envelope:
         return self
 
 
-def check_knn(env, d, lab, cnt, k, ctx=""):
-    """distances inside the envelope of the rows their labels name, sorted, min(k, n) results, and no missing row with hi < d_k"""
+def label_rows(lab):
+    """the envelope row a label names when row r was inserted as O.row_labels: its row id"""
+    return (np.asarray(lab, np.uint64) >> np.uint64(32)).astype(np.int64)
+
+
+def check_knn(env, d, lab, cnt, k, ctx="", row_of=label_rows):
+    """distances inside the envelope of the rows their labels name, sorted, min(k, n) results, and no missing row with hi < d_k;
+    row_of maps labels to envelope rows (-1: no such row)"""
     nq, n = env.lo.shape
     avail = getattr(env, "allowed", np.ones((nq, n), bool)).sum(1)
     for q in range(nq):
@@ -123,7 +129,7 @@ def check_knn(env, d, lab, cnt, k, ctx=""):
         if want == 0:
             continue
         dq = d[q, :want].astype(np.float64)
-        rows = (lab[q, :want] >> np.uint64(32)).astype(np.int64)
+        rows = row_of(lab[q, :want])
         assert len(np.unique(rows)) == want, (ctx, q, "a row returned twice")
         assert ((rows >= 0) & (rows < n)).all(), (ctx, q, rows)
         assert (np.diff(dq) >= 0).all(), (ctx, q, "not sorted", dq)
@@ -138,7 +144,7 @@ def check_knn(env, d, lab, cnt, k, ctx=""):
             assert len(ahead) == 0, (ctx, q, "rows missing from the result", ahead[:5], env.mid[q, ahead[:5]], dq[-1])
 
 
-def check_range(env, radius, d, lab, cnt, ctx=""):
+def check_range(env, radius, d, lab, cnt, ctx="", row_of=label_rows):
     """every row with hi < radius returned, every returned row lo < radius, distances in the envelope and sorted, totals exact"""
     nq, n = env.lo.shape
     radius = np.broadcast_to(np.asarray(radius, np.float32), (nq,)).astype(np.float64)
@@ -146,8 +152,9 @@ def check_range(env, radius, d, lab, cnt, ctx=""):
         c = int(cnt[q])
         assert c <= d.shape[1], (ctx, q, c)
         dq = d[q, :c].astype(np.float64)
-        rows = (lab[q, :c] >> np.uint64(32)).astype(np.int64)
+        rows = row_of(lab[q, :c])
         assert len(np.unique(rows)) == c, (ctx, q, "a row returned twice")
+        assert ((rows >= 0) & (rows < n)).all(), (ctx, q, rows)
         assert (np.diff(dq) >= 0).all(), (ctx, q, "not sorted")
         assert ((env.lo[q, rows] <= dq) & (dq <= env.hi[q, rows])).all(), (ctx, q, "distance outside the fp64 envelope")
         assert (dq < radius[q]).all() and (env.lo[q, rows] < radius[q]).all(), (ctx, q, "a row at or above the radius")
