@@ -277,6 +277,16 @@ int rxgpu_gather_labels_device(const rxgpu_index*, uint64_t n, const uint32_t* d
  * hnsw_index.cc:185).  ef == 0 is treated as 1. */
 int rxgpu_hnsw_search_range(const rxgpu_index*, const float* query /* host */, float radius, uint32_t ef, uint64_t max_out,
 							float* out_dist, uint64_t* out_label, uint64_t* out_n);
+/* HierarchicalNSWImpl::SearchRange for nq queries at once (our extension; the reference takes one query per call).
+ * Per query q the result is identical to rxgpu_hnsw_search_range(queries + q*dim, radius[q], ef, max_out, ...):
+ * out_n[q] = total matches, the best min(out_n[q], max_out) go best-first into row q of out_dist / out_label (nq x max_out).
+ * One ef-search for the batch seeds the closures; one launch per BFS level expands the closures of up to (SMs x 32) queries.
+ * A query keeps min(n, max(4096, 2 * min(max_out, 131072))) matches on the device; one with more is answered again with room for
+ * the whole graph (same answer).  A NaN or -inf radius matches nothing, +inf floods the query's reachable component.
+ * rxgpu_last_search_stats: launches = all kernel launches, passes = BFS levels run, tc_fallbacks = queries answered again. */
+int rxgpu_hnsw_search_range_batch(const rxgpu_index*, uint32_t nq, const float* queries /* nq x dim, host */,
+								  const float* radius /* nq, map space */, uint32_t ef, uint64_t max_out,
+								  float* out_dist, uint64_t* out_label, uint64_t* out_n /* nq */);
 
 /* Streaming (resumable) search: HierarchicalNSWImpl::BeginStreamingSearch / ContinueStreamingSearch   hnswlib/hnswalg.h:1864-1975
  * (the KNN iterator of filtered queries pulls batches until enough rows pass the other conditions,
@@ -492,7 +502,8 @@ typedef struct {
 	uint32_t scan_launches;     /* with rxgpu_set_profile(1): launches of the dominant kernel timed ... */
 	float scan_kernel_ms;       /* ... and their summed device time (CUDA events on the launching stream) */
 	uint32_t tc_used;           /* 1 when the tensor-core filter + exact re-rank path answered the batch */
-	uint32_t tc_fallbacks;      /* queries whose candidate list overflowed and were answered by the exact scan */
+	uint32_t tc_fallbacks;      /* queries whose candidate list overflowed and were answered by the exact scan
+	                               (rxgpu_hnsw_search_range_batch: whose result region overflowed and were answered again) */
 	uint64_t tc_candidates;     /* rows re-ranked exactly */
 	uint32_t tc_cluster;        /* CTAs per cluster in the filter kernel (row tiles are TMA-multicast inside a cluster) */
 	uint32_t tc_kernel;         /* 1 = knn_tc_filter (wgmma, queries in shared memory) */
