@@ -192,6 +192,7 @@ _SIGNATURES = {
     "rxgpu_set_query_tile": (C.c_int, [C.c_void_p, C.c_uint32]),
     "rxgpu_last_search_stats": (None, [C.POINTER(SearchStats)]),
     "rxgpu_set_profile": (C.c_int, [C.c_int]),
+    "rxgpu_tc_diag": (C.c_int, [C.c_int, C.c_void_p]),
     "rxgpu_set_tensor_core_filter": (C.c_int, [C.c_void_p, C.c_int]),
 }
 

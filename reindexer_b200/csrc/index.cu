@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <memory>
 #include <mutex>
@@ -267,6 +268,14 @@ TcKernel tcKernel(uint32_t nqb, uint32_t cluster) {
 										 {knn_tc_filter<128, 1>, knn_tc_filter<128, 2>}};
 	return table[nqb / 32 - 1][cluster == 2 ? 1 : 0];
 }
+// rxgpu_tc_diag: the diagnostic instantiation every filter launch of this process takes instead (0 = none), and its counters
+std::atomic<int> g_tc_diag{0};
+unsigned long long* g_tc_diag_buf = nullptr;
+TcKernel tcDiagKernel(int mode) {
+	static const TcKernel table[3] = {knn_tc_filter<128, 1, kTcDiagStamps>, knn_tc_filter<128, 1, kTcDiagNoRare>,
+									  knn_tc_filter<128, 1, kTcDiagNoFetch>};
+	return table[mode - 1];
+}
 
 uint32_t tcQueryBlock(uint32_t nq, uint32_t kchunks) {
 	uint32_t nqb = std::min<uint32_t>(kTcMaxNq, (nq + 31u) & ~31u);
@@ -345,7 +354,9 @@ int ensureShadow(const rxgpu_index* ix, cudaStream_t st) {
 
 // One batch of queries on the candidate filter: the int8 query codes and their tensor map, prepared once, and the launch shape.
 struct TcBatch {
-	uint32_t nq, nqb, cluster, ngroups, nqPad, kchunks;
+	uint32_t nq, nqb, cluster, ngroups, nqPad, kchunks, queueSlots;
+	int diag;     // the diagnostic instantiation taken (rxgpu_tc_diag), 0 = the production kernel
+	size_t smem;  // tc_smem_bytes + the candidate queues
 	int resident;
 	TcKernel kfn;
 	CUtensorMap mapQ;
@@ -378,11 +389,23 @@ int tcPrepare(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float
 		return rc;
 	}
 	b.kfn = tcKernel(nqb, cluster);
+	b.queueSlots = tc_queue_slots(nqb, kchunks, kTcSmemLimit);
+	b.smem = tc_smem_bytes(nqb, kchunks) + tc_queue_bytes(b.queueSlots);
+	if (b.queueSlots == 0) {
+		return fail(RXGPU_ERR_SYSTEM, "rxgpu: no room for the tensor-core filter's candidate queues");
+	}
+	b.diag = g_tc_diag.load();
+	if (const int diag = b.diag) {
+		if (nqb != 128 || cluster != 1) {
+			return fail(RXGPU_ERR_PARAMS, "rxgpu: the diagnostic filter instantiations take query blocks of 128 and single CTAs");
+		}
+		b.kfn = tcDiagKernel(diag);
+	}
 	RX_CUDA(raiseSmemCeilingOnce(b.kfn, ix->device, int(kTcSmemLimit)));
 	cudaLaunchConfig_t cfg{};
 	cfg.gridDim = dim3(unsigned(ix->sm_count) / cluster * cluster);
 	cfg.blockDim = dim3(kTcThreads);
-	cfg.dynamicSmemBytes = tc_smem_bytes(nqb, kchunks);
+	cfg.dynamicSmemBytes = b.smem;
 	cudaLaunchAttribute attr[1];
 	attr[0].id = cudaLaunchAttributeClusterDimension;
 	attr[0].val.clusterDim.x = cluster;
@@ -418,7 +441,7 @@ int tcLaunch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const TcBatc
 	RX_CUDA(cudaGetLastError());
 	cudaLaunchConfig_t cfg{};
 	cfg.blockDim = dim3(kTcThreads);
-	cfg.dynamicSmemBytes = tc_smem_bytes(nqb, kchunks);
+	cfg.dynamicSmemBytes = b.smem;
 	cfg.stream = st;
 	cudaLaunchAttribute attr[1];
 	attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -444,6 +467,8 @@ int tcLaunch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const TcBatc
 	a.nq_total = nq;
 	a.k1 = k1;
 	a.metric = ix->metric;
+	a.queue_slots = b.queueSlots;
+	a.diag = g_tc_diag_buf;
 	// One launch serves G = min(groups left, resident) query groups with W = resident / G tile walkers each, so the G clusters of a
 	// walker read every row tile from HBM about once and from L2 otherwise (config 1: 8 blocks x 16 walkers = 128 CTAs, the shadow
 	// streamed once per batch instead of once per block).  The grid never exceeds what is resident at once: a second wave would put
@@ -473,7 +498,7 @@ int tcLaunch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const TcBatc
 		g0 += groups;
 	}
 	g_stats.tc_cluster = cluster;
-	g_stats.tc_kernel = 1;
+	g_stats.tc_kernel = 1 + uint32_t(b.diag);  // > 1: a diagnostic instantiation answered, the results are not to be used
 	g_stats.query_tile = nqb * cluster;
 	return 0;
 }
@@ -1177,6 +1202,18 @@ int rxgpu_set_tensor_core_filter(rxgpu_index* ix, int mode) {
 	}
 	ix->tc_mode = uint32_t(mode >= 3 ? 1 : mode);
 	ix->tc_cluster_max = mode == 4 ? 2u : 0u;
+	return 0;
+}
+int rxgpu_tc_diag(int mode, void* d_counters) {
+	if (mode < 0 || mode > kTcDiagNoFetch || (mode && !d_counters)) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: diagnostic filter mode must be 0..3, with a counter buffer");
+	}
+	const char* env = std::getenv("RXGPU_TC_DIAG");
+	if (mode && !(env && std::strcmp(env, "1") == 0)) {  // a stray call must not turn every search of the process into a diagnostic
+		return fail(RXGPU_ERR_LOGIC, "rxgpu: diagnostic filter instantiations are enabled only with RXGPU_TC_DIAG=1 in the environment");
+	}
+	g_tc_diag_buf = static_cast<unsigned long long*>(d_counters);
+	g_tc_diag.store(mode);
 	return 0;
 }
 int rxgpu_set_profile(int on) {

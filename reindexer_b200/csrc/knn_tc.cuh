@@ -42,10 +42,12 @@
 //                fp32 stays the source of truth; the shadow is private, derived).  In a cluster of two CTAs (optional; single CTAs
 //                are faster on the H100) each CTA fetches half of every stage and multicasts it to both, which own consecutive
 //                query blocks.
+//   warps 2, 3   bookkeepers: warp 2 + w serves the candidate queue of consumer warpgroup w (below): the row's own bound, the
+//                append to the per-query candidate lists in HBM, the bound list and tau, off the MMA path.
 //   warpgroups 1, 2   consumers: warpgroup w multiplies its 64-row blocks with the whole query block (wgmma.m64nNQk32.s32.s8.s8,
 //                both operands from shared memory, exact int32 accumulators in registers), releases each stage as soon as its MMAs
-//                retired, then tests its 64 x NQ scores against tau, appends candidates to per-query lists in HBM and tightens
-//                tau.  The two rings are independent, so one warpgroup's epilogue overlaps the other's MMAs.
+//                retired, then tests its 64 x NQ scores against tau and hands every hit to its bookkeeper through a queue in shared
+//                memory.  The two rings are independent, so one warpgroup's epilogue overlaps the other's MMAs.
 #pragma once
 #include <cuda.h>
 
@@ -85,7 +87,44 @@ struct TcArgs {
 	uint32_t groups;           // G: query groups of this launch (a group = one query block per CTA of a cluster)
 	uint32_t k1;
 	int metric;                // kL2 / kIP / kCos
+	uint32_t queue_slots;      // records per candidate queue (tc_queue_slots; a power of two)
+	unsigned long long* diag;  // diagnostic instantiations only (kDiag != 0): the counters of tc_diag_* below; unused otherwise
 };
+
+// Diagnostic instantiations of knn_tc_filter (template flag kDiag, 0 in every search; bench_tc_phases.py selects one through
+// rxgpu_tc_diag).  kTcDiagStamps stamps every phase of every tile with clock64(); the two ablations bound what the epilogue and the
+// row stream cost: kTcDiagNoRare compiles the rare path out (the block test stays, hits are only counted, tau never tightens), and
+// kTcDiagNoFetch lets the producers cycle the barriers without fetching (the consumers multiply zeroed stages).  Their candidate
+// lists are meaningless; only the time and the counters are read.
+constexpr int kTcDiagStamps = 1;
+constexpr int kTcDiagNoRare = 2;
+constexpr int kTcDiagNoFetch = 3;
+// a.diag layout: [gridDim.x][kTcDiagSlots] per-CTA counters, then [kTcDiagWalk] hits per walk position (position i = the walker's
+// i-th tile, summed over all CTAs), then [gridDim.x][kTcDiagWalk / kTcDiagMarkEvery] %globaltimer marks taken when a CTA starts the
+// walk positions 0, kTcDiagMarkEvery, 2 kTcDiagMarkEvery, ...
+constexpr uint32_t kTcDiagSlots = 32;
+constexpr uint32_t kTcDiagWalk = 8192;
+constexpr uint32_t kTcDiagMarkEvery = 64;
+// per-CTA counters: consumer warpgroup w at w * kTcDgPerWg + (one of the phases below, in clock64 cycles summed over its four warps;
+// blocks, hits and queue waits are counts), producer ring r at kTcDgEmpty + r (cycles waiting on `empty`) and kTcDgProd + r (total)
+enum : uint32_t {
+	kTcDgFull,     // waiting on full[stage]
+	kTcDgMma,      // the rest of the K loop: tau refresh, row constants, MMA issue, wgmma_wait<1> and stage release
+	kTcDgDrain,    // wgmma_wait<0> and the last release
+	kTcDgBar1,     // the first bar.sync
+	kTcDgTest,     // the block test (the scan without its rare path)
+	kTcDgAppend,   // the rare path: the enqueues of the hits (their waits on a full queue included)
+	kTcDgBound,    // unused since the bookkeepers took the bound list off the consumers (the rare path's lock section before)
+	kTcDgBar2,     // the second bar.sync
+	kTcDgTile,     // the whole tile
+	kTcDgBlocks,   // 64-row blocks walked (count, per warp)
+	kTcDgHits,     // (query, row) pairs that passed the block test (count)
+	kTcDgQueueWait,  // enqueues that found the candidate queue full (count)
+	kTcDgPerWg,
+	kTcDgEmpty = 2 * kTcDgPerWg,
+	kTcDgProd = kTcDgEmpty + 2,
+};
+static_assert(kTcDgProd + 2 <= kTcDiagSlots, "diagnostic counters fit their slots");
 
 // shared memory: query block, two stage rings, barriers, per-query constants, then per consumer warpgroup thresholds and (P, R)
 __host__ __device__ inline size_t tc_smem_bytes(uint32_t nq_block, uint32_t kchunks) {
@@ -267,7 +306,7 @@ __device__ __forceinline__ void wgmma_s8(int (&d)[N / 2], uint64_t adesc, uint64
 //   IP, Cosine  x S_v + P M_v + R >= 0               P = n_q / k_q   R = tau / k_q
 //   L2          x S_v + P M_v - Z W_v + R >= 0       Z = 1 / k_q     R = (tau - (1 - eps) n_q^2) / (2 k_q)    W_v = (1 - eps) n_v^2 / 2
 // The test is evaluated as "not below zero", so an overflow to NaN (magnitudes far outside the data the exact scan handles) lets
-// the row through to tc_candidate, which decides with the per-query bound e(q, v) and no division.
+// the row through to the bookkeeper, which decides with the per-query bound e(q, v) and no division.
 __device__ __forceinline__ float tc_l2eps(uint32_t dim) { return kTcL2Eps + float(dim + 1) * 0x1p-23f; }
 __device__ __forceinline__ float2 tc_make_pr(int metric, float tau, float4 qc, float l2eps) {  // qc = (s_q, r_q, n_q, 1 / k_q)
 	const float p = qc.z * qc.w;
@@ -277,73 +316,205 @@ __device__ __forceinline__ float2 tc_make_pr(int metric, float tau, float4 qc, f
 	return make_float2(p, 0.5f * (tau - (1.f - l2eps) * qc.z * qc.z) * qc.w);
 }
 
-// The rare path of the epilogue: row `row` passed the block test for query `q` (x = float(I), qc and rc the query's and the row's
-// constants).  When the row's own bound lb = d~ - e(q, v) passes the threshold it is appended as a candidate, and when its upper
-// bound beats the query's current threshold, it is inserted into the query's global bound list (under the per-query lock; other
-// CTAs contend) and tightens the global tau.  Returns the new threshold (+inf when it did not change).
-// Kept out of line: it runs for a few hundred of 10M rows per query, and inlining it at every accumulator only costs instruction cache.
-__device__ __noinline__ float tc_candidate(const TcArgs& a, uint32_t q, uint32_t row, float x, float4 qc, float4 rc, float tau) {
+// ---- the candidate queue: consumers -> bookkeepers --------------------------------------------------------------------------------
+// A (query, row) pair that passes the block test is a hit.  The consumer warpgroup that found it only enqueues it: one shared-memory
+// atomicAdd takes a ticket, a 16-byte record (query in the block, row, x = float(I), ticket + 1) goes into the warpgroup's ring of
+// `slots` records, the last word stored with release semantics.  Its BOOKKEEPER warp (warp 2 for consumer warpgroup 0, warp 3 for
+// warpgroup 1; idle otherwise) takes the records in ticket order, up to 32 at a time, frees their slots, and runs the rare path off
+// the MMA path: the row's own bound, the candidate append, the bound list and tau.  A full ring makes the consumer wait until the
+// bookkeeper frees a slot; no hit is ever dropped.
+struct TcQueue {
+	uint32_t tail;        // tickets taken by the consumers
+	uint32_t head;        // tickets whose records the bookkeeper has read (their slots are free again)
+	uint32_t done;        // consumer warps that finished their walk
+	uint32_t full_waits;  // diagnostic instantiations: enqueues that found the ring full
+};
+constexpr uint32_t kTcQueueMax = 512;  // records per consumer warpgroup at most (2 x 8 KB), ...
+constexpr uint32_t kTcQueueMin = 128;  // ... and at least: what tc_smem_bytes leaves free under the opt-in limit at every shape
+__host__ __device__ inline size_t tc_queue_bytes(uint32_t slots) { return 2 * sizeof(TcQueue) + size_t(2) * slots * 16; }
+// records per ring: the largest power of two in [kTcQueueMin, kTcQueueMax] whose rings fit beside the layout tc_smem_bytes counts
+// (0: none fits -- tcQueryBlock never picks such a shape)
+inline uint32_t tc_queue_slots(uint32_t nq_block, uint32_t kchunks, size_t limit) {
+	for (uint32_t s = kTcQueueMax; s >= kTcQueueMin; s /= 2) {
+		if (tc_smem_bytes(nq_block, kchunks) + tc_queue_bytes(s) <= limit) {
+			return s;
+		}
+	}
+	return 0;
+}
+
+__device__ __forceinline__ uint32_t ld_acquire_shared(const uint32_t* p) {
+	uint32_t v;
+	asm volatile("ld.acquire.cta.shared::cta.u32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory");
+	return v;
+}
+__device__ __forceinline__ void st_release_shared(uint32_t* p, uint32_t v) {
+	asm volatile("st.release.cta.shared::cta.u32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
+}
+
+// consumer side: returns whether the ring was full (the caller waited)
+__device__ __forceinline__ bool tc_enqueue(TcQueue* qu, uint4* rec, uint32_t slots, uint32_t q, uint32_t row, float x) {
+	const uint32_t t = atomicAdd(&qu->tail, 1u);
+	bool waited = false;
+	while (t - ld_acquire_shared(&qu->head) >= slots) {  // the bookkeeper has not read the record this slot held yet
+		waited = true;
+		__nanosleep(64);
+	}
+	uint4* r = rec + (t & (slots - 1));
+	r->x = q;
+	r->y = row;
+	r->z = __float_as_uint(x);
+	st_release_shared(&r->w, t + 1);
+	return waited;
+}
+
+// the hits of one accumulator quad (h = bits 0..3 for (row0, q), (row0, q + 1), (row1, q), (row1, q + 1)), out of line: inlined at
+// each of the kNq / 8 quads of the unrolled block test it only spreads the test's hot loop over more instruction cache
+__device__ __noinline__ bool tc_enqueue_quad(TcQueue* qu, uint4* rec, uint32_t slots, uint32_t h, uint32_t q, uint32_t row0, uint32_t row1,
+											 float x0, float x1, float x2, float x3) {
+	bool waited = false;
+	if (h & 1u) waited |= tc_enqueue(qu, rec, slots, q, row0, x0);
+	if (h & 2u) waited |= tc_enqueue(qu, rec, slots, q + 1, row0, x1);
+	if (h & 4u) waited |= tc_enqueue(qu, rec, slots, q, row1, x2);
+	if (h & 8u) waited |= tc_enqueue(qu, rec, slots, q + 1, row1, x3);
+	return waited;
+}
+
+// The row's own bound: d~ and its certified error (header comment), from x = float(I) and the query's and the row's constants.
+__device__ __forceinline__ float2 tc_row_bound(const TcArgs& a, float x, float4 qc, float4 rc) {
 	const float p = qc.x * rc.x * x;
 	const float e = (1.f + 0x1p-8f) * fmaf(qc.z + qc.y, rc.y, (qc.y + float(a.dim + 16) * 0x1p-23f * qc.z) * rc.z);
-	float d, err;
 	if (a.metric == kL2) {
-		d = fmaf(-2.f, p, fmaf(qc.z, qc.z, rc.z * rc.z));
-		err = 2.f * e + tc_l2eps(a.dim) * (qc.z * qc.z + rc.z * rc.z);
-	} else if (a.metric == kCos) {
-		d = -p * rc.w;
-		err = e * rc.w;
-	} else {
-		d = -p;
-		err = e;
+		return make_float2(fmaf(-2.f, p, fmaf(qc.z, qc.z, rc.z * rc.z)), 2.f * e + tc_l2eps(a.dim) * (qc.z * qc.z + rc.z * rc.z));
 	}
-	if (d - err > tau) {  // the block test was looser than the row's own bound (NaN: keep the row)
-		return INFINITY;
+	if (a.metric == kCos) {
+		return make_float2(-p * rc.w, e * rc.w);
 	}
-	const unsigned pos = atomicAdd(&a.cand_count[q], 1u);
-	if (pos < a.cand_cap) {
-		a.cand_rows[size_t(q) * a.cand_cap + pos] = row;
+	return make_float2(-p, e);
+}
+
+// Upper bound ub of a candidate row below the query's threshold: insert it into the query's global bound list (under the per-query
+// lock; other CTAs contend) and tighten the global tau.  Returns the list's largest entry afterwards, the query's new threshold.
+__device__ __noinline__ float tc_bound_insert(const TcArgs& a, uint32_t q, float ub) {
+	while (atomicCAS(&a.ub_lock[q], 0u, 1u) != 0u) {
 	}
-	const float ub = d + err;
-	float tightened = INFINITY;
-	if (ub < tau && row >= a.init_rows) {
-		while (atomicCAS(&a.ub_lock[q], 0u, 1u) != 0u) {
+	__threadfence();
+	volatile float* list = a.ub_list + size_t(q) * kTcMaxK1;
+	uint32_t mi = 0;
+	float mx = list[0];
+	for (uint32_t x = 1; x < a.k1; ++x) {
+		const float y = list[x];
+		if (y > mx) {
+			mx = y;
+			mi = x;
 		}
-		__threadfence();
-		volatile float* list = a.ub_list + size_t(q) * kTcMaxK1;
-		uint32_t mi = 0;
-		float mx = list[0];
+	}
+	float tightened = mx;
+	if (ub < mx) {
+		list[mi] = ub;
+		float nmx = list[0];
 		for (uint32_t x = 1; x < a.k1; ++x) {
-			const float y = list[x];
-			if (y > mx) {
-				mx = y;
-				mi = x;
-			}
+			nmx = fmaxf(nmx, list[x]);
 		}
-		if (ub < mx) {
-			list[mi] = ub;
-			float nmx = list[0];
-			for (uint32_t x = 1; x < a.k1; ++x) {
-				nmx = fmaxf(nmx, list[x]);
-			}
-			atomicMin(&a.tau[q], float_ord(nmx));
-			tightened = nmx;
-		} else {
-			tightened = mx;
-		}
-		__threadfence();
-		atomicExch(&a.ub_lock[q], 0u);
+		atomicMin(&a.tau[q], float_ord(nmx));
+		tightened = nmx;
 	}
+	__threadfence();
+	atomicExch(&a.ub_lock[q], 0u);
 	return tightened;
+}
+
+// Bookkeeper warp of one consumer warpgroup's queue, until every consumer warp is done and the ring is empty.  A row is appended
+// when its own lower bound d~ - err passes the tightest threshold the CTA knows for the query (NaN: appended); the appends of one
+// batch go to the candidate lists with one global atomicAdd per distinct query.  When the row's upper bound beats that threshold it
+// goes into the bound list, and the threshold that comes back is published to the (P, R) of BOTH consumer warpgroups.  A consumer may
+// read a looser threshold meanwhile (a concurrent store of another writer may even replace a tighter one): every threshold ever
+// published is a valid upper bound of the query's final k1-th distance, so the test stays certified.
+template <int kNq>
+__device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, const uint4* rec, uint32_t slots, uint32_t q0, const float4* s_qc,
+											  float* s_thr, float2* s_pr, float l2eps, int lane) {
+	uint32_t head = 0;
+	for (;;) {
+		const bool fin = ld_acquire_shared(&qu->done) == 4;  // read before the tail: after it, the tail is final
+		const uint32_t n = __shfl_sync(0xffffffffu, min(ld_acquire_shared(&qu->tail) - head, 32u), 0);
+		if (n == 0) {
+			if (__shfl_sync(0xffffffffu, fin, 0)) {
+				break;
+			}
+			__nanosleep(256);
+			continue;
+		}
+		const bool active = uint32_t(lane) < n;
+		uint32_t ql = 0, row = 0;
+		float x = 0.f;
+		if (active) {
+			const uint32_t t = head + lane;
+			const uint4* r = rec + (t & (slots - 1));
+			while (ld_acquire_shared(&r->w) != t + 1) {  // the consumer holding ticket t has not stored its record yet
+			}
+			ql = r->x;
+			row = r->y;
+			x = __uint_as_float(r->z);
+		}
+		__syncwarp();
+		head += n;
+		if (lane == 0) {
+			st_release_shared(&qu->head, head);  // the records are read: their slots go back to the consumers
+		}
+		float d = 0.f, err = 0.f, tau = 0.f;
+		if (active) {
+			const float4 qc = s_qc[ql], rc = a.rowc[row];
+			const float2 de = tc_row_bound(a, x, qc, rc);
+			d = de.x;
+			err = de.y;
+			tau = fminf(s_thr[ql], s_thr[kNq + ql]);
+		}
+		const bool append = active && !(d - err > tau);
+		const unsigned peers = __match_any_sync(0xffffffffu, append ? ql : ~0u);
+		const int leader = __ffs(peers) - 1;
+		unsigned base = 0;
+		if (append && lane == leader) {
+			base = atomicAdd(&a.cand_count[q0 + ql], unsigned(__popc(peers)));
+		}
+		base = __shfl_sync(0xffffffffu, base, leader);
+		if (append) {
+			const unsigned pos = base + __popc(peers & ((1u << lane) - 1u));
+			if (pos < a.cand_cap) {
+				a.cand_rows[size_t(q0 + ql) * a.cand_cap + pos] = row;
+			}
+			const float ub = d + err;
+			if (ub < tau && row >= a.init_rows) {
+				const float nt = tc_bound_insert(a, q0 + ql, ub);
+				for (uint32_t w = 0; w < 2; ++w) {
+					if (nt < s_thr[w * kNq + ql]) {
+						s_thr[w * kNq + ql] = nt;
+						s_pr[w * kNq + ql] = tc_make_pr(a.metric, nt, s_qc[ql], l2eps);
+					}
+				}
+			}
+		}
+		__syncwarp();
+	}
 }
 
 // ---- the filter kernel -----------------------------------------------------------------------------------------------------------
 // kNq = queries per CTA (wgmma N); kCluster = CTAs that walk the same row tiles with DIFFERENT query blocks, sharing every stage
 // through TMA multicast.
-template <int kNq, int kCluster>
+template <int kNq, int kCluster, int kDiag = 0>
 __global__ void __launch_bounds__(kTcThreads, 1)
 	knn_tc_filter(const __grid_constant__ CUtensorMap map_queries, const __grid_constant__ TcArgs a) {
 	static_assert(kNq % 32 == 0 && kNq <= int(kTcMaxNq), "query block");
 	static_assert(kCluster == 1 || kCluster == 2, "a stage is split in 1 or 2 equal copies");
+	static_assert(kDiag == 0 || kCluster == 1, "the diagnostic instantiations are single CTAs");
+	constexpr bool kStamp = kDiag == kTcDiagStamps;
+	auto clk = [] {  // 0 outside the stamped instantiation, where every stamp and sum below folds away
+		if constexpr (kStamp) {
+			return clock64();
+		} else {
+			return 0ll;
+		}
+	};
+	unsigned long long* dg = kDiag ? a.diag + size_t(blockIdx.x) * kTcDiagSlots : nullptr;
 	extern __shared__ unsigned char smem_raw[];
 	unsigned char* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // offset arithmetic keeps the shared window
 	constexpr uint32_t kQchunkBytes = kNq * 128;                       // one K-chunk of the query block: kNq rows x 128 B
@@ -357,6 +528,8 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 	float4* s_qc = reinterpret_cast<float4*>(bars + 32);               // [kNq] (s_q, r_q, n_q, 1 / k_q)
 	float* s_thr = reinterpret_cast<float*>(s_qc + kNq);               // [2][kNq] current tau (map space), per consumer warpgroup
 	float2* s_pr = reinterpret_cast<float2*>(s_thr + 2 * kNq);         // [2][kNq] (P, R) of the candidate test
+	TcQueue* s_queue = reinterpret_cast<TcQueue*>(s_pr + 2 * kNq);    // [2] candidate queue of each consumer warpgroup
+	uint4* s_rec = reinterpret_cast<uint4*>(s_queue + 2);              // [2][queue_slots] their records (beyond tc_smem_bytes)
 	static_assert(4 * kTcStages + 2 <= 32, "barriers and (a*, b*) fit in front of the per-query constants");
 
 	const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;  // provably warp-uniform
@@ -377,6 +550,16 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		mbar_init(q_bar, 1);
 		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 		s_ab[0] = s_ab[1] = 0.f;
+		s_queue[0] = s_queue[1] = TcQueue{0u, 0u, 0u, 0u};
+	}
+	for (uint32_t i = threadIdx.x; i < 2 * a.queue_slots; i += blockDim.x) {
+		s_rec[i].w = 0u;  // no ticket yet (a record of ticket t carries t + 1)
+	}
+	if constexpr (kDiag == kTcDiagNoFetch) {  // the stages the consumers multiply without a fetch hold zero codes
+		for (uint32_t i = threadIdx.x; i < 2 * kTcStages * kTcBlockBytes / 16; i += blockDim.x) {
+			reinterpret_cast<uint4*>(s_rows)[i] = make_uint4(0u, 0u, 0u, 0u);
+		}
+		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 	}
 	__syncthreads();
 	const float delta = float(a.dim + 16) * 0x1p-23f;
@@ -412,13 +595,23 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		uint64_t* empty = empty_bar + ring * kTcStages;
 		unsigned char* ring_smem = s_rows + size_t(ring) * kTcStages * kTcBlockBytes;
 		uint32_t stage = 0, phase = 0;
+		[[maybe_unused]] long long t_empty = 0;
+		[[maybe_unused]] const long long t_start = clk();
 		for (uint32_t t = walker; t < ntiles; t += walkers) {
 			// the 64-row shadow block 2t + ring, its K chunks 8 KB apart in HBM
 			const unsigned char* src = a.shadow + size_t(2 * t + ring) * a.kchunks * kTcBlockBytes;
 			for (uint32_t kc = 0; kc < a.kchunks; ++kc) {
+				[[maybe_unused]] const long long c0 = clk();
 				mbar_wait(&empty[stage], phase ^ 1);
+				if constexpr (kStamp) {
+					t_empty += clk() - c0;
+				}
 				unsigned char* dst = ring_smem + size_t(stage) * kTcBlockBytes;
-				if (elect_one_sync()) {
+				if constexpr (kDiag == kTcDiagNoFetch) {
+					if (elect_one_sync()) {
+						mbar_arrive(&full[stage]);
+					}
+				} else if (elect_one_sync()) {
 					mbar_expect_tx(&full[stage], kTcBlockBytes);
 					if constexpr (kCluster == 1) {
 						bulk_load(dst, src + size_t(kc) * kTcBlockBytes, kTcBlockBytes, &full[stage]);
@@ -435,11 +628,24 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 				}
 			}
 		}
-	} else if (warp >= 4) {
+		if constexpr (kStamp) {
+			if (lane == 0) {
+				atomicAdd(&dg[kTcDgEmpty + ring], (unsigned long long)t_empty);
+				atomicAdd(&dg[kTcDgProd + ring], (unsigned long long)(clk() - t_start));
+			}
+		}
+	} else if (warp < 4) {
+		// ===== bookkeeper of consumer warpgroup warp - 2 =====
+		const uint32_t wg = uint32_t(warp) - 2;
+		tc_bookkeeper<kNq>(a, s_queue + wg, s_rec + wg * a.queue_slots, a.queue_slots, q0, s_qc, s_thr, s_pr, l2eps, lane);
+	} else {
 		// ===== consumer warpgroup wg: the 64-row blocks 2t + wg of the walker's tiles t, through ring wg =====
 		const uint32_t wg = uint32_t(warp) / 4 - 1, wtid = threadIdx.x - 128 * (wg + 1);
 		float* thr = s_thr + wg * kNq;
 		float2* pr = s_pr + wg * kNq;
+		TcQueue* qu = s_queue + wg;
+		uint4* rec = s_rec + wg * a.queue_slots;
+		const uint32_t slots = a.queue_slots;
 		uint64_t* full = full_bar + wg * kTcStages;
 		uint64_t* empty = empty_bar + wg * kTcStages;
 		const unsigned char* ring_smem = s_rows + size_t(wg) * kTcStages * kTcBlockBytes;
@@ -460,7 +666,19 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		};
 		mbar_wait(q_bar, 0);
 		uint32_t stage = 0, phase = 0;
+		[[maybe_unused]] long long dt[kTcDgPerWg] = {};  // kStamp: this warp's cycles per phase (kTcDg*)
+		[[maybe_unused]] unsigned long long nhits = 0;
 		for (uint32_t t = walker; t < ntiles; t += walkers) {
+			[[maybe_unused]] const uint32_t walk = (t - walker) / walkers;
+			[[maybe_unused]] long long s0 = clk(), s1, s2, s3, s4, rare = 0;
+			if constexpr (kStamp) {
+				if (wg == 0 && wtid == 0 && walk % kTcDiagMarkEvery == 0 && walk < kTcDiagWalk) {
+					unsigned long long now;
+					asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+					a.diag[size_t(gridDim.x) * kTcDiagSlots + kTcDiagWalk + size_t(blockIdx.x) * (kTcDiagWalk / kTcDiagMarkEvery) +
+						   walk / kTcDiagMarkEvery] = now;
+				}
+			}
 			// refresh tau from the other CTAs: the global load was issued during the PREVIOUS tile, so its latency is hidden
 			if (my_q < nq_valid) {
 				const float tn = ord_float(tau_ahead);
@@ -479,7 +697,11 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 			}
 			uint32_t prev = 0;
 			for (uint32_t kc = 0; kc < a.kchunks; ++kc) {
+				[[maybe_unused]] const long long c0 = clk();
 				mbar_wait(&full[stage], phase);
+				if constexpr (kStamp) {
+					dt[kTcDgFull] += clk() - c0;
+				}
 				const uint32_t a_addr = smem_u32(ring_smem + size_t(stage) * kTcBlockBytes);
 				const uint32_t b_addr = smem_u32(s_q + size_t(kc) * kQchunkBytes);
 				wgmma_fence();
@@ -500,19 +722,14 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 					phase ^= 1;
 				}
 			}
+			s1 = clk();
 			wgmma_wait<0>();
 			if (lane == 0) {
 				release(prev);
 			}
+			s2 = clk();
 			asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // the refreshed (P, R) of all queries are visible
-			// a tightened threshold takes effect at once for the rest of the tile: other threads of the warpgroup may store a looser one
-			// for the same query concurrently, which is still a valid upper bound (each store is a single aligned store)
-			auto tighten = [&](uint32_t qq, float nt) {
-				if (nt < thr[qq]) {
-					thr[qq] = nt;
-					pr[qq] = tc_make_pr(a.metric, nt, s_qc[qq], l2eps);
-				}
-			};
+			s3 = clk();
 			// per-row factors of the block test (rows beyond n have all-zero constants and are masked anyway)
 			const float S0 = rc0.x * rc0.w, S1 = rc1.x * rc1.w;
 			const float M0 = rc0.w * fmaf(ka, rc0.y, kb * rc0.z), M1 = rc1.w * fmaf(ka, rc1.y, kb * rc1.z);
@@ -537,24 +754,77 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 					const bool h1 = ok0 && !(fmaf(x1, S0, fmaf(p2.z, M0, Rb)) < 0.f);
 					const bool h2 = ok1 && !(fmaf(x2, S1, fmaf(p2.x, M1, Rc)) < 0.f);
 					const bool h3 = ok1 && !(fmaf(x3, S1, fmaf(p2.z, M1, Rd)) < 0.f);
-					if (h0 | h1 | h2 | h3) {  // rare path: the row's own bound, candidate append, threshold tightening
-						if (h0) tighten(q, tc_candidate(a, q0 + q, row0, x0, s_qc[q], rc0, thr[q]));
-						if (h1) tighten(q + 1, tc_candidate(a, q0 + q + 1, row0, x1, s_qc[q + 1], rc0, thr[q + 1]));
-						if (h2) tighten(q, tc_candidate(a, q0 + q, row1, x2, s_qc[q], rc1, thr[q]));
-						if (h3) tighten(q + 1, tc_candidate(a, q0 + q + 1, row1, x3, s_qc[q + 1], rc1, thr[q + 1]));
+					if (h0 | h1 | h2 | h3) {  // rare path: hand the hits to the bookkeeper
+						if constexpr (kDiag != 0) {
+							nhits += uint32_t(h0) + uint32_t(h1) + uint32_t(h2) + uint32_t(h3);
+						}
+						if constexpr (kDiag != kTcDiagNoRare) {
+							[[maybe_unused]] const long long r = clk();
+							const bool waited = tc_enqueue_quad(qu, rec, slots, uint32_t(h0) | uint32_t(h1) << 1 | uint32_t(h2) << 2 | uint32_t(h3) << 3,
+																q, row0, row1, x0, x1, x2, x3);
+							if constexpr (kStamp) {
+								rare += clk() - r;
+								if (waited) {
+									atomicAdd(&qu->full_waits, 1u);
+								}
+							}
+						}
 					}
 				}
 			};
+			[[maybe_unused]] const unsigned long long hits_before = nhits;
 			if (l2) {
 				scan(std::true_type{});
 			} else {
 				scan(std::false_type{});
 			}
-			__syncwarp();  // the rare path diverges (per-lane lock loops): reconverge before the .aligned wgmma of the next tile
+			__syncwarp();  // the rare path diverges (per-lane queue waits): reconverge before the .aligned wgmma of the next tile
+			s4 = clk();
 			asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // nobody still reads (P, R) when the next refresh writes them
+			if constexpr (kStamp) {
+				// the warp's rare path time: its slowest lane (the lanes of a diverged warp run one after another)
+				const long long rare_w = __reduce_max_sync(0xffffffffu, uint32_t(rare));
+				const long long s5 = clk();
+				dt[kTcDgMma] += s1 - s0;
+				dt[kTcDgDrain] += s2 - s1;
+				dt[kTcDgBar1] += s3 - s2;
+				dt[kTcDgTest] += (s4 - s3) - rare_w;
+				dt[kTcDgAppend] += rare_w;
+				dt[kTcDgBar2] += s5 - s4;
+				dt[kTcDgTile] += s5 - s0;
+				dt[kTcDgBlocks] += 1;
+				const uint32_t h = __reduce_add_sync(0xffffffffu, uint32_t(nhits - hits_before));
+				if (lane == 0 && h && walk < kTcDiagWalk) {
+					atomicAdd(&a.diag[size_t(gridDim.x) * kTcDiagSlots + walk], (unsigned long long)h);
+				}
+			}
+		}
+		__syncwarp();
+		if (lane == 0) {  // this warp's tickets are all taken: once all four warps are done, the bookkeeper drains and leaves
+			__threadfence_block();
+			atomicAdd(&qu->done, 1u);
+		}
+		if constexpr (kDiag != 0) {
+			const uint32_t h = __reduce_add_sync(0xffffffffu, uint32_t(nhits));
+			if (lane == 0) {
+				atomicAdd(&dg[wg * kTcDgPerWg + kTcDgHits], (unsigned long long)h);
+				if constexpr (kStamp) {
+					dt[kTcDgMma] -= dt[kTcDgFull];  // the K loop's waits are counted on their own
+					for (uint32_t i = 0; i < kTcDgPerWg; ++i) {
+						if (i != kTcDgHits) {
+							atomicAdd(&dg[wg * kTcDgPerWg + i], (unsigned long long)dt[i]);
+						}
+					}
+				}
+			}
 		}
 	}
-	__syncthreads();
+	__syncthreads();  // every bookkeeper has drained its queue
+	if constexpr (kStamp) {
+		if (threadIdx.x < 2) {
+			dg[threadIdx.x * kTcDgPerWg + kTcDgQueueWait] = s_queue[threadIdx.x].full_waits;
+		}
+	}
 	if constexpr (kCluster > 1) {
 		cluster_sync_all();  // nobody leaves while a peer may still multicast into this CTA or signal its barriers
 	}
