@@ -362,7 +362,8 @@ int rxgpu_ivf_list_stats(const rxgpu_index*, uint64_t* slab_rows, uint64_t* dead
  * document statistics = the DocsStatsGetter duck-type (index/indextext/indextext.h:245-258), FTConfig members the merger reads
  * (ft/config/ftconfig.h:118-236), query parts = TermResults/SubtermResults + FtDslOpts (ft_fast/querymergedata.h, ft/ftdsl.h:13-30).
  * Output = ft::MergeData (ft_fast/phrasemerger.h:57-78), bit-identical to the reference: same docs, same order for
- * RankAndID / IDOnly, same uint8 ranks, same field. */
+ * RankAndID / IDOnly, same uint8 ranks, same field; rxgpu_ft_merge_query_areas adds the highlight areas of
+ * ft::MergeDataAreas<Area> for queries without phrases. */
 typedef struct {
 	uint32_t ndocs;
 	const uint32_t* doc_ids;   /* ascending vdoc ids, >= 1 (vdoc 0 is the reference's dummy, mergerimpl.h:122) */
@@ -449,6 +450,19 @@ int rxgpu_ft_merge(rxgpu_ft_index*, const rxgpu_ft_config* cfg, uint32_t nterms,
  * a document that holds all terms of one of its synonyms (buildRestrictingBitmask, :352-363). */
 int rxgpu_ft_merge_query(rxgpu_ft_index*, const rxgpu_ft_config* cfg, const rxgpu_ft_query* query, const uint8_t* excluded, int rank_sort_type,
 						 uint64_t max_out, rxgpu_ft_merge_info* out, uint64_t* out_n);
+/* The same merge with highlight areas: ft::Merger<IdCont, ft::MergeDataAreas<Area>, OffsetT> (ft_fast/merger.h:196-205,
+ * core/ft/areaholder.h), what IndexText asks for when the query's context is kFtArea (highlight() / snippet()).  `out` is
+ * bit-identical to rxgpu_ft_merge_query's.  For returned entry i and field f its committed areas (AreasInDocument::GetAreas(f), ordered
+ * by start) are out_areas[out_area_begin[i * nfields + f] .. out_area_begin[i * nfields + f + 1]); out_area_begin holds
+ * min(*out_n, max_out) * nfields + 1 offsets, out_areas has room for max_out * nfields * max_areas_in_doc entries.  out_raw_count (max_out
+ * entries, or NULL) = GetAreasCount() before the commit.  max_areas_in_doc = FTConfig::maxAreasInDoc, in [1, 64]; outside that range,
+ * or for a query with a phrase, the call returns errParams and changes nothing. */
+typedef struct {
+	uint32_t start, end; /* Area(start, end, arrayIdx = 0) */
+} rxgpu_ft_area;
+int rxgpu_ft_merge_query_areas(rxgpu_ft_index*, const rxgpu_ft_config* cfg, const rxgpu_ft_query* query, const uint8_t* excluded,
+							   int rank_sort_type, int32_t max_areas_in_doc, uint64_t max_out, rxgpu_ft_merge_info* out,
+							   uint32_t* out_area_begin, rxgpu_ft_area* out_areas, uint32_t* out_raw_count, uint64_t* out_n);
 /* IndexText::afterSelect + sortAfterSelect on top of the merge, without leaving the device (core/index/indextext/indextext.cc:480-611;
  * Merger::postProcessResults, ft_fast/merger.h:111-155): ranks below min_rank are dropped, the rest is normalised to uint8 by the
  * global maximum, every merged vdoc expands to its row ids, rows whose external status is 0 are skipped (FtUseExternStatuses::Yes),

@@ -178,6 +178,8 @@ _SIGNATURES = {
                                  C.POINTER(C.c_uint64)]),
     "rxgpu_ft_add_postings_packed_batch": (C.c_int, [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), _u32p, _u32p]),
     "rxgpu_ft_merge_query": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, _u8p, C.c_int, C.c_uint64, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "rxgpu_ft_merge_query_areas": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, _u8p, C.c_int, C.c_int32, C.c_uint64, C.c_void_p, _u32p,
+                                              C.c_void_p, _u32p, C.POINTER(C.c_uint64)]),
     "rxgpu_ft_select_query": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, _u8p, _u8p, C.c_int, C.c_uint64, _i32p, _f32p,
                                          C.POINTER(C.c_uint64)]),
     "rxgpu_ft_set_rows": (C.c_int, [C.c_void_p, _u32p, _i32p]),
@@ -750,6 +752,28 @@ class GpuFtIndex:
             _check(self._lib.rxgpu_ft_merge(self._h, C.byref(c), len(terms), arr, None if ex is None else _p(ex, _u8p), rank_sort_type,
                                             max_out, out.ctypes.data, C.byref(n)))
         return out[:min(n.value, max_out)].copy()
+
+    def merge_areas(self, cfg: dict, field_cfg: list, terms: list, max_areas_in_doc=5, excluded=None, rank_sort_type=1, max_out=None,
+                    synonyms=None):
+        """merge() with highlight areas (rxgpu_ft_merge_query_areas, MergeDataAreas<Area>): returns (infos, begin, areas, raw).  For
+        entry i and field f the committed areas are areas[begin[i * nfields + f]:begin[i * nfields + f + 1]] as (start, end) rows;
+        raw[i] = the document's area count before the commit."""
+        c, arr, keep = self._config_and_terms(cfg, field_cfg, terms)
+        q = self._query(arr, len(terms), synonyms or [], keep)
+        ex = None if excluded is None else np.ascontiguousarray(excluded, np.uint8)
+        max_out = self.total_docs if max_out is None else max_out
+        out = np.zeros(max(max_out, 1), FT_MERGE_INFO_DTYPE)
+        a = min(max(int(max_areas_in_doc), 1), 64)
+        begin = np.zeros(max(max_out, 1) * self.nfields + 1, np.uint32)
+        areas = np.zeros((max(max_out * self.nfields * a, 1), 2), np.uint32)
+        raw = np.zeros(max(max_out, 1), np.uint32)
+        n = C.c_uint64(0)
+        _check(self._lib.rxgpu_ft_merge_query_areas(self._h, C.byref(c), C.byref(q), None if ex is None else _p(ex, _u8p), rank_sort_type,
+                                                    int(max_areas_in_doc), max_out, out.ctypes.data, _p(begin, _u32p), areas.ctypes.data,
+                                                    _p(raw, _u32p), C.byref(n)))
+        m = min(n.value, max_out)
+        begin = begin[:m * self.nfields + 1].copy()
+        return out[:m].copy(), begin, areas[:int(begin[-1])].copy(), raw[:m].copy()
 
     def _query(self, arr, nterms, synonyms, keep):
         syn = (FtSynonym * len(synonyms))()
