@@ -110,7 +110,8 @@ int rxgpu_last_range_results(uint64_t offset, uint64_t n, float* out_dist, uint6
  * internal index (insertion order with swap-deletes, as in the reference).  No tie replay is applied here. */
 int rxgpu_search_knn_device(const rxgpu_index*, uint32_t nq, const float* d_queries, uint32_t k1, float* d_out_dist,
 							uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count, void* stream);
-/* rows with dist <= dstar in internal order: the first k of them (device in/out, one query); feeds the tie replay */
+/* rows with dist <= dstar (a float compare: -0 == +0) in internal order: the first k of them (device in/out, one query); feeds the
+ * tie replay.  *d_out_count = min(k, number of such rows); d_out_* hold k entries, of which the first *d_out_count are written. */
 int rxgpu_search_tie_rows_device(const rxgpu_index*, const float* d_query, float dstar, uint32_t k, float* d_out_dist,
 								 uint32_t* d_out_idx, uint64_t* d_out_label, uint32_t* d_out_count, void* stream);
 
@@ -155,7 +156,9 @@ int rxgpu_comm_rank(const rxgpu_comm*);
 int rxgpu_comm_size(const rxgpu_comm*);
 /* collective: every rank calls it with its own shard and the SAME queries / k.  queries: nq x dim floats, host pointer
  * (queries_on_device == 0) or device pointer on the shard's GPU (!= 0).  Outputs: host buffers nq x k, best first, reference tie rule
- * applied globally; out_count[q] = min(k, total rows). */
+ * applied globally; out_count[q] = min(k, total rows).  k must be at most 65535 even when all shards together hold fewer rows (a rank
+ * does not know the others' sizes before it scans; rxgpu_search_knn clamps k to its size first): a larger k fails with
+ * RXGPU_ERR_PARAMS. */
 int rxgpu_sharded_search_knn(rxgpu_comm*, const rxgpu_index* shard, uint32_t nq, const float* queries, int queries_on_device, uint32_t k,
 							 float* out_dist, uint64_t* out_label, uint32_t* out_count);
 /* collective: every rank calls it with its own shard and the SAME queries / radius / max_out.  Per query q the result on EVERY rank is

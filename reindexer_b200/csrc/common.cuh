@@ -55,6 +55,12 @@ __host__ __device__ __forceinline__ float ord_float(uint32_t o) {
 #endif
 }
 __host__ __device__ __forceinline__ uint64_t make_key(float dist, uint32_t row) { return (uint64_t(float_ord(dist)) << 32) | row; }
+// the distance of a key.  Keys hold a zero distance as +0, but the exact arithmetic gives -(+0) = -0 for an inner-product or cosine row
+// whose dot product is zero -- as the reference's DistCalculator::ip does -- and +0 for L2: neg_zero (metric != L2) restores the sign
+__host__ __device__ __forceinline__ float key_dist(uint32_t o, bool neg_zero) {
+	const float f = ord_float(o);
+	return neg_zero && f == 0.f ? -0.f : f;
+}
 
 enum Metric : int { kL2 = 0, kIP = 1, kCos = 2 };
 enum ScanMode : int { kModeTopK = 0, kModeTieRows = 1 };

@@ -197,6 +197,7 @@ int scanTopKExact(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const f
 			m.out_stride = k1;
 			m.out_offset = round * kr;
 			m.mode = mode;
+			m.neg_zero = ix->metric != RXGPU_L2;
 			knn_merge_lists<<<a.nq, 256, 0, st>>>(m);
 			RX_CUDA(cudaGetLastError());
 			g_stats.launches += 2;
@@ -589,6 +590,7 @@ int scanTopKStaged(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const 
 	s.out_idx = d_out_idx;
 	s.out_label = d_out_label;
 	s.out_count = d_out_count;
+	s.neg_zero = ix->metric != RXGPU_L2;
 	do {
 		rows = uint32_t(std::min<uint64_t>(size, uint64_t(rows) * kStageRatio));
 		if (int rc = tcLaunch(ix, ws, st, b, k1, cap, rows, true)) {
@@ -661,6 +663,7 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 	m.out_stride = k1;
 	m.out_offset = 0;
 	m.mode = kModeTopK;
+	m.neg_zero = ix->metric != RXGPU_L2;
 	knn_merge_lists<<<nq, 256, 0, st>>>(m);
 	RX_CUDA(cudaGetLastError());
 	g_stats.launches += 2;
@@ -790,6 +793,7 @@ int tieRowsAfterScan(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, cons
 		s.out_idx = d_out_idx;
 		s.out_label = d_out_label;
 		s.out_count = d_out_count;
+		s.neg_zero = ix->metric != RXGPU_L2;
 		knn_select_topk<<<nsel, kSelThreads, 0, st>>>(s);
 		RX_CUDA(cudaGetLastError());
 		g_stats.launches += 1;
@@ -825,6 +829,7 @@ int tieRowsAfterScan(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, cons
 	m.out_stride = k;
 	m.out_offset = 0;
 	m.mode = kModeTieRows;
+	m.neg_zero = ix->metric != RXGPU_L2;
 	knn_merge_lists<<<nsel, 256, 0, st>>>(m);
 	RX_CUDA(cudaGetLastError());
 	g_stats.launches += 2;

@@ -356,6 +356,7 @@ struct MergeArgs {
 	uint32_t out_stride;   // result slots per query
 	uint32_t out_offset;   // first slot of this round
 	int mode;
+	bool neg_zero;         // key_dist: zero distances come out as -0 (inner product, cosine)
 };
 
 __global__ void __launch_bounds__(256) knn_merge_lists(const MergeArgs a) {
@@ -415,10 +416,10 @@ __global__ void __launch_bounds__(256) knn_merge_lists(const MergeArgs a) {
 		uint32_t idx;
 		if (a.mode == kModeTieRows) {
 			idx = uint32_t(b >> 32);
-			dist = ord_float(uint32_t(b));
+			dist = key_dist(uint32_t(b), a.neg_zero);
 		} else {
 			idx = uint32_t(b);
-			dist = ord_float(uint32_t(b >> 32));
+			dist = key_dist(uint32_t(b >> 32), a.neg_zero);
 		}
 		a.out_dist[ob + r] = dist;
 		a.out_idx[ob + r] = idx;

@@ -1001,6 +1001,7 @@ struct SelectArgs {
 	uint32_t* out_idx;
 	uint64_t* out_label;           // may be null
 	uint32_t* out_count;
+	bool neg_zero;                 // key_dist: zero distances come out as -0 (inner product, cosine)
 };
 
 // One CTA per query: the k1 smallest of the query's unordered key region, ascending, in time linear in the region.  A radix select on
@@ -1137,7 +1138,7 @@ __global__ void __launch_bounds__(kSelThreads) knn_select_topk(const SelectArgs 
 	for (uint32_t r = threadIdx.x; r < m; r += kSelThreads) {
 		const uint64_t k = s_keys[r];
 		const uint32_t idx = tie ? uint32_t(k >> 32) : uint32_t(k);
-		a.out_dist[ob + r] = ord_float(tie ? uint32_t(k) : uint32_t(k >> 32));
+		a.out_dist[ob + r] = key_dist(tie ? uint32_t(k) : uint32_t(k >> 32), a.neg_zero);
 		a.out_idx[ob + r] = idx;
 		if (a.out_label) {
 			a.out_label[ob + r] = a.labels[idx];

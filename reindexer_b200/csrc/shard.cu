@@ -617,7 +617,7 @@ int rxgpu_sharded_search_knn(rxgpu_comm* c, const rxgpu_index* ix, uint32_t nq, 
 		g_stats.tc_kernel = scanStats.tc_kernel;
 		g_stats.tc_candidates = scanStats.tc_candidates;
 		g_stats.tc_fallbacks = scanStats.tc_fallbacks;
-		g_stats.launches = after.launches + 1 + (tieQ.empty() ? 0 : 0);
+		g_stats.launches = after.launches + 1;
 		g_stats.tie_replays = uint32_t(tieQ.size());
 	} catch (const std::bad_alloc&) {
 		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
