@@ -379,11 +379,13 @@ int tcPrepare(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float
 	const uint32_t nqPad = ngroups * cluster * nqb;
 	RX_CUDA(ws.d_qcodes.ensure(size_t(nqPad) * pitchQ));
 	RX_CUDA(ws.d_qc.ensure(nqPad));
+	RX_CUDA(ws.d_qf.ensure(size_t(nqPad) * pitchQ));
 	RX_CUDA(ws.d_tau.ensure(nqPad));
 	RX_CUDA(ws.d_cand_count.ensure(nqPad));
 	RX_CUDA(ws.d_cand_rows.ensure(size_t(nqPad) * candCap));
 	RX_CUDA(ws.h_cand_count.ensure(nqPad));
-	tc_prepare_queries<<<(nqPad * 32 + 255) / 256, 256, 0, st>>>(d_queries, nq, nqPad, ix->dim, pitchQ, ws.d_qcodes.p, ws.d_qc.p);
+	tc_prepare_queries<<<(nqPad * 32 + 255) / 256, 256, 0, st>>>(d_queries, nq, nqPad, ix->dim, pitchQ, ws.d_qcodes.p, ws.d_qc.p,
+																 ws.d_qf.p);
 	g_stats.launches += 1;
 	RX_CUDA(cudaGetLastError());
 	if (int rc = makeCodeMap(&b.mapQ, ws.d_qcodes.p, pitchQ, nqPad, nqb)) {
@@ -431,7 +433,8 @@ int tcPrepare(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float
 // The filter launches of a prepared batch over the rows [0, nrows), with the thresholds already in ws.d_tau: the rows whose certified
 // lower bound is at or below the query's threshold tau go to ws.d_cand_rows[q][candCap], and ws.d_cand_count[q] counts them all (also
 // past candCap: an overflowed list).  fixedTau: init_rows = UINT32_MAX keeps every row out of the bound list, so tau never moves
-// (knn_tc.cuh header comment) and k1 is not used; otherwise tau tightens to the k1-th best upper bound from tc_init_tau's list.
+// (knn_tc.cuh header comment) and k1 is not used; otherwise tau tightens to the k1-th best exact distance of the bound list that
+// tc_init_tau seeded.
 int tcLaunch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const TcBatch& b, uint32_t k1, uint32_t candCap, uint32_t nrows, bool fixedTau) {
 	const uint32_t nq = b.nq, nqb = b.nqb, cluster = b.cluster, ngroups = b.ngroups, kchunks = b.kchunks, pitchQ = ix->pitch_q;
 	const uint32_t ntiles = (nrows + kTcTileRows - 1) / kTcTileRows;
@@ -459,6 +462,10 @@ int tcLaunch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const TcBatc
 	a.ub_list = fixedTau ? nullptr : ws.d_ub_list.p;
 	a.ub_lock = fixedTau ? nullptr : ws.d_ub_lock.p;
 	a.init_rows = fixedTau ? UINT32_MAX : uint32_t(std::min<uint64_t>(ix->size, kTcInitRows));
+	a.rows = ix->d_rows;
+	a.norm_coefs = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
+	a.qf = ws.d_qf.p;
+	a.pitch = ix->pitch;
 	a.cand_rows = ws.d_cand_rows.p;
 	a.cand_count = ws.d_cand_count.p;
 	a.cand_cap = candCap;
@@ -505,7 +512,7 @@ int tcLaunch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const TcBatc
 }
 
 // The candidate filter over a whole batch and all rows.  KNN (h_tau == nullptr): tau starts from tc_init_tau and tightens to the k1-th
-// best upper bound.  Range search: h_tau[q] = float_ord(radius) fixes tau.
+// best exact distance of the bound list.  Range search: h_tau[q] = float_ord(radius) fixes tau.
 int tcFilter(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1, uint32_t candCap,
 			 const unsigned int* h_tau) {
 	TcBatch b;
@@ -517,10 +524,10 @@ int tcFilter(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float*
 	} else {
 		RX_CUDA(ws.d_ub_list.ensure(size_t(b.nqPad) * kTcMaxK1));
 		RX_CUDA(ws.d_ub_lock.ensure(b.nqPad));
-		RX_CUDA(raiseSmemCeilingOnce(tc_init_tau, ix->device, int(tc_init_smem_bytes(2048))));
-		tc_init_tau<<<(nq + kTcInitQ - 1) / kTcInitQ, 256, tc_init_smem_bytes(ix->pitch), st>>>(
-			ix->d_rows, ix->pitch, ix->dim, ix->metric == RXGPU_COS ? ix->d_norms : nullptr, uint32_t(std::min<uint64_t>(ix->size, kTcInitRows)),
-			d_queries, nq, k1, ix->metric, ws.d_tau.p, ws.d_ub_list.p, ws.d_ub_lock.p);
+		RX_CUDA(raiseSmemCeilingOnce(tc_init_tau, ix->device, int(tc_init_smem_bytes())));
+		tc_init_tau<<<(nq + kTcInitQ - 1) / kTcInitQ, 256, tc_init_smem_bytes(), st>>>(
+			ix->d_rows, ix->pitch, b.kchunks, ix->metric == RXGPU_COS ? ix->d_norms : nullptr, uint32_t(std::min<uint64_t>(ix->size, kTcInitRows)),
+			ws.d_qf.p, nq, k1, ix->metric, ws.d_tau.p, ws.d_ub_list.p, ws.d_ub_lock.p);
 		g_stats.launches += 1;
 	}
 	return tcLaunch(ix, ws, st, b, k1, candCap, uint32_t(ix->size), h_tau != nullptr);

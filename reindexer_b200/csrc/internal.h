@@ -138,6 +138,7 @@ struct Workspace {
 	PinBuf<unsigned int> h_range_n;
 	DevBuf<unsigned char> d_qcodes;  // int8 query codes for the tensor-core filter
 	DevBuf<float4> d_qc;             // their per-query constants (s_q, r_q, ||q||, 1 / k_q)
+	DevBuf<float> d_qf;              // the fp32 queries zero padded to the codes' pitch (exact distances of the bound list)
 	DevBuf<unsigned int> d_tau, d_cand_count, d_ub_lock;
 	DevBuf<float> d_ub_list;
 	DevBuf<uint32_t> d_cand_rows;

@@ -435,39 +435,85 @@ __global__ void __launch_bounds__(256) knn_merge_lists(const MergeArgs a) {
 	}
 }
 
-// ---- IVF ----------------------------------------------------------------------------------------------------------------
-// distance of one row to the query staged in sq4, all lanes return the sum: the per-row arithmetic of knn_scan_warp (per-lane
-// sequential FMA over the 128-float chunks, then the xor butterfly), so a row's distance has the same bits on every path
-template <bool kIsL2>
-__device__ __forceinline__ float row_dist_warp(const float4* rows4, uint32_t pitch4, uint32_t nch, uint32_t row, const float4* sq4, int lane) {
-	float s = 0.f;
+// ---- one exact distance outside the scan ------------------------------------------------------------------------------------
+// The per-row arithmetic of knn_scan_warp for every other exact fp32 distance (knn_rerank, the IVF coarse quantiser, the int8
+// filter's seed and its bookkeepers): lane l accumulates float4 #l of every 128-float chunk, chunk after chunk, with sequential FMAs
+// (x, y, z, w); an xor butterfly adds the lanes; then the sign (inner product, cosine) and the row's Cosine norm coefficient
+// (norm_coefs != nullptr).  So a row's distance has the same bits on every path: the tie rule needs that, and the filter's bound list
+// holds the exact scan's own distances.  R rows x Q queries at once: row r against the queries q4[r][0, Q) (zero padded to nch * 128
+// floats), the R rows' loads of a chunk in flight together and each row read once for its Q queries.  Every lane returns every distance.
+template <bool kIsL2, int R, int Q>
+__device__ __forceinline__ void row_dists_warp(const float4* rows4, uint32_t pitch4, uint32_t nch, const uint32_t (&row)[R],
+											   const float4* const (&q4)[R][Q], const float* norm_coefs, int lane, float (&dist)[R][Q]) {
+	float s[R][Q];
+#pragma unroll
+	for (int r = 0; r < R; ++r) {
+#pragma unroll
+		for (int j = 0; j < Q; ++j) {
+			s[r][j] = 0.f;
+		}
+	}
 	for (uint32_t c = 0; c < nch; ++c) {
 		const uint32_t f4 = c * 32u + lane;
-		const float4 v = f4 < pitch4 ? ldg_stream(rows4 + size_t(row) * pitch4 + f4) : make_float4(0.f, 0.f, 0.f, 0.f);
-		const float4 q = sq4[f4];
-		if constexpr (kIsL2) {
-			float d;
-			d = q.x - v.x;
-			s = fmaf(d, d, s);
-			d = q.y - v.y;
-			s = fmaf(d, d, s);
-			d = q.z - v.z;
-			s = fmaf(d, d, s);
-			d = q.w - v.w;
-			s = fmaf(d, d, s);
-		} else {
-			s = fmaf(q.x, v.x, s);
-			s = fmaf(q.y, v.y, s);
-			s = fmaf(q.z, v.z, s);
-			s = fmaf(q.w, v.w, s);
+		float4 v[R];
+#pragma unroll
+		for (int r = 0; r < R; ++r) {
+			v[r] = f4 < pitch4 ? ldg_stream(rows4 + size_t(row[r]) * pitch4 + f4) : make_float4(0.f, 0.f, 0.f, 0.f);
+		}
+#pragma unroll
+		for (int r = 0; r < R; ++r) {
+#pragma unroll
+			for (int j = 0; j < Q; ++j) {
+				const float4 q = q4[r][j][f4];
+				if constexpr (kIsL2) {
+					float d;
+					d = q.x - v[r].x;
+					s[r][j] = fmaf(d, d, s[r][j]);
+					d = q.y - v[r].y;
+					s[r][j] = fmaf(d, d, s[r][j]);
+					d = q.z - v[r].z;
+					s[r][j] = fmaf(d, d, s[r][j]);
+					d = q.w - v[r].w;
+					s[r][j] = fmaf(d, d, s[r][j]);
+				} else {
+					s[r][j] = fmaf(q.x, v[r].x, s[r][j]);
+					s[r][j] = fmaf(q.y, v[r].y, s[r][j]);
+					s[r][j] = fmaf(q.z, v[r].z, s[r][j]);
+					s[r][j] = fmaf(q.w, v[r].w, s[r][j]);
+				}
+			}
 		}
 	}
 #pragma unroll
-	for (int off = 16; off > 0; off >>= 1) {
-		s += __shfl_xor_sync(0xffffffffu, s, off);
+	for (int r = 0; r < R; ++r) {
+		const float coef = !kIsL2 && norm_coefs != nullptr ? norm_coefs[row[r]] : 1.f;
+#pragma unroll
+		for (int j = 0; j < Q; ++j) {
+			float t = s[r][j];
+#pragma unroll
+			for (int off = 16; off > 0; off >>= 1) {
+				t += __shfl_xor_sync(0xffffffffu, t, off);
+			}
+			t = kIsL2 ? t : -t;
+			if (!kIsL2 && norm_coefs != nullptr) {
+				t *= coef;  // Cosine: hnswlib.h:160-161
+			}
+			dist[r][j] = t;
+		}
 	}
-	return kIsL2 ? s : -s;
 }
+// one row against the query staged in sq4
+template <bool kIsL2>
+__device__ __forceinline__ float row_dist_warp(const float4* rows4, uint32_t pitch4, uint32_t nch, uint32_t row, const float4* sq4,
+											   const float* norm_coefs, int lane) {
+	const uint32_t r[1] = {row};
+	const float4* const q[1][1] = {{sq4}};
+	float d[1][1];
+	row_dists_warp<kIsL2, 1, 1>(rows4, pitch4, nch, r, q, norm_coefs, lane, d);
+	return d[0][0];
+}
+
+// ---- IVF ----------------------------------------------------------------------------------------------------------------
 // coarse quantiser (faiss::IndexIVF::search -> quantizer->search(nprobe), IndexIVF.cpp): one CTA per query computes the distance to
 // every centroid (a warp per centroid) and selects the nprobe nearest under (distance, centroid id); then it emits the work items
 // of the list scan, probe-major: work[p * nq + q] = (q, list_begin[c], list_begin[c + 1], c)
@@ -491,10 +537,8 @@ __global__ void __launch_bounds__(kScanThreads) ivf_coarse_kernel(const float* c
 	__syncthreads();
 	const float4* rows4 = reinterpret_cast<const float4*>(centroids);
 	for (uint32_t c = warp; c < nlist; c += kScanWarps) {
-		float d = row_dist_warp<kIsL2>(rows4, pitch4, nch, c, sq4, lane);
-		if (!kIsL2 && centroid_norm_coefs != nullptr) {
-			d *= centroid_norm_coefs[c];  // IndexFlatCosine: knn_cosine = IP * norm coefficient of the centroid
-		}
+		// IndexFlatCosine: knn_cosine = IP * norm coefficient of the centroid
+		const float d = row_dist_warp<kIsL2>(rows4, pitch4, nch, c, sq4, centroid_norm_coefs, lane);
 		if (lane == 0) {
 			keys[c] = make_key(d, c);
 		}

@@ -2,7 +2,7 @@
 //
 // knn_scan_warp is HBM-bound only while <= ~16 queries share a pass; a batch of 1024 queries is FMA-bound there.  This kernel
 // computes APPROXIMATE scores for a block of NQ queries against every row with int8 operands on the tensor cores and keeps, per
-// query, only the rows that can still be among the k best under a CERTIFIED error bound; the survivors (~1 600 per query at config 1)
+// query, only the rows that can still be among the k best under a CERTIFIED error bound; the survivors (~430 per query at config 1)
 // are then re-ranked with the exact fp32 routine of knn_scan_warp, so the final result is identical to the exact scan.
 //
 // Quantisation (tc_quantize, the same for rows and queries; fp32 vector v of dimension D):
@@ -19,10 +19,16 @@
 //   L2      d~ = n_q^2 + n_v^2 - 2p,  lb/ub = d~ -+ (2e + eps (n_q^2 + n_v^2)),  eps = kTcL2Eps + (D + 1) 2^-23 (the exact scan's sum
 //                                                                                  of squares and the rounding of d~ itself)
 // For sigma = 0.25 rows at 768 dims r_v / n_v is about 0.7 %, so e is about 0.015 n_q n_v.
-//   threshold     tau_q = k1-th smallest ub over all DISTINCT rows seen so far by any CTA (one small list per query in HBM,
-//                 updated under a per-query lock -- only O(k log n) successful inserts per query over a whole pass) => a valid
-//                 upper bound of the final k1-th best TRUE distance; a row is a candidate iff lb <= tau_q.  tau starts from an
-//                 exact scan of the first rows (tc_init_tau) and only decreases.
+//   threshold     tau_q = the largest entry of the query's BOUND LIST: k1 EXACT distances (the exact scan's own arithmetic,
+//                 row_dists_warp) of k1 distinct rows (one small list per query in HBM, updated under a per-query lock -- only
+//                 O(k log n) successful inserts per query over a whole pass); a row is a candidate iff lb <= tau_q.  tc_init_tau
+//                 seeds the list with the exact k1 best of the first kTcInitRows rows; a bookkeeper computes the exact distance d of
+//                 a candidate row beyond them whose midpoint d~ is below the threshold and inserts d when it is below it too.
+//                 Every list entry is the exact distance of a distinct row (every tile is visited once per query, seed rows are
+//                 never inserted again), so tau_q is at or above the final k1-th best exact distance at every moment: every row of
+//                 the true top k1 has lb <= d <= tau_q and stays a candidate, and so does every row at or below the k-th distance
+//                 (the tie replay from the lists).  Which rows get rescored only decides how fast tau_q tightens, never whether
+//                 it is valid.  tau only decreases.
 //   range search  tau_q = the query's radius, seeded by the host and never tightened (init_rows = UINT32_MAX: no row reaches the
 //                 bound list, so ub_list, ub_lock and k1 are never read).  A row matches iff its exact distance d < radius, and every
 //                 such row has lb <= d < tau_q, so it is a candidate; the exact re-rank (knn_rerank's range mode) then keeps the
@@ -73,9 +79,14 @@ struct TcArgs {
 								// (1 for IP / L2); zero beyond n
 	const float4* qc;          // [nq_total] (s_q, r_q, n_q, 1 / max(s_q, tiny)) of tc_prepare_queries
 	unsigned int* tau;         // [nq_total] ordered-uint of the current threshold (map space), shared by all CTAs
-	float* ub_list;            // [nq_total][kTcMaxK1] the k1 smallest upper bounds over ALL rows seen by any CTA (guarded by ub_lock)
+	float* ub_list;            // [nq_total][kTcMaxK1] the bound list: the k1 smallest exact distances of the rows inserted by any CTA
+							   // (guarded by ub_lock)
 	unsigned int* ub_lock;     // [nq_total]
 	uint32_t init_rows;        // rows [0, init_rows) are already represented in ub_list by tc_init_tau (never insert them twice)
+	const float* rows;         // fp32 rows [n][pitch] and the Cosine norm coefficients (nullptr otherwise): the bookkeepers' exact
+	const float* norm_coefs;   // distances of the rows they insert into the bound list
+	const float* qf;           // [nq_total][kchunks * 128] fp32 queries, zero padded (tc_prepare_queries)
+	uint32_t pitch;
 	uint32_t* cand_rows;       // [nq_total][cand_cap]
 	unsigned int* cand_count;  // [nq_total]
 	uint32_t cand_cap;
@@ -123,8 +134,11 @@ enum : uint32_t {
 	kTcDgPerWg,
 	kTcDgEmpty = 2 * kTcDgPerWg,
 	kTcDgProd = kTcDgEmpty + 2,
+	kTcDgRescored = kTcDgProd + 2,  // bookkeepers (both warps summed): rows whose exact distance they computed (count), ...
+	kTcDgInserts,                   // ... bound-list inserts attempted under the lock (count), ...
+	kTcDgRescoreCycles,             // ... and clock64 cycles spent computing those distances (stamped instantiation only)
 };
-static_assert(kTcDgProd + 2 <= kTcDiagSlots, "diagnostic counters fit their slots");
+static_assert(kTcDgRescoreCycles < kTcDiagSlots, "diagnostic counters fit their slots");
 
 // shared memory: query block, two stage rings, barriers, per-query constants, then per consumer warpgroup thresholds and (P, R)
 __host__ __device__ inline size_t tc_smem_bytes(uint32_t nq_block, uint32_t kchunks) {
@@ -393,8 +407,8 @@ __device__ __forceinline__ float2 tc_row_bound(const TcArgs& a, float x, float4 
 	return make_float2(-p, e);
 }
 
-// Upper bound ub of a candidate row below the query's threshold: insert it into the query's global bound list (under the per-query
-// lock; other CTAs contend) and tighten the global tau.  Returns the list's largest entry afterwards, the query's new threshold.
+// Exact distance d of a row below the query's threshold: insert it into the query's global bound list (under the per-query lock;
+// other CTAs contend) and tighten the global tau.  Returns the list's largest entry afterwards, the query's new threshold.
 __device__ __noinline__ float tc_bound_insert(const TcArgs& a, uint32_t q, float ub) {
 	while (atomicCAS(&a.ub_lock[q], 0u, 1u) != 0u) {
 	}
@@ -424,15 +438,47 @@ __device__ __noinline__ float tc_bound_insert(const TcArgs& a, uint32_t q, float
 	return tightened;
 }
 
+// The exact distances of the rows flagged in `todo` (one row per lane: row, query ql of the CTA's block), kTcRescoreRows rows in
+// flight per pass of the warp; lane l gets its own row's distance.
+constexpr int kTcRescoreRows = 4;
+template <bool kIsL2>
+__device__ __noinline__ float tc_rescore(const TcArgs& a, unsigned todo, uint32_t row, uint32_t ql, uint32_t q0, int lane) {
+	const uint32_t nch = a.kchunks, pitch4 = a.pitch >> 2;
+	const float4* rows4 = reinterpret_cast<const float4*>(a.rows);
+	float mine = 0.f;
+	while (todo) {
+		uint32_t rr[kTcRescoreRows];
+		const float4* qp[kTcRescoreRows][1];
+		int who[kTcRescoreRows];
+#pragma unroll
+		for (int i = 0; i < kTcRescoreRows; ++i) {
+			who[i] = todo ? __ffs(todo) - 1 : who[0];  // a short last pass repeats its first row
+			todo &= todo - 1u;
+			rr[i] = __shfl_sync(0xffffffffu, row, who[i]);
+			qp[i][0] = reinterpret_cast<const float4*>(a.qf) + size_t(q0 + __shfl_sync(0xffffffffu, ql, who[i])) * nch * 32u;
+		}
+		float d[kTcRescoreRows][1];
+		row_dists_warp<kIsL2, kTcRescoreRows, 1>(rows4, pitch4, nch, rr, qp, a.norm_coefs, lane, d);
+#pragma unroll
+		for (int i = 0; i < kTcRescoreRows; ++i) {
+			mine = lane == who[i] ? d[i][0] : mine;
+		}
+	}
+	return mine;
+}
+
 // Bookkeeper warp of one consumer warpgroup's queue, until every consumer warp is done and the ring is empty.  A row is appended
 // when its own lower bound d~ - err passes the tightest threshold the CTA knows for the query (NaN: appended); the appends of one
-// batch go to the candidate lists with one global atomicAdd per distinct query.  When the row's upper bound beats that threshold it
-// goes into the bound list, and the threshold that comes back is published to the (P, R) of BOTH consumer warpgroups.  A consumer may
-// read a looser threshold meanwhile (a concurrent store of another writer may even replace a tighter one): every threshold ever
-// published is a valid upper bound of the query's final k1-th distance, so the test stays certified.
-template <int kNq>
+// batch go to the candidate lists with one global atomicAdd per distinct query.  When the row's midpoint d~ beats that threshold
+// (and the seed does not hold the row already) the warp computes the row's EXACT distance d with the exact scan's arithmetic; a d
+// below the threshold goes into the bound list, and the threshold that comes back is published to the (P, R) of BOTH consumer
+// warpgroups.  A consumer may read a looser threshold meanwhile (a concurrent store of another writer may even replace a tighter one):
+// every threshold ever published is a valid upper bound of the query's final k1-th distance, so the test stays certified.
+template <int kNq, int kDiag>
 __device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, const uint4* rec, uint32_t slots, uint32_t q0, const float4* s_qc,
-											  float* s_thr, float2* s_pr, float l2eps, int lane) {
+											  float* s_thr, float2* s_pr, float l2eps, int lane, unsigned long long* dg) {
+	[[maybe_unused]] unsigned long long n_rescored = 0, n_inserts = 0;
+	[[maybe_unused]] long long rescore_cycles = 0;
 	uint32_t head = 0;
 	for (;;) {
 		const bool fin = ld_acquire_shared(&qu->done) == 4;  // read before the tail: after it, the tail is final
@@ -482,9 +528,25 @@ __device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, cons
 			if (pos < a.cand_cap) {
 				a.cand_rows[size_t(q0 + ql) * a.cand_cap + pos] = row;
 			}
-			const float ub = d + err;
-			if (ub < tau && row >= a.init_rows) {
-				const float nt = tc_bound_insert(a, q0 + ql, ub);
+		}
+		// the midpoint rather than the upper bound d + err: tau then follows the k1-th best exact distance instead of trailing it by
+		// about err (DESIGN 3.2: 490 against 780 candidates per query at config 1, and the faster step)
+		const bool rescore = append && row >= a.init_rows && d < tau;  // NaN: never
+		const unsigned todo = __ballot_sync(0xffffffffu, rescore);
+		if (todo) {
+			[[maybe_unused]] const long long c0 = kDiag == kTcDiagStamps ? clock64() : 0ll;
+			const float dx = a.metric == kL2 ? tc_rescore<true>(a, todo, row, ql, q0, lane) : tc_rescore<false>(a, todo, row, ql, q0, lane);
+			if constexpr (kDiag != 0) {
+				n_rescored += __popc(todo);
+				if constexpr (kDiag == kTcDiagStamps) {
+					rescore_cycles += clock64() - c0;
+				}
+			}
+			if (rescore && dx < fminf(s_thr[ql], s_thr[kNq + ql])) {  // the threshold may have dropped while the batch was rescored
+				if constexpr (kDiag != 0) {
+					++n_inserts;
+				}
+				const float nt = tc_bound_insert(a, q0 + ql, dx);
 				for (uint32_t w = 0; w < 2; ++w) {
 					if (nt < s_thr[w * kNq + ql]) {
 						s_thr[w * kNq + ql] = nt;
@@ -494,6 +556,14 @@ __device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, cons
 			}
 		}
 		__syncwarp();
+	}
+	if constexpr (kDiag != 0) {
+		const unsigned long long ins = __reduce_add_sync(0xffffffffu, uint32_t(n_inserts));
+		if (lane == 0) {
+			atomicAdd(&dg[kTcDgRescored], n_rescored);
+			atomicAdd(&dg[kTcDgInserts], ins);
+			atomicAdd(&dg[kTcDgRescoreCycles], (unsigned long long)rescore_cycles);
+		}
 	}
 }
 
@@ -637,7 +707,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 	} else if (warp < 4) {
 		// ===== bookkeeper of consumer warpgroup warp - 2 =====
 		const uint32_t wg = uint32_t(warp) - 2;
-		tc_bookkeeper<kNq>(a, s_queue + wg, s_rec + wg * a.queue_slots, a.queue_slots, q0, s_qc, s_thr, s_pr, l2eps, lane);
+		tc_bookkeeper<kNq, kDiag>(a, s_queue + wg, s_rec + wg * a.queue_slots, a.queue_slots, q0, s_qc, s_thr, s_pr, l2eps, lane, dg);
 	} else {
 		// ===== consumer warpgroup wg: the 64-row blocks 2t + wg of the walker's tiles t, through ring wg =====
 		const uint32_t wg = uint32_t(warp) / 4 - 1, wtid = threadIdx.x - 128 * (wg + 1);
@@ -856,7 +926,7 @@ __global__ void __launch_bounds__(kScanThreads) knn_rerank(const float* rows, ui
 	const float bound = tie ? tie_bound[blockIdx.x] : 0.f;
 	const uint32_t nch = (dim + 127u) / 128u, dp4 = nch * 32u, pitch4 = pitch >> 2;
 	const uint32_t m = k1 + kCandBuf;
-	float4* sq4 = reinterpret_cast<float4*>(smem_raw);
+	float4* sq4 = reinterpret_cast<float4*>(smem_raw);  // the query, zero padded to nch * 128 floats (as tc_prepare_queries' qf)
 	uint64_t* skeys = reinterpret_cast<uint64_t*>(smem_raw + size_t(dp4) * 16);  // [8 warps][m]
 	{
 		float* sq = reinterpret_cast<float*>(sq4);
@@ -876,36 +946,7 @@ __global__ void __launch_bounds__(kScanThreads) knn_rerank(const float* rows, ui
 	const uint32_t* my = cand_rows + size_t(q) * cand_cap;
 	for (uint32_t i = warp; i < ncand; i += kScanWarps) {
 		const uint32_t row = my[i];
-		float s = 0.f;
-		for (uint32_t c = 0; c < nch; ++c) {
-			const uint32_t f4 = c * 32u + lane;
-			const float4 db = f4 < pitch4 ? ldg_stream(rows4 + size_t(row) * pitch4 + f4) : make_float4(0.f, 0.f, 0.f, 0.f);
-			const float4 qv = sq4[f4];
-			if constexpr (kIsL2) {
-				float d;
-				d = qv.x - db.x;
-				s = fmaf(d, d, s);
-				d = qv.y - db.y;
-				s = fmaf(d, d, s);
-				d = qv.z - db.z;
-				s = fmaf(d, d, s);
-				d = qv.w - db.w;
-				s = fmaf(d, d, s);
-			} else {
-				s = fmaf(qv.x, db.x, s);
-				s = fmaf(qv.y, db.y, s);
-				s = fmaf(qv.z, db.z, s);
-				s = fmaf(qv.w, db.w, s);
-			}
-		}
-#pragma unroll
-		for (int off = 16; off > 0; off >>= 1) {
-			s += __shfl_xor_sync(0xffffffffu, s, off);
-		}
-		float dist = kIsL2 ? s : -s;
-		if (!kIsL2 && norm_coefs != nullptr) {
-			dist *= norm_coefs[row];
-		}
+		const float dist = row_dist_warp<kIsL2>(rows4, pitch4, nch, row, sq4, norm_coefs, lane);
 		if (range) {
 			if (lane == 0 && dist < rad) {
 				range_keys[size_t(q) * cand_cap + atomicAdd(&range_count[q], 1u)] = make_key(dist, row);
@@ -1208,84 +1249,53 @@ __global__ void tc_convert_rows(const float* rows, uint32_t pitch, uint32_t dim,
 	}
 }
 
-// tau_init[q] = upper bound of the k1-th best distance among the first `nrows` (<= 1024) rows, fp32 dot products.  Any upper bound is
-// valid; a small relative slack covers the difference to the arithmetic order of knn_scan_warp.  One block serves kTcInitQ queries
-// (staged in shared memory, zero padded to the row pitch) so the rows come from L2 once per kTcInitQ queries; a warp keeps four rows
-// (128-bit loads) in flight; the k1 smallest distances of a query are then picked by one warp (k1 rounds of a warp-wide argmin).
+// tau_init[q] = the k1-th best EXACT distance among the first `nrows` (<= kTcInitRows) rows, and ub_list[q] their k1 best: computed
+// with row_dists_warp, the exact scan's own arithmetic, so every list entry is a row's exact-scan distance (knn_tc.cuh header).  One
+// block serves kTcInitQ queries (tc_prepare_queries' zero-padded fp32 copy) so a row comes from L2 once per kTcInitQ queries; a warp
+// keeps four rows (128-bit loads) in flight; the k1 smallest distances of a query are then picked by one warp (k1 rounds of a
+// warp-wide argmin).
 constexpr int kTcInitQ = 4;
-constexpr uint32_t kTcInitRows = 1024;
-__host__ __device__ inline size_t tc_init_smem_bytes(uint32_t pitch) { return size_t(kTcInitQ) * (pitch + kTcInitRows) * sizeof(float); }
-__global__ void __launch_bounds__(256) tc_init_tau(const float* rows, uint32_t pitch, uint32_t dim, const float* norm_coefs, uint32_t nrows,
-												   const float* queries, uint32_t nq, uint32_t k1, int metric, unsigned int* tau, float* ub_list,
+constexpr uint32_t kTcInitRows = 4096;  // DESIGN 3.2: 4096 against 1024 and 2048 at config 1 (fewer early hits and full queues)
+__host__ __device__ inline size_t tc_init_smem_bytes() { return size_t(kTcInitQ) * kTcInitRows * sizeof(float); }
+__global__ void __launch_bounds__(256) tc_init_tau(const float* rows, uint32_t pitch, uint32_t kchunks, const float* norm_coefs, uint32_t nrows,
+												   const float* qf, uint32_t nq, uint32_t k1, int metric, unsigned int* tau, float* ub_list,
 												   unsigned int* ub_lock) {
-	extern __shared__ __align__(16) float s_init[];
-	float* s_q = s_init;                     // [kTcInitQ][pitch]
-	float* s_d = s_init + kTcInitQ * pitch;  // [kTcInitQ][kTcInitRows]
+	extern __shared__ __align__(16) float s_d[];  // [kTcInitQ][kTcInitRows]
 	const uint32_t q0 = blockIdx.x * kTcInitQ;
 	const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-	for (uint32_t i = threadIdx.x; i < kTcInitQ * pitch; i += blockDim.x) {
-		const uint32_t qi = i / pitch, c = i % pitch;
-		s_q[i] = (q0 + qi < nq && c < dim) ? queries[size_t(q0 + qi) * dim + c] : 0.f;
+	const float4* rows4 = reinterpret_cast<const float4*>(rows);
+	const float4* q4[kTcInitQ];
+#pragma unroll
+	for (int qi = 0; qi < kTcInitQ; ++qi) {  // padding queries of the last block read query q0 (their distances are never picked)
+		q4[qi] = reinterpret_cast<const float4*>(qf) + size_t(q0 + qi < nq ? q0 + qi : q0) * kchunks * 32u;
 	}
-	__syncthreads();
-	const uint32_t pitch4 = pitch / 4;
 	constexpr uint32_t kRows = 4;  // rows in flight per warp
 	for (uint32_t r0 = warp * kRows; r0 < kTcInitRows; r0 += 8 * kRows) {
-		float acc[kRows][kTcInitQ];
-#pragma unroll
-		for (uint32_t x = 0; x < kRows; ++x) {
-#pragma unroll
-			for (int qi = 0; qi < kTcInitQ; ++qi) {
-				acc[x][qi] = 0.f;
-			}
-		}
+		float dist[kRows][kTcInitQ];
 		if (r0 < nrows) {
-			const float4* p4[kRows];
+			uint32_t rr[kRows];
+			const float4* qp[kRows][kTcInitQ];
 #pragma unroll
 			for (uint32_t x = 0; x < kRows; ++x) {
-				p4[x] = reinterpret_cast<const float4*>(rows + size_t(min(r0 + x, nrows - 1)) * pitch);
-			}
-#pragma unroll 3
-			for (uint32_t c = lane; c < pitch4; c += 32) {
-				float4 v[kRows];
-#pragma unroll
-				for (uint32_t x = 0; x < kRows; ++x) {
-					v[x] = __ldg(p4[x] + c);
-				}
+				rr[x] = min(r0 + x, nrows - 1);
 #pragma unroll
 				for (int qi = 0; qi < kTcInitQ; ++qi) {
-					const float4 qq = reinterpret_cast<const float4*>(s_q + qi * pitch)[c];
-#pragma unroll
-					for (uint32_t x = 0; x < kRows; ++x) {
-						if (metric == kL2) {
-							const float a0 = qq.x - v[x].x, a1 = qq.y - v[x].y, a2 = qq.z - v[x].z, a3 = qq.w - v[x].w;
-							acc[x][qi] = fmaf(a0, a0, fmaf(a1, a1, fmaf(a2, a2, fmaf(a3, a3, acc[x][qi]))));
-						} else {
-							acc[x][qi] = fmaf(qq.x, v[x].x, fmaf(qq.y, v[x].y, fmaf(qq.z, v[x].z, fmaf(qq.w, v[x].w, acc[x][qi]))));
-						}
-					}
+					qp[x][qi] = q4[qi];
 				}
+			}
+			if (metric == kL2) {
+				row_dists_warp<true, kRows, kTcInitQ>(rows4, pitch / 4, kchunks, rr, qp, nullptr, lane, dist);
+			} else {
+				row_dists_warp<false, kRows, kTcInitQ>(rows4, pitch / 4, kchunks, rr, qp, norm_coefs, lane, dist);
 			}
 		}
 #pragma unroll
 		for (uint32_t x = 0; x < kRows; ++x) {
 #pragma unroll
 			for (int qi = 0; qi < kTcInitQ; ++qi) {
-				float s = acc[x][qi];
-				for (int off = 16; off > 0; off >>= 1) {
-					s += __shfl_xor_sync(0xffffffffu, s, off);
-				}
 				if (lane == uint32_t(qi)) {
 					const uint32_t r = r0 + x;
-					float d = INFINITY;
-					if (r < nrows) {
-						d = metric == kL2 ? s : -s;
-						if (metric == kCos) {
-							d *= norm_coefs[r];
-						}
-						d += 1e-4f * fabsf(d) + 1e-6f;
-					}
-					s_d[qi * kTcInitRows + r] = d;
+					s_d[qi * kTcInitRows + r] = r < nrows ? dist[x][qi] : INFINITY;
 				}
 			}
 		}
@@ -1331,13 +1341,17 @@ __global__ void __launch_bounds__(256) tc_init_tau(const float* rows, uint32_t p
 	}
 }
 
-// queries fp32 [nq][dim] -> int8 codes [nq_pad][pitch] (zero padded) + (s_q, r_q, n_q, 1 / k_q), k_q = s_q (1 when s_q = 0)
+// queries fp32 [nq][dim] -> int8 codes [nq_pad][pitch] (zero padded) + (s_q, r_q, n_q, 1 / k_q), k_q = s_q (1 when s_q = 0), and the
+// fp32 queries zero padded to the same pitch, qf [nq_pad][pitch] (the exact distances of tc_init_tau and the filter's bookkeepers)
 __global__ void tc_prepare_queries(const float* queries, uint32_t nq, uint32_t nq_pad, uint32_t dim, uint32_t pitch, unsigned char* codes,
-								   float4* qc) {
+								   float4* qc, float* qf) {
 	const uint32_t q = (blockIdx.x * blockDim.x + threadIdx.x) / 32;
 	const int lane = threadIdx.x & 31;
 	if (q >= nq_pad) {
 		return;
+	}
+	for (uint32_t c = lane; c < pitch; c += 32) {
+		qf[size_t(q) * pitch + c] = q < nq && c < dim ? queries[size_t(q) * dim + c] : 0.f;
 	}
 	unsigned char* out = codes + size_t(q) * pitch;
 	const float3 srn = tc_quantize(queries + size_t(q) * dim, q < nq ? dim : 0u, pitch, lane,
