@@ -340,6 +340,13 @@ int rxgpu_hnsw_search_knn_sq8(const rxgpu_index*, uint32_t nq, const float* quer
 int rxgpu_ivf_import(rxgpu_index*, uint32_t nlist, const float* centroids /* nlist x dim, host */, const uint64_t* list_sizes /* nlist */);
 int rxgpu_ivf_search_knn(const rxgpu_index*, uint32_t nq, const float* queries /* host */, uint32_t k, uint32_t nprobe, float* out_dist,
 						 uint64_t* out_label, uint32_t* out_count);
+/* The same search at any k in [1, 65535] and any nprobe (clamped to [1, nlist]): the best min(k, probed rows) rows per query, cut at
+ * the k-th place by (distance, internal row) and then ordered by (distance, label), as rxgpu_ivf_search_knn orders them.  k <= 256 with
+ * nprobe <= 1024 runs rxgpu_ivf_search_knn itself (same bits); otherwise one distance pass writes every probed row's key to a device
+ * workspace and an exact radix select keeps the k best per query (DESIGN.md §3.5).  Same errors as rxgpu_ivf_search_knn; k = 0 or
+ * k > 65535: RXGPU_ERR_PARAMS; device memory exhausted: RXGPU_ERR_SYSTEM.  Entries past out_count[q] are not written. */
+int rxgpu_ivf_search_knn_large_k(const rxgpu_index*, uint32_t nq, const float* queries /* host */, uint32_t k, uint32_t nprobe,
+								 float* out_dist, uint64_t* out_label, uint32_t* out_count);
 /* map_->range_search(1, key, radius, &result, &params) (ivf_index.cc:205-300): every row of the nprobe probed lists with
  * dist < radius in map space (strict; IP / Cosine radius negated by the caller), best first; *out_n = total number of matches. */
 int rxgpu_ivf_search_range(const rxgpu_index*, const float* query /* host */, float radius, uint32_t nprobe, uint64_t max_out,

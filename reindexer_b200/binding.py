@@ -168,6 +168,7 @@ _SIGNATURES = {
     "rxgpu_hnsw_search_knn_sq8": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, _f32p, C.c_uint32, C.c_uint32, _f32p, _u64p, _u32p, _u32p]),
     "rxgpu_ivf_import": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, _u64p]),
     "rxgpu_ivf_search_knn": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, C.c_uint32, C.c_uint32, _f32p, _u64p, _u32p]),
+    "rxgpu_ivf_search_knn_large_k": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, C.c_uint32, C.c_uint32, _f32p, _u64p, _u32p]),
     "rxgpu_ivf_search_range": (C.c_int, [C.c_void_p, _f32p, C.c_float, C.c_uint32, C.c_uint64, _f32p, _u64p, C.POINTER(C.c_uint64)]),
     "rxgpu_ft_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_uint32, C.c_uint32, _u32p, _f32p, _u8p, C.c_int]),
     "rxgpu_ft_destroy": (None, [C.c_void_p]),
@@ -548,6 +549,16 @@ class GpuBruteforceSearch:
         l = np.zeros((nq, max(k, 1)), np.uint64)
         c = np.zeros(nq, np.uint32)
         _check(self._lib.rxgpu_ivf_search_knn(self._h, nq, _p(q, _f32p), k, nprobe, _p(d, _f32p), _p(l, _u64p), _p(c, _u32p)))
+        return d, l, c
+
+    def ivf_search_knn_large_k(self, queries, k: int, nprobe: int):
+        """ivf_search_knn at any k in [1, 65535] and any nprobe (rxgpu_ivf_search_knn_large_k)"""
+        q = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, self.dim)
+        nq = q.shape[0]
+        d = np.zeros((nq, max(k, 1)), np.float32)
+        l = np.zeros((nq, max(k, 1)), np.uint64)
+        c = np.zeros(nq, np.uint32)
+        _check(self._lib.rxgpu_ivf_search_knn_large_k(self._h, nq, _p(q, _f32p), k, nprobe, _p(d, _f32p), _p(l, _u64p), _p(c, _u32p)))
         return d, l, c
 
     def ivf_search_range(self, query, radius: float, nprobe: int, max_out: int | None = None):

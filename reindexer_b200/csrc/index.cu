@@ -4,6 +4,9 @@
 // There is no CPU fallback anywhere in this file: without a usable CUDA device every compute entry point fails.
 #include <cuda_runtime.h>
 
+#include <cub/device/device_scan.cuh>
+#include <cub/device/device_segmented_radix_sort.cuh>
+
 #include <algorithm>
 #include <atomic>
 #include <cstdio>
@@ -22,6 +25,7 @@
 #include "../host/knn_select.h"
 #include "knn_scan.cuh"
 #include "knn_tc.cuh"
+#include "ivf_select.cuh"
 
 using namespace rxgpu;
 
@@ -49,19 +53,19 @@ int allocDevice(rxgpu_index* ix, uint64_t capacity, float** rows, uint64_t** lab
 }
 
 // ---------------------------------------------------------------------------------------------------------------- launches
-template <int QT, int RW, int CG>
+template <int QT, int RW, int CG, bool kKeysOut>
 cudaError_t launchScanT(const rxgpu_index* ix, const ScanArgs& a, unsigned grid, size_t smem, cudaStream_t st) {
 	if (smem > size_t(kScanSmemBudget)) {
 		return cudaErrorInvalidValue;
 	}
 	if (ix->metric == RXGPU_L2) {
-		auto kfn = knn_scan_warp<QT, RW, CG, true>;
+		auto kfn = knn_scan_warp<QT, RW, CG, true, kKeysOut>;
 		if (const cudaError_t e = raiseSmemCeilingOnce(kfn, ix->device, kScanSmemBudget); e != cudaSuccess) {
 			return e;
 		}
 		kfn<<<grid, kScanThreads, smem, st>>>(a);
 	} else {
-		auto kfn = knn_scan_warp<QT, RW, CG, false>;
+		auto kfn = knn_scan_warp<QT, RW, CG, false, kKeysOut>;
 		if (const cudaError_t e = raiseSmemCeilingOnce(kfn, ix->device, kScanSmemBudget); e != cudaSuccess) {
 			return e;
 		}
@@ -70,7 +74,8 @@ cudaError_t launchScanT(const rxgpu_index* ix, const ScanArgs& a, unsigned grid,
 	return cudaGetLastError();
 }
 
-template <int QT>
+// kKeysOut: the key mode of the work-item scan (every scanned row's key to ScanArgs::lists), QT = 1 only
+template <int QT, bool kKeysOut = false>
 cudaError_t launchScanQ(const rxgpu_index* ix, const ScanArgs& a, uint32_t nch, unsigned* gridOut, cudaStream_t st, bool dryRun) {
 	// chunk group CG divides nch; RW*CG float4 loads in flight per lane
 	int cg, rw;
@@ -98,15 +103,15 @@ cudaError_t launchScanQ(const rxgpu_index* ix, const ScanArgs& a, uint32_t nch, 
 	const size_t smem = scan_smem_bytes(QT, a.dim, a.k1);
 	switch (cg) {
 		case 6:
-			return launchScanT<QT, 2, 6>(ix, a, grid, smem, st);
+			return launchScanT<QT, 2, 6, kKeysOut>(ix, a, grid, smem, st);
 		case 4:
-			return launchScanT<QT, 2, 4>(ix, a, grid, smem, st);
+			return launchScanT<QT, 2, 4, kKeysOut>(ix, a, grid, smem, st);
 		case 3:
-			return launchScanT<QT, 4, 3>(ix, a, grid, smem, st);
+			return launchScanT<QT, 4, 3, kKeysOut>(ix, a, grid, smem, st);
 		case 2:
-			return launchScanT<QT, 4, 2>(ix, a, grid, smem, st);
+			return launchScanT<QT, 4, 2, kKeysOut>(ix, a, grid, smem, st);
 		default:
-			return launchScanT<QT, 8, 1>(ix, a, grid, smem, st);
+			return launchScanT<QT, 8, 1, kKeysOut>(ix, a, grid, smem, st);
 	}
 }
 
@@ -1877,6 +1882,15 @@ struct rxgpu_ivf_device {
 	DevBuf<uint32_t> d_idx, d_count;
 	DevBuf<uint64_t> d_range;
 	DevBuf<unsigned long long> d_range_count;
+	// any-k select path (rxgpu_ivf_search_knn_large_k): probed rows and key offsets per query, a query chunk's work items (query-major,
+	// with the slot of their first key) and key workspace, the survivors (ordered distance word + label, double-buffered for the sorts)
+	DevBuf<uint64_t> d_qrows, d_qoff, d_keys;
+	DevBuf<uint4> d_work_chunk;
+	DevBuf<uint32_t> d_sel_ord, d_sel_ord2, d_sel_count, d_sel_hist;
+	DevBuf<uint64_t> d_sel_label, d_sel_label2;
+	DevBuf<int> d_seg_begin, d_seg_end;
+	DevBuf<SelState> d_sel_state;
+	DevBuf<unsigned char> d_cub;
 	// mutable lists (rxgpu_ivf_create / _add / _remove): every list owns a region [begin, begin + cap) of a row slab; size <= cap
 	bool own = false;
 	float* rows = nullptr;       // [slab_rows][pitch]
@@ -1900,6 +1914,32 @@ struct rxgpu_ivf_device {
 namespace rxgpu {
 void ivfRelease(rxgpu_ivf_device* p) { delete p; }
 }  // namespace rxgpu
+
+namespace {
+size_t ivfCoarseSmem(const rxgpu_index* ix, const rxgpu_ivf_device* h) { return size_t((ix->dim + 127u) / 128u) * 512 + size_t(h->nlist) * 8; }
+int ivfCheckCoarseSmem(const rxgpu_index* ix, const rxgpu_ivf_device* h) {
+	if (ivfCoarseSmem(ix, h) > 200 * 1024) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: dimension / centroid count exceeds the coarse quantiser's shared memory");
+	}
+	return 0;
+}
+// the coarse quantiser over the nq queries in h->d_q: work items of the list scans in h->d_work, probe-major
+int ivfLaunchCoarse(const rxgpu_index* ix, rxgpu_ivf_device* h, uint32_t nq, uint32_t nprobe, cudaStream_t st) {
+	const size_t coarseSmem = ivfCoarseSmem(ix, h);
+	if (ix->metric == RXGPU_L2) {
+		RX_CUDA(raiseSmemCeilingOnce(ivf_coarse_kernel<true>, ix->device, 200 * 1024));
+		ivf_coarse_kernel<true><<<nq, kScanThreads, coarseSmem, st>>>(h->centroids.p, ix->pitch, ix->dim, h->nlist, h->d_q.p, nq, nprobe,
+																	   h->list_begin.p, h->own ? h->list_end.p : nullptr, nullptr, h->d_work.p);
+	} else {
+		RX_CUDA(raiseSmemCeilingOnce(ivf_coarse_kernel<false>, ix->device, 200 * 1024));
+		ivf_coarse_kernel<false><<<nq, kScanThreads, coarseSmem, st>>>(h->centroids.p, ix->pitch, ix->dim, h->nlist, h->d_q.p, nq, nprobe,
+																		h->list_begin.p, h->own ? h->list_end.p : nullptr,
+																		ix->metric == RXGPU_COS ? h->cnorm.p : nullptr, h->d_work.p);
+	}
+	RX_CUDA(cudaGetLastError());
+	return 0;
+}
+}  // namespace
 
 extern "C" {
 
@@ -1979,10 +2019,8 @@ int rxgpu_ivf_search_knn(const rxgpu_index* ix, uint32_t nq, const float* querie
 	if (nprobe > 256u * kMergeOwn) {
 		return fail(RXGPU_ERR_PARAMS, "rxgpu: nprobe exceeds the merge fan-in (1024)");
 	}
-	const uint32_t nch = (ix->dim + 127u) / 128u;
-	const size_t coarseSmem = size_t(nch) * 512 + size_t(h->nlist) * 8;
-	if (coarseSmem > 200 * 1024) {
-		return fail(RXGPU_ERR_PARAMS, "rxgpu: dimension / centroid count exceeds the coarse quantiser's shared memory");
+	if (int rc = ivfCheckCoarseSmem(ix, h)) {
+		return rc;
 	}
 	std::lock_guard<std::mutex> lck(h->mtx);
 	cudaStream_t st = ix->stream;
@@ -1995,16 +2033,9 @@ int rxgpu_ivf_search_knn(const rxgpu_index* ix, uint32_t nq, const float* querie
 	RX_CUDA(h->d_label.ensure(size_t(nq) * k));
 	RX_CUDA(h->d_count.ensure(nq));
 	RX_CUDA(cudaMemcpyAsync(h->d_q.p, queries, size_t(nq) * ix->dim * 4, cudaMemcpyHostToDevice, st));
-	if (ix->metric == RXGPU_L2) {
-		RX_CUDA(raiseSmemCeilingOnce(ivf_coarse_kernel<true>, ix->device, 200 * 1024));
-		ivf_coarse_kernel<true><<<nq, kScanThreads, coarseSmem, st>>>(h->centroids.p, ix->pitch, ix->dim, h->nlist, h->d_q.p, nq, nprobe,
-																	   h->list_begin.p, h->own ? h->list_end.p : nullptr, nullptr, h->d_work.p);
-	} else {
-		RX_CUDA(raiseSmemCeilingOnce(ivf_coarse_kernel<false>, ix->device, 200 * 1024));
-		ivf_coarse_kernel<false><<<nq, kScanThreads, coarseSmem, st>>>(h->centroids.p, ix->pitch, ix->dim, h->nlist, h->d_q.p, nq, nprobe,
-																		h->list_begin.p, h->own ? h->list_end.p : nullptr, ix->metric == RXGPU_COS ? h->cnorm.p : nullptr, h->d_work.p);
+	if (int rc = ivfLaunchCoarse(ix, h, nq, nprobe, st)) {
+		return rc;
 	}
-	RX_CUDA(cudaGetLastError());
 	// list scans: the exact scan kernel in work-item mode, one CTA per (query, probed list), fused top-k per CTA
 	ScanArgs a{};
 	a.rows = h->own ? h->rows : ix->d_rows;
@@ -2069,6 +2100,171 @@ int rxgpu_ivf_search_knn(const rxgpu_index* ix, uint32_t nq, const float* querie
 	return 0;
 }
 
+int rxgpu_ivf_search_knn_large_k(const rxgpu_index* ix, uint32_t nq, const float* queries, uint32_t k, uint32_t nprobe, float* out_dist,
+								 uint64_t* out_label, uint32_t* out_count) {
+	if (int rc = checkIndex(ix)) {
+		return rc;
+	}
+	g_stats = rxgpu_search_stats{};
+	if (nq == 0) {
+		return 0;
+	}
+	if (!queries || !out_count || (k && (!out_dist || !out_label))) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: null argument");
+	}
+	rxgpu_ivf_device* h = ix->ivf;
+	if (!h) {
+		return fail(RXGPU_ERR_LOGIC, "rxgpu: no IVF lists imported into this index");
+	}
+	if (h->index_version != ix->version) {
+		return fail(RXGPU_ERR_LOGIC, "rxgpu: the index changed after the IVF lists were imported");
+	}
+	if (k == 0 || k > kMaxLargeK) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: IVF search needs k in [1, 65535]");
+	}
+	nprobe = std::max(1u, std::min(nprobe, h->nlist));
+	if (k <= kMaxFusedK1 && nprobe <= 256u * kMergeOwn) {  // what the fused per-list top-k serves: that path, same bits
+		return rxgpu_ivf_search_knn(ix, nq, queries, k, nprobe, out_dist, out_label, out_count);
+	}
+	if (int rc = ivfCheckCoarseSmem(ix, h)) {
+		return rc;
+	}
+	std::lock_guard<std::mutex> lck(h->mtx);
+	cudaStream_t st = ix->stream;
+	const size_t nwork = size_t(nq) * nprobe;
+	RX_CUDA(h->d_q.ensure(size_t(nq) * ix->dim));
+	RX_CUDA(h->d_work.ensure(nwork));
+	RX_CUDA(h->d_qrows.ensure(nq));
+	RX_CUDA(h->d_qoff.ensure(nq));
+	RX_CUDA(cudaMemcpyAsync(h->d_q.p, queries, size_t(nq) * ix->dim * 4, cudaMemcpyHostToDevice, st));
+	if (int rc = ivfLaunchCoarse(ix, h, nq, nprobe, st)) {
+		return rc;
+	}
+	// probed rows per query and their exclusive scan: each query's first key
+	ivf_probe_rows_kernel<<<(nq + 7u) / 8u, 256, 0, st>>>(h->d_work.p, nq, nprobe, h->d_qrows.p);
+	RX_CUDA(cudaGetLastError());
+	size_t cubBytes = 0;
+	RX_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, cubBytes, h->d_qrows.p, h->d_qoff.p, int(nq), st));
+	RX_CUDA(h->d_cub.ensure(cubBytes));
+	RX_CUDA(cub::DeviceScan::ExclusiveSum(h->d_cub.p, cubBytes, h->d_qrows.p, h->d_qoff.p, int(nq), st));
+	uint32_t launches = 3;  // coarse quantiser, probed rows, their scan (one CUB call)
+	try {
+		std::vector<uint64_t> rows(nq), off(size_t(nq) + 1, 0);
+		RX_CUDA(cudaMemcpyAsync(rows.data(), h->d_qrows.p, size_t(nq) * 8, cudaMemcpyDeviceToHost, st));
+		RX_CUDA(cudaStreamSynchronize(st));
+		for (uint32_t q = 0; q < nq; ++q) {
+			off[q + 1] = off[q] + rows[q];
+		}
+		const uint64_t* labels = h->own ? h->labels : ix->d_labels;
+		const uint32_t nch = (ix->dim + 127u) / 128u;
+		std::vector<uint32_t> ord, cnt;
+		std::vector<uint64_t> lab;
+		// query chunks: at most kIvfKeyCap keys and kIvfSlotCap survivor slots each; a query above the key cap is a chunk of its own
+		for (uint32_t q0 = 0, q1 = 0; q0 < nq; q0 = q1) {
+			q1 = q0 + 1;
+			while (q1 < nq && off[q1 + 1] - off[q0] <= kIvfKeyCap && uint64_t(q1 + 1 - q0) * k <= kIvfSlotCap) {
+				++q1;
+			}
+			const uint32_t cq = q1 - q0;
+			const uint64_t nkeys = off[q1] - off[q0];
+			const size_t slots = size_t(cq) * k;
+			RX_CUDA(h->d_keys.ensure(std::max<uint64_t>(nkeys, 1)));
+			RX_CUDA(h->d_work_chunk.ensure(size_t(cq) * nprobe));
+			RX_CUDA(h->d_sel_ord.ensure(slots));
+			RX_CUDA(h->d_sel_ord2.ensure(slots));
+			RX_CUDA(h->d_sel_label.ensure(slots));
+			RX_CUDA(h->d_sel_label2.ensure(slots));
+			RX_CUDA(h->d_sel_count.ensure(cq));
+			RX_CUDA(h->d_seg_begin.ensure(cq));
+			RX_CUDA(h->d_seg_end.ensure(cq));
+			RX_CUDA(cudaMemsetAsync(h->d_sel_count.p, 0, size_t(cq) * 4, st));
+			if (nkeys) {
+				// key pass: the exact scan in work-item key mode, one CTA per (query, probed list)
+				ivf_key_plan_kernel<<<(cq + 7u) / 8u, 256, 0, st>>>(h->d_work.p, nq, nprobe, q0, cq, h->d_qoff.p, h->d_work_chunk.p);
+				RX_CUDA(cudaGetLastError());
+				ScanArgs a{};
+				a.rows = h->own ? h->rows : ix->d_rows;
+				a.norm_coefs = ix->metric != RXGPU_COS ? nullptr : h->own ? h->norms : ix->d_norms;
+				a.queries = h->d_q.p;
+				a.pitch = ix->pitch;
+				a.dim = ix->dim;
+				a.nq = 1;
+				a.k1 = 1;
+				a.mode = kModeTopK;
+				a.work = h->d_work_chunk.p;
+				a.nwork = cq * nprobe;
+				a.lists = h->d_keys.p;
+				unsigned grid = 0;
+				RX_CUDA((launchScanQ<1, true>(ix, a, nch, &grid, st, false)));
+				ivf_select_cta_kernel<<<cq, kIvfSelThreads, 0, st>>>(h->d_keys.p, h->d_qoff.p + q0, h->d_qrows.p + q0, off[q0], k, labels,
+																  h->d_sel_ord.p, h->d_sel_label.p, h->d_sel_count.p);
+				RX_CUDA(cudaGetLastError());
+				launches += 3;
+				for (uint32_t qi = 0; qi < cq; ++qi) {  // queries with many keys: the same select over many CTAs
+					const uint64_t n = rows[q0 + qi];
+					if (n <= kIvfSelCtaKeys) {
+						continue;
+					}
+					RX_CUDA(h->d_sel_state.ensure(1));
+					RX_CUDA(h->d_sel_hist.ensure(kIvfSelBins));
+					const SelState init{0ull, kKeyNone, k, 0u};
+					RX_CUDA(cudaMemcpyAsync(h->d_sel_state.p, &init, sizeof(init), cudaMemcpyHostToDevice, st));
+					RX_CUDA(cudaMemsetAsync(h->d_sel_hist.p, 0, kIvfSelBins * 4, st));
+					const uint64_t* kq = h->d_keys.p + (off[q0 + qi] - off[q0]);
+					const unsigned g = unsigned(std::min<uint64_t>((n + 16 * kIvfSelThreads - 1) / (16 * kIvfSelThreads), uint64_t(ix->sm_count) * 2));
+					for (int pass = 0; pass < kIvfSelPasses; ++pass) {
+						ivf_select_hist_kernel<<<g, kIvfSelThreads, 0, st>>>(kq, n, h->d_sel_state.p, pass, h->d_sel_hist.p);
+						ivf_select_pick_kernel<<<1, kIvfSelThreads, 0, st>>>(h->d_sel_state.p, pass, h->d_sel_hist.p);
+					}
+					ivf_select_compact_kernel<<<g, kIvfSelThreads, 0, st>>>(kq, n, h->d_sel_state.p, labels, h->d_sel_ord.p + size_t(qi) * k,
+																		 h->d_sel_label.p + size_t(qi) * k, h->d_sel_count.p + qi);
+					RX_CUDA(cudaGetLastError());
+					launches += 2 * kIvfSelPasses + 1;
+				}
+				// order the survivors by (distance, label): stable radix sorts by label, then by the ordered distance word
+				ivf_sort_bounds_kernel<<<(cq + 255u) / 256u, 256, 0, st>>>(h->d_sel_count.p, k, cq, h->d_seg_begin.p, h->d_seg_end.p);
+				RX_CUDA(cudaGetLastError());
+				size_t sortBytes = 0, sortBytes2 = 0;
+				RX_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, sortBytes, h->d_sel_label.p, h->d_sel_label2.p, h->d_sel_ord.p,
+																 h->d_sel_ord2.p, int(slots), int(cq), h->d_seg_begin.p, h->d_seg_end.p, 0, 64, st));
+				RX_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, sortBytes2, h->d_sel_ord2.p, h->d_sel_ord.p, h->d_sel_label2.p,
+																 h->d_sel_label.p, int(slots), int(cq), h->d_seg_begin.p, h->d_seg_end.p, 0, 32, st));
+				RX_CUDA(h->d_cub.ensure(std::max(sortBytes, sortBytes2)));
+				RX_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(h->d_cub.p, sortBytes, h->d_sel_label.p, h->d_sel_label2.p, h->d_sel_ord.p,
+																 h->d_sel_ord2.p, int(slots), int(cq), h->d_seg_begin.p, h->d_seg_end.p, 0, 64, st));
+				RX_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(h->d_cub.p, sortBytes2, h->d_sel_ord2.p, h->d_sel_ord.p, h->d_sel_label2.p,
+																 h->d_sel_label.p, int(slots), int(cq), h->d_seg_begin.p, h->d_seg_end.p, 0, 32, st));
+				launches += 3;
+			}
+			ord.resize(slots);
+			lab.resize(slots);
+			cnt.resize(cq);
+			RX_CUDA(cudaMemcpyAsync(cnt.data(), h->d_sel_count.p, size_t(cq) * 4, cudaMemcpyDeviceToHost, st));
+			if (nkeys) {
+				RX_CUDA(cudaMemcpyAsync(ord.data(), h->d_sel_ord.p, slots * 4, cudaMemcpyDeviceToHost, st));
+				RX_CUDA(cudaMemcpyAsync(lab.data(), h->d_sel_label.p, slots * 8, cudaMemcpyDeviceToHost, st));
+			}
+			RX_CUDA(cudaStreamSynchronize(st));
+			for (uint32_t qi = 0; qi < cq; ++qi) {
+				const size_t at = size_t(q0 + qi) * k, from = size_t(qi) * k;
+				for (uint32_t j = 0; j < cnt[qi]; ++j) {
+					out_dist[at + j] = key_dist(ord[from + j], false);  // as the fused path decodes it: a zero distance is +0
+					out_label[at + j] = lab[from + j];
+				}
+				out_count[q0 + qi] = cnt[qi];
+			}
+		}
+		const uint64_t probed = off[nq];
+		g_stats.launches = launches;
+		g_stats.passes = 1;
+		// rows read once; each key written once and read once by the select
+		g_stats.algorithmic_bytes = probed * ix->dim * 4 + (ix->metric == RXGPU_COS ? probed * 4 : 0) + probed * 16;
+	} catch (const std::bad_alloc&) {
+		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
+	}
+	return 0;
+}
+
 int rxgpu_ivf_search_range(const rxgpu_index* ix, const float* query, float radius, uint32_t nprobe, uint64_t max_out, float* out_dist,
 						   uint64_t* out_label, uint64_t* out_n) {
 	if (int rc = checkIndex(ix)) {
@@ -2087,10 +2283,8 @@ int rxgpu_ivf_search_range(const rxgpu_index* ix, const float* query, float radi
 		return fail(RXGPU_ERR_LOGIC, "rxgpu: the index changed after the IVF lists were imported");
 	}
 	nprobe = std::max(1u, std::min(nprobe, h->nlist));
-	const uint32_t nch = (ix->dim + 127u) / 128u;
-	const size_t coarseSmem = size_t(nch) * 512 + size_t(h->nlist) * 8;
-	if (coarseSmem > 200 * 1024) {
-		return fail(RXGPU_ERR_PARAMS, "rxgpu: dimension / centroid count exceeds the coarse quantiser's shared memory");
+	if (int rc = ivfCheckCoarseSmem(ix, h)) {
+		return rc;
 	}
 	std::lock_guard<std::mutex> lck(h->mtx);
 	cudaStream_t st = ix->stream;
@@ -2098,17 +2292,9 @@ int rxgpu_ivf_search_range(const rxgpu_index* ix, const float* query, float radi
 	RX_CUDA(h->d_work.ensure(nprobe));
 	RX_CUDA(h->d_range_count.ensure(1));
 	RX_CUDA(cudaMemcpyAsync(h->d_q.p, query, size_t(ix->dim) * 4, cudaMemcpyHostToDevice, st));
-	if (ix->metric == RXGPU_L2) {
-		RX_CUDA(raiseSmemCeilingOnce(ivf_coarse_kernel<true>, ix->device, 200 * 1024));
-		ivf_coarse_kernel<true><<<1, kScanThreads, coarseSmem, st>>>(h->centroids.p, ix->pitch, ix->dim, h->nlist, h->d_q.p, 1, nprobe,
-																	  h->list_begin.p, h->own ? h->list_end.p : nullptr, nullptr, h->d_work.p);
-	} else {
-		RX_CUDA(raiseSmemCeilingOnce(ivf_coarse_kernel<false>, ix->device, 200 * 1024));
-		ivf_coarse_kernel<false><<<1, kScanThreads, coarseSmem, st>>>(h->centroids.p, ix->pitch, ix->dim, h->nlist, h->d_q.p, 1, nprobe,
-																	   h->list_begin.p, h->own ? h->list_end.p : nullptr,
-																	   ix->metric == RXGPU_COS ? h->cnorm.p : nullptr, h->d_work.p);
+	if (int rc = ivfLaunchCoarse(ix, h, 1, nprobe, st)) {
+		return rc;
 	}
-	RX_CUDA(cudaGetLastError());
 	g_stats.launches = 1;
 	uint64_t cap = std::max<uint64_t>(h->d_range.n, 1u << 14);
 	unsigned long long total = 0;

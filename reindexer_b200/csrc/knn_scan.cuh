@@ -47,6 +47,8 @@ struct ScanArgs {
 	const uint64_t* floor_keys;  // [nq] only keys ABOVE the floor compete (rounds of a k > 255 search), or nullptr
 	// work-item mode (IVF list scans, QT = 1): CTA b scans rows [work[b].y, work[b].z) for query work[b].x with its own 8 warps and
 	// writes list b; row_begin / row_end / nq are ignored (nq = 1)
+	// key mode (knn_scan_warp<..., kKeysOut = true>, work-item mode only): no top-k; the key make_key(dist, row) of every scanned row goes
+	// to lists[work[b].w + (row - work[b].y)] -- one fixed slot per (work item, row), no atomics
 	const uint4* work;
 	uint32_t nwork;
 };
@@ -94,13 +96,14 @@ __device__ __forceinline__ void warp_select(uint64_t* arr, uint32_t total, uint3
 	}
 }
 
-template <int QT, int RW, int CG, bool kIsL2>
+template <int QT, int RW, int CG, bool kIsL2, bool kKeysOut = false>
 __global__ void __launch_bounds__(kScanThreads, 2) knn_scan_warp(const ScanArgs a) {
 	static_assert(RW * QT <= 32, "one lane per (row, query) result");
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const float* qsrc = a.queries;
 	uint32_t row_begin = a.row_begin, row_end = a.row_end;
 	uint32_t gfirst = blockIdx.x * kScanWarps + (threadIdx.x >> 5), gstride = gridDim.x * kScanWarps;
+	uint32_t key_base = 0;  // key mode: slot of the work item's first row
 	if (a.work != nullptr) {
 		const uint4 w = a.work[blockIdx.x];
 		qsrc += size_t(w.x) * a.dim;
@@ -108,6 +111,9 @@ __global__ void __launch_bounds__(kScanThreads, 2) knn_scan_warp(const ScanArgs 
 		row_end = w.z;
 		gfirst = threadIdx.x >> 5;
 		gstride = kScanWarps;
+		if constexpr (kKeysOut) {
+			key_base = w.w;
+		}
 	}
 	const int lane = threadIdx.x & 31;
 	const int warp = threadIdx.x >> 5;
@@ -233,6 +239,12 @@ __global__ void __launch_bounds__(kScanThreads, 2) knn_scan_warp(const ScanArgs 
 		if (!kIsL2 && a.norm_coefs != nullptr && valid) {
 			dist *= a.norm_coefs[row];  // Cosine: hnswlib.h:160-161
 		}
+		if constexpr (kKeysOut) {
+			if (valid) {
+				a.lists[size_t(key_base) + (row - row_begin)] = make_key(dist, row);
+			}
+			continue;
+		}
 		if (a.mode == kModeRange) {
 			const bool hit = valid && dist < a.bound;  // strict, bruteforce.cc:137
 			const unsigned hm = __ballot_sync(0xffffffffu, hit);
@@ -288,49 +300,51 @@ __global__ void __launch_bounds__(kScanThreads, 2) knn_scan_warp(const ScanArgs 
 	if (a.mode == kModeRange) {
 		return;
 	}
-	// flush the candidate buffers
+	if constexpr (!kKeysOut) {  // key mode wrote every key in the loop: no lists
+		// flush the candidate buffers
 #pragma unroll
-	for (int qi = 0; qi < QT; ++qi) {
-		const uint32_t c = wcnt[qi];
-		if (c) {
-			warp_select(wkeys + qi * m, a.k1 + c, a.k1, lane);
-		}
-	}
-	__syncthreads();
-	// CTA merge: warp w merges query w, w+8, ... over the 8 warp lists into warp 0's list region, then writes it out
-	for (int qi = warp; qi < QT; qi += kScanWarps) {
-		if (uint32_t(qi) >= a.nq) {
-			continue;
-		}
-		// gather the 8 x k1 best keys behind warp 0's list of this query (its buffer region is free now) -- may not fit:
-		// do a k1-round selection over the strided sources instead.
-		uint64_t* out = a.lists + (size_t(blockIdx.x) * QT + qi) * a.k1;
-		uint64_t last = 0;  // keys are unique except kKeyNone: select strictly increasing keys
-		bool first = true;
-		for (uint32_t r = 0; r < a.k1; ++r) {
-			uint64_t best = kKeyNone;
-			for (uint32_t i = lane; i < kScanWarps * a.k1; i += 32) {
-				const uint32_t w = i / a.k1, j = i - w * a.k1;
-				const uint64_t kx = skeys[(size_t(w) * QT + qi) * m + j];
-				if ((first || kx > last) && kx < best) {
-					best = kx;
-				}
+		for (int qi = 0; qi < QT; ++qi) {
+			const uint32_t c = wcnt[qi];
+			if (c) {
+				warp_select(wkeys + qi * m, a.k1 + c, a.k1, lane);
 			}
+		}
+		__syncthreads();
+		// CTA merge: warp w merges query w, w+8, ... over the 8 warp lists into warp 0's list region, then writes it out
+		for (int qi = warp; qi < QT; qi += kScanWarps) {
+			if (uint32_t(qi) >= a.nq) {
+				continue;
+			}
+			// gather the 8 x k1 best keys behind warp 0's list of this query (its buffer region is free now) -- may not fit:
+			// do a k1-round selection over the strided sources instead.
+			uint64_t* out = a.lists + (size_t(blockIdx.x) * QT + qi) * a.k1;
+			uint64_t last = 0;  // keys are unique except kKeyNone: select strictly increasing keys
+			bool first = true;
+			for (uint32_t r = 0; r < a.k1; ++r) {
+				uint64_t best = kKeyNone;
+				for (uint32_t i = lane; i < kScanWarps * a.k1; i += 32) {
+					const uint32_t w = i / a.k1, j = i - w * a.k1;
+					const uint64_t kx = skeys[(size_t(w) * QT + qi) * m + j];
+					if ((first || kx > last) && kx < best) {
+						best = kx;
+					}
+				}
 #pragma unroll
-			for (int off = 16; off > 0; off >>= 1) {
-				const uint64_t ok = __shfl_xor_sync(0xffffffffu, best, off);
-				best = ok < best ? ok : best;
-			}
-			if (lane == 0) {
-				out[r] = best;
-			}
-			last = best;
-			first = false;
-			if (best == kKeyNone) {
-				for (uint32_t rr = r + 1 + lane; rr < a.k1; rr += 32) {
-					out[rr] = kKeyNone;
+				for (int off = 16; off > 0; off >>= 1) {
+					const uint64_t ok = __shfl_xor_sync(0xffffffffu, best, off);
+					best = ok < best ? ok : best;
 				}
-				break;
+				if (lane == 0) {
+					out[r] = best;
+				}
+				last = best;
+				first = false;
+				if (best == kKeyNone) {
+					for (uint32_t rr = r + 1 + lane; rr < a.k1; rr += 32) {
+						out[rr] = kKeyNone;
+					}
+					break;
+				}
 			}
 		}
 	}

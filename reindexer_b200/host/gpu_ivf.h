@@ -4,7 +4,7 @@
 // clone, RebuildCentroids read its inverted lists and direct map through operator->), the four calls on the query/update path --
 //   search(1, key, k, dists, ids, &IVFSearchParameters{nprobe})      range_search(1, key, radius, &result, &params)
 //   add_with_ids(1, vec[, norm], &id)                                 remove_ids(IDSelectorArray{1, &id})
-// -- are served by librxgpu (include/rxgpu.h: rxgpu_ivf_create / _add / _remove / _search_knn / _search_range).  The device lists are
+// -- are served by librxgpu (include/rxgpu.h: rxgpu_ivf_create / _add / _remove / _search_knn_large_k / _search_range).  The device lists are
 // filled once, from the trained index, by the first search; after that every upsert / delete patches them in place (the list number
 // is read back from FAISS' direct map, so both sides agree on the assignment bit for bit).  Distances follow FAISS' conventions
 // (L2: squared distance ascending; inner product / cosine: +similarity descending, labels -1 past the end).
@@ -99,7 +99,8 @@ public:
 		const uint32_t nprobe = nprobeOf(params);
 		std::vector<uint64_t> lab(size_t(n) * k);
 		std::vector<uint32_t> cnt(n);
-		check(rxgpu_ivf_search_knn(gpu_, uint32_t(n), x, uint32_t(k), nprobe, distances, lab.data(), cnt.data()));
+		// any k (IvfIndex asks for large k when other conditions filter the KNN result): k <= 256 at nprobe <= 1024 takes the fused path
+		check(rxgpu_ivf_search_knn_large_k(gpu_, uint32_t(n), x, uint32_t(k), nprobe, distances, lab.data(), cnt.data()));
 		const bool similarity = cpu_->metric_type != faiss::METRIC_L2;
 		for (faiss::idx_t q = 0; q < n; ++q) {
 			for (faiss::idx_t j = 0; j < k; ++j) {
