@@ -6,14 +6,16 @@
 Runs the batch through the diagnostic instantiations of knn_tc_filter (knn_tc.cuh: kTcDiag*, selected with rxgpu_tc_diag; the
 searches themselves never take them) and prints one JSON line with
   * phases      per consumer warpgroup, the share of its clock64 cycles in each phase of a 64-row block (wait on `full`, the rest of
-                the K loop, the wgmma_wait<0> drain, the two bar.syncs, the block test, the rare path split into the append and the
-                bound-list update, the candidate queue's wait when it is full), the cycles per block, and the producers' share of time
-                waiting on `empty`;
+                the K loop, the wgmma_wait<0> drain, the two bar.syncs, the block test (the loop that builds the hit mask), the append
+                (the vote and the enqueues of the hits, their waits on a full candidate queue included), the wait for the
+                warpgroup's turn to issue its MMAs),
+                the cycles per block, the enqueues that found the queue full, and the producers' share of time waiting on `empty`;
   * hits        (query, row) pairs that passed the block test per 64-row block, against the walk position (the walker's i-th tile);
   * drift       how far apart the CTAs of one walker are: the spread of the walk positions they have reached at fixed times;
-  * launches    the filter launch time (CUDA events, median of --runs) of the production kernel, of the stamped kernel, and of the two
-                ablations: (a) the rare path compiled out (block test kept, hits only counted) and (b) the producers not fetching
-                (the consumers multiply zeroed stages; the barriers still cycle).
+  * launches    the filter launch time (CUDA events, median of --runs) of the production kernel, of the stamped kernel, and of the three
+                ablations: (a) the rare path compiled out (block test kept, hits only counted), (b) the producers not fetching
+                (the consumers multiply zeroed stages; the barriers still cycle) and (c) the block test and the rare path compiled
+                out (rings, MMAs, drain and bar.syncs kept): the MMA path's own floor.
 Clock stamps are cycles of the SM clock; the card, its power limit and the SM clock samples of the timed runs are in the line.
 """
 import argparse
@@ -34,10 +36,10 @@ from bench_range import card  # noqa: E402
 
 # knn_tc.cuh: the diagnostic counters
 SLOTS, WALK, MARK_EVERY = 32, 8192, 64
-PHASES = ["full_wait", "k_loop", "drain", "bar1", "block_test", "append", "bound_list", "bar2"]
+PHASES = ["full_wait", "k_loop", "drain", "bar1", "block_test", "append", "turn_wait", "bar2"]
 TILE, BLOCKS, HITS, QWAIT, PER_WG = 8, 9, 10, 11, 12
 EMPTY, PROD = 2 * PER_WG, 2 * PER_WG + 2
-MODES = {"production": 0, "stamped": 1, "no_rare_path": 2, "no_fetch": 3}
+MODES = {"production": 0, "stamped": 1, "no_rare_path": 2, "no_fetch": 3, "mma_only": 4}
 MAX_CTAS = 1024
 
 
@@ -150,6 +152,7 @@ def main(argv=None):
         "launches": launches,
         "ablation_ceiling_no_rare_path_speedup": prod_ms / launches["no_rare_path"]["median_ms"],
         "ablation_floor_no_fetch_speedup": prod_ms / launches["no_fetch"]["median_ms"],
+        "ablation_floor_mma_only_speedup": prod_ms / launches["mma_only"]["median_ms"],
         "int8_ops_per_clk_per_sm": (ops / (prod_ms * 1e-3) / (sm_mhz * 1e6) / grid) if sm_mhz else None,
         "candidates_per_batch": prod_stats["tc_candidates"], "fallbacks": prod_stats["tc_fallbacks"],
         "phases": phases, "hits_by_walk_position": hits, "drift": drift, "clocks": clocks,

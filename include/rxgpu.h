@@ -530,7 +530,7 @@ typedef struct {
 	                               (rxgpu_hnsw_search_range_batch: whose result region overflowed and were answered again) */
 	uint64_t tc_candidates;     /* rows re-ranked exactly */
 	uint32_t tc_cluster;        /* CTAs per cluster in the filter kernel (row tiles are TMA-multicast inside a cluster) */
-	uint32_t tc_kernel;         /* 1 = knn_tc_filter (wgmma, queries in shared memory); 2..4 = its diagnostic instantiations (rxgpu_tc_diag) */
+	uint32_t tc_kernel;         /* 1 = knn_tc_filter (wgmma, queries in shared memory); 2..5 = its diagnostic instantiations (rxgpu_tc_diag) */
 } rxgpu_search_stats;
 void rxgpu_last_search_stats(rxgpu_search_stats* out);
 /* large query batches: int8 tensor-core filter (exact integer dot products of per-row scaled codes, certified by per-row
@@ -541,8 +541,9 @@ int rxgpu_set_tensor_core_filter(rxgpu_index*, int mode);
 /* process-wide switch: bracket every scan-kernel launch with CUDA events (used by bench.py for the roofline figure) */
 int rxgpu_set_profile(int on);
 /* process-wide, diagnostics only (bench_tc_phases.py): every tensor-core filter launch takes the diagnostic instantiation `mode`
- * (1 = per-phase clock stamps, 2 = rare path compiled out, 3 = producers not fetching; 0 = the production kernel again) and adds its
- * counters to the zeroed device buffer d_counters (knn_tc.cuh: kTcDiag*).  Modes 2 and 3 return meaningless results; only query
+ * (1 = per-phase clock stamps, 2 = rare path compiled out, 3 = producers not fetching, 4 = block test and rare path compiled out;
+ * 0 = the production kernel again) and adds its counters to the zeroed device buffer d_counters (knn_tc.cuh: kTcDiag*).  Modes 2
+ * to 4 return meaningless results; only query
  * blocks of 128 and single CTAs are served.  A mode other than 0 is refused (RXGPU_ERR_LOGIC) unless the environment has
  * RXGPU_TC_DIAG=1, and a search a diagnostic instantiation answered reports tc_kernel = 1 + mode in its statistics. */
 int rxgpu_tc_diag(int mode, void* d_counters);

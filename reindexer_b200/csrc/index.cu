@@ -278,8 +278,8 @@ TcKernel tcKernel(uint32_t nqb, uint32_t cluster) {
 std::atomic<int> g_tc_diag{0};
 unsigned long long* g_tc_diag_buf = nullptr;
 TcKernel tcDiagKernel(int mode) {
-	static const TcKernel table[3] = {knn_tc_filter<128, 1, kTcDiagStamps>, knn_tc_filter<128, 1, kTcDiagNoRare>,
-									  knn_tc_filter<128, 1, kTcDiagNoFetch>};
+	static const TcKernel table[4] = {knn_tc_filter<128, 1, kTcDiagStamps>, knn_tc_filter<128, 1, kTcDiagNoRare>,
+									  knn_tc_filter<128, 1, kTcDiagNoFetch>, knn_tc_filter<128, 1, kTcDiagNoTest>};
 	return table[mode - 1];
 }
 
@@ -1222,8 +1222,8 @@ int rxgpu_set_tensor_core_filter(rxgpu_index* ix, int mode) {
 	return 0;
 }
 int rxgpu_tc_diag(int mode, void* d_counters) {
-	if (mode < 0 || mode > kTcDiagNoFetch || (mode && !d_counters)) {
-		return fail(RXGPU_ERR_PARAMS, "rxgpu: diagnostic filter mode must be 0..3, with a counter buffer");
+	if (mode < 0 || mode > kTcDiagNoTest || (mode && !d_counters)) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: diagnostic filter mode must be 0..4, with a counter buffer");
 	}
 	const char* env = std::getenv("RXGPU_TC_DIAG");
 	if (mode && !(env && std::strcmp(env, "1") == 0)) {  // a stray call must not turn every search of the process into a diagnostic

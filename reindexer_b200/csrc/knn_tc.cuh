@@ -53,7 +53,8 @@
 //   warpgroups 1, 2   consumers: warpgroup w multiplies its 64-row blocks with the whole query block (wgmma.m64nNQk32.s32.s8.s8,
 //                both operands from shared memory, exact int32 accumulators in registers), releases each stage as soon as its MMAs
 //                retired, then tests its 64 x NQ scores against tau and hands every hit to its bookkeeper through a queue in shared
-//                memory.  The two rings are independent, so one warpgroup's epilogue overlaps the other's MMAs.
+//                memory.  The two warpgroups take turns issuing a block's MMAs (ping-pong), so one warpgroup's epilogue overlaps
+//                the other's MMAs.
 #pragma once
 #include <cuda.h>
 
@@ -103,13 +104,15 @@ struct TcArgs {
 };
 
 // Diagnostic instantiations of knn_tc_filter (template flag kDiag, 0 in every search; bench_tc_phases.py selects one through
-// rxgpu_tc_diag).  kTcDiagStamps stamps every phase of every tile with clock64(); the two ablations bound what the epilogue and the
-// row stream cost: kTcDiagNoRare compiles the rare path out (the block test stays, hits are only counted, tau never tightens), and
-// kTcDiagNoFetch lets the producers cycle the barriers without fetching (the consumers multiply zeroed stages).  Their candidate
-// lists are meaningless; only the time and the counters are read.
+// rxgpu_tc_diag).  kTcDiagStamps stamps every phase of every tile with clock64(); the three ablations bound what the epilogue and the
+// row stream cost: kTcDiagNoRare compiles the rare path out (the block test stays, hits are only counted, tau never tightens),
+// kTcDiagNoFetch lets the producers cycle the barriers without fetching (the consumers multiply zeroed stages), and kTcDiagNoTest
+// compiles the block test and the rare path out (rings, MMAs, drain and both bar.syncs stay; the accumulators only feed an XOR sink
+// so the MMAs are kept).  Their candidate lists are meaningless; only the time and the counters are read.
 constexpr int kTcDiagStamps = 1;
 constexpr int kTcDiagNoRare = 2;
 constexpr int kTcDiagNoFetch = 3;
+constexpr int kTcDiagNoTest = 4;
 // a.diag layout: [gridDim.x][kTcDiagSlots] per-CTA counters, then [kTcDiagWalk] hits per walk position (position i = the walker's
 // i-th tile, summed over all CTAs), then [gridDim.x][kTcDiagWalk / kTcDiagMarkEvery] %globaltimer marks taken when a CTA starts the
 // walk positions 0, kTcDiagMarkEvery, 2 kTcDiagMarkEvery, ...
@@ -120,12 +123,13 @@ constexpr uint32_t kTcDiagMarkEvery = 64;
 // blocks, hits and queue waits are counts), producer ring r at kTcDgEmpty + r (cycles waiting on `empty`) and kTcDgProd + r (total)
 enum : uint32_t {
 	kTcDgFull,     // waiting on full[stage]
-	kTcDgMma,      // the rest of the K loop: tau refresh, row constants, MMA issue, wgmma_wait<1> and stage release
+	kTcDgMma,      // the rest of the K loop: tau refresh, row constants, MMA issue, wgmma_wait<1>, stage release, handing the turn over
 	kTcDgDrain,    // wgmma_wait<0> and the last release
 	kTcDgBar1,     // the first bar.sync
-	kTcDgTest,     // the block test (the scan without its rare path)
-	kTcDgAppend,   // the rare path: the enqueues of the hits (their waits on a full queue included)
-	kTcDgBound,    // unused since the bookkeepers took the bound list off the consumers (the rare path's lock section before)
+	kTcDgTest,     // the block test: the branch-free loop that builds the hit mask
+	kTcDgAppend,   // the vote on the hit masks and the enqueues of the hits (their waits on a full queue included)
+	kTcDgTurn,     // waiting for the warpgroup's turn to issue its MMAs (kTcDiagNoTest: the XOR of its accumulators instead, the sink
+				   // that keeps its MMAs)
 	kTcDgBar2,     // the second bar.sync
 	kTcDgTile,     // the whole tile
 	kTcDgBlocks,   // 64-row blocks walked (count, per warp)
@@ -383,7 +387,7 @@ __device__ __forceinline__ bool tc_enqueue(TcQueue* qu, uint4* rec, uint32_t slo
 }
 
 // the hits of one accumulator quad (h = bits 0..3 for (row0, q), (row0, q + 1), (row1, q), (row1, q + 1)), out of line: inlined at
-// each of the kNq / 8 quads of the unrolled block test it only spreads the test's hot loop over more instruction cache
+// each of the kNq / 8 quads of the unrolled append loop it only spreads the consumer loop over more instruction cache
 __device__ __noinline__ bool tc_enqueue_quad(TcQueue* qu, uint4* rec, uint32_t slots, uint32_t h, uint32_t q, uint32_t row0, uint32_t row1,
 											 float x0, float x1, float x2, float x3) {
 	bool waited = false;
@@ -738,9 +742,10 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		uint32_t stage = 0, phase = 0;
 		[[maybe_unused]] long long dt[kTcDgPerWg] = {};  // kStamp: this warp's cycles per phase (kTcDg*)
 		[[maybe_unused]] unsigned long long nhits = 0;
+		[[maybe_unused]] uint32_t sink = 0;  // kTcDiagNoTest
 		for (uint32_t t = walker; t < ntiles; t += walkers) {
 			[[maybe_unused]] const uint32_t walk = (t - walker) / walkers;
-			[[maybe_unused]] long long s0 = clk(), s1, s2, s3, s4, rare = 0;
+			[[maybe_unused]] long long s0 = clk(), s1, s2, s3, s4, s5;
 			if constexpr (kStamp) {
 				if (wg == 0 && wtid == 0 && walk % kTcDiagMarkEvery == 0 && walk < kTcDiagWalk) {
 					unsigned long long now;
@@ -764,6 +769,20 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 #pragma unroll
 			for (int i = 0; i < kNq / 2; ++i) {
 				acc[i] = 0;
+			}
+			// Warpgroup turns (ping-pong): the two consumer warpgroups take turns issuing a block's MMAs, so one's block test runs
+			// under the other's MMAs instead of both testing at once while the tensor pipe idles.  Warpgroup w waits on named barrier
+			// 3 + w, which the other warpgroup arrives on once it has issued its block's last chunk.  No deadlock: both warpgroups walk
+			// the same tiles (block 2t + wg of every tile t), so their turns alternate 0, 1, 0, 1, ...; warpgroup 0 takes the first turn
+			// without waiting, and warpgroup 1 does not hand over after its last block, so no arrival is left pending at exit.  The
+			// producers and the bookkeepers never wait on a turn.  In a cluster of two each CTA orders its own warpgroups in the same
+			// order, and a stage shared with the peer only waits on the peer's same warpgroup at an earlier point of that order.
+			[[maybe_unused]] const long long c_turn = clk();
+			if (wg == 1 || t != walker) {
+				asm volatile("bar.sync %0, 256;" ::"r"(3 + wg) : "memory");
+			}
+			if constexpr (kStamp) {
+				dt[kTcDgTurn] += clk() - c_turn;
 			}
 			uint32_t prev = 0;
 			for (uint32_t kc = 0; kc < a.kchunks; ++kc) {
@@ -792,6 +811,10 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 					phase ^= 1;
 				}
 			}
+			// hand the turn over once the last chunk is issued, before it retires (warpgroup 1: unless this was its last block)
+			if (wg == 0 || t + walkers < ntiles) {
+				asm volatile("bar.arrive %0, 256;" ::"r"(3 + (wg ^ 1)) : "memory");
+			}
 			s1 = clk();
 			wgmma_wait<0>();
 			if (lane == 0) {
@@ -804,8 +827,14 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 			const float S0 = rc0.x * rc0.w, S1 = rc1.x * rc1.w;
 			const float M0 = rc0.w * fmaf(ka, rc0.y, kb * rc0.z), M1 = rc1.w * fmaf(ka, rc1.y, kb * rc1.z);
 			const float W0 = l2 ? 0.5f * (1.f - l2eps) * rc0.z * rc0.z : 0.f, W1 = l2 ? 0.5f * (1.f - l2eps) * rc1.z * rc1.z : 0.f;
-			const bool ok0 = row0 < a.n, ok1 = row1 < a.n;
-			auto scan = [&](auto kL2Tag) {
+			// The block test: the predicate of every accumulator into the hit mask, bit i for acc[i] (quad j: bits 4j + {0, 1, 2, 3} =
+			// (row0, q), (row0, q + 1), (row1, q), (row1, q + 1)).  No call and no branch in the loop, so the quads' (P, R) loads and
+			// arithmetic overlap; the rows beyond n are masked out of every quad at once after it, and the hits, about one per block,
+			// are appended after that.
+			const uint32_t ok = (row0 < a.n ? 0x33333333u : 0u) | (row1 < a.n ? 0xCCCCCCCCu : 0u);
+			constexpr int kMaskWords = (kNq / 2 + 31) / 32;
+			uint32_t hm[kMaskWords] = {};
+			auto test = [&](auto kL2Tag) {
 				constexpr bool kL2 = decltype(kL2Tag)::value;
 #pragma unroll
 				for (int j = 0; j < kNq / 8; ++j) {
@@ -820,20 +849,47 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 						Rd = fmaf(-zb, W1, Rd);
 					}
 					const float x0 = float(acc[4 * j]), x1 = float(acc[4 * j + 1]), x2 = float(acc[4 * j + 2]), x3 = float(acc[4 * j + 3]);
-					const bool h0 = ok0 && !(fmaf(x0, S0, fmaf(p2.x, M0, Ra)) < 0.f);
-					const bool h1 = ok0 && !(fmaf(x1, S0, fmaf(p2.z, M0, Rb)) < 0.f);
-					const bool h2 = ok1 && !(fmaf(x2, S1, fmaf(p2.x, M1, Rc)) < 0.f);
-					const bool h3 = ok1 && !(fmaf(x3, S1, fmaf(p2.z, M1, Rd)) < 0.f);
-					if (h0 | h1 | h2 | h3) {  // rare path: hand the hits to the bookkeeper
-						if constexpr (kDiag != 0) {
-							nhits += uint32_t(h0) + uint32_t(h1) + uint32_t(h2) + uint32_t(h3);
-						}
-						if constexpr (kDiag != kTcDiagNoRare) {
-							[[maybe_unused]] const long long r = clk();
-							const bool waited = tc_enqueue_quad(qu, rec, slots, uint32_t(h0) | uint32_t(h1) << 1 | uint32_t(h2) << 2 | uint32_t(h3) << 3,
-																q, row0, row1, x0, x1, x2, x3);
+					const bool h0 = !(fmaf(x0, S0, fmaf(p2.x, M0, Ra)) < 0.f);
+					const bool h1 = !(fmaf(x1, S0, fmaf(p2.z, M0, Rb)) < 0.f);
+					const bool h2 = !(fmaf(x2, S1, fmaf(p2.x, M1, Rc)) < 0.f);
+					const bool h3 = !(fmaf(x3, S1, fmaf(p2.z, M1, Rd)) < 0.f);
+					hm[4 * j / 32] |= (uint32_t(h0) | uint32_t(h1) << 1 | uint32_t(h2) << 2 | uint32_t(h3) << 3) << (4 * j % 32);
+				}
+			};
+			if constexpr (kDiag == kTcDiagNoTest) {
+#pragma unroll
+				for (int i = 0; i < kNq / 2; ++i) {
+					sink ^= uint32_t(acc[i]);
+				}
+			} else if (l2) {
+				test(std::true_type{});
+			} else {
+				test(std::false_type{});
+			}
+#pragma unroll
+			for (int w = 0; w < kMaskWords; ++w) {
+				hm[w] &= ok;
+			}
+			s4 = clk();
+			// the append (rare path): one vote per warp, then the lanes with hits hand them to the bookkeeper quad by quad, x = float(I)
+			// taken again from the accumulator
+			[[maybe_unused]] uint32_t nh = 0;
+#pragma unroll
+			for (int w = 0; w < kMaskWords; ++w) {
+				nh += __popc(hm[w]);
+			}
+			if constexpr (kDiag != 0) {
+				nhits += nh;
+			}
+			if constexpr (kDiag != kTcDiagNoRare && kDiag != kTcDiagNoTest) {
+				if (__any_sync(0xffffffffu, nh != 0)) {
+#pragma unroll
+					for (int j = 0; j < kNq / 8; ++j) {
+						const uint32_t h = hm[4 * j / 32] >> (4 * j % 32) & 15u;
+						if (h) {
+							const bool waited = tc_enqueue_quad(qu, rec, slots, h, 8 * j + c2, row0, row1, float(acc[4 * j]), float(acc[4 * j + 1]),
+																float(acc[4 * j + 2]), float(acc[4 * j + 3]));
 							if constexpr (kStamp) {
-								rare += clk() - r;
 								if (waited) {
 									atomicAdd(&qu->full_waits, 1u);
 								}
@@ -841,29 +897,21 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 						}
 					}
 				}
-			};
-			[[maybe_unused]] const unsigned long long hits_before = nhits;
-			if (l2) {
-				scan(std::true_type{});
-			} else {
-				scan(std::false_type{});
 			}
 			__syncwarp();  // the rare path diverges (per-lane queue waits): reconverge before the .aligned wgmma of the next tile
-			s4 = clk();
+			s5 = clk();
 			asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // nobody still reads (P, R) when the next refresh writes them
 			if constexpr (kStamp) {
-				// the warp's rare path time: its slowest lane (the lanes of a diverged warp run one after another)
-				const long long rare_w = __reduce_max_sync(0xffffffffu, uint32_t(rare));
-				const long long s5 = clk();
+				const long long s6 = clk();
 				dt[kTcDgMma] += s1 - s0;
 				dt[kTcDgDrain] += s2 - s1;
 				dt[kTcDgBar1] += s3 - s2;
-				dt[kTcDgTest] += (s4 - s3) - rare_w;
-				dt[kTcDgAppend] += rare_w;
-				dt[kTcDgBar2] += s5 - s4;
-				dt[kTcDgTile] += s5 - s0;
+				dt[kTcDgTest] += s4 - s3;
+				dt[kTcDgAppend] += s5 - s4;
+				dt[kTcDgBar2] += s6 - s5;
+				dt[kTcDgTile] += s6 - s0;
 				dt[kTcDgBlocks] += 1;
-				const uint32_t h = __reduce_add_sync(0xffffffffu, uint32_t(nhits - hits_before));
+				const uint32_t h = __reduce_add_sync(0xffffffffu, nh);
 				if (lane == 0 && h && walk < kTcDiagWalk) {
 					atomicAdd(&a.diag[size_t(gridDim.x) * kTcDiagSlots + walk], (unsigned long long)h);
 				}
@@ -876,10 +924,14 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		}
 		if constexpr (kDiag != 0) {
 			const uint32_t h = __reduce_add_sync(0xffffffffu, uint32_t(nhits));
+			const uint32_t x = __reduce_xor_sync(0xffffffffu, sink);
 			if (lane == 0) {
 				atomicAdd(&dg[wg * kTcDgPerWg + kTcDgHits], (unsigned long long)h);
+				if constexpr (kDiag == kTcDiagNoTest) {
+					atomicXor(&dg[wg * kTcDgPerWg + kTcDgTurn], (unsigned long long)x);
+				}
 				if constexpr (kStamp) {
-					dt[kTcDgMma] -= dt[kTcDgFull];  // the K loop's waits are counted on their own
+					dt[kTcDgMma] -= dt[kTcDgFull] + dt[kTcDgTurn];  // the K loop's waits are counted on their own
 					for (uint32_t i = 0; i < kTcDgPerWg; ++i) {
 						if (i != kTcDgHits) {
 							atomicAdd(&dg[wg * kTcDgPerWg + i], (unsigned long long)dt[i]);
