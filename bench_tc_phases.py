@@ -9,13 +9,13 @@ searches themselves never take them) and prints one JSON line with
                 the K loop, the wgmma_wait<0> drain, the two bar.syncs, the block test (the loop that builds the hit mask), the append
                 (the vote and the enqueues of the hits, their waits on a full candidate queue included), the wait for the
                 warpgroup's turn to issue its MMAs),
-                the cycles per block, the enqueues that found the queue full, and the producers' share of time waiting on `empty`;
+                the cycles per block, the enqueues that found the queue full, and the producer's share of time waiting on `empty`;
   * hits        (query, row) pairs that passed the block test per 64-row block, against the walk position (the walker's i-th tile);
   * drift       how far apart the CTAs of one walker are: the spread of the walk positions they have reached at fixed times;
   * launches    the filter launch time (CUDA events, median of --runs) of the production kernel, of the stamped kernel, and of the three
-                ablations: (a) the rare path compiled out (block test kept, hits only counted), (b) the producers not fetching
+                ablations: (a) the rare path compiled out (block test kept, hits only counted), (b) the producer not fetching
                 (the consumers multiply zeroed stages; the barriers still cycle) and (c) the block test and the rare path compiled
-                out (rings, MMAs, drain and bar.syncs kept): the MMA path's own floor.
+                out (ring, MMAs, turns, drain and bar.syncs kept): the MMA path's own floor.
 Clock stamps are cycles of the SM clock; the card, its power limit and the SM clock samples of the timed runs are in the line.
 """
 import argparse
@@ -35,10 +35,11 @@ from bench import DIM, K, ROWS_FULL, SEED, ClockSampler, bench_queries  # noqa: 
 from bench_range import card  # noqa: E402
 
 # knn_tc.cuh: the diagnostic counters
-SLOTS, WALK, MARK_EVERY = 32, 8192, 64
+SLOTS, WALK, MARK_EVERY = 64, 8192, 64
 PHASES = ["full_wait", "k_loop", "drain", "bar1", "block_test", "append", "turn_wait", "bar2"]
 TILE, BLOCKS, HITS, QWAIT, PER_WG = 8, 9, 10, 11, 12
-EMPTY, PROD = 2 * PER_WG, 2 * PER_WG + 2
+CONSUMERS = 3  # consumer warpgroups, each followed by PER_WG counters; then the producer's
+EMPTY, PROD = CONSUMERS * PER_WG, CONSUMERS * PER_WG + 1
 MODES = {"production": 0, "stamped": 1, "no_rare_path": 2, "no_fetch": 3, "mma_only": 4}
 MAX_CTAS = 1024
 
@@ -107,7 +108,7 @@ def main(argv=None):
     grid = groups * walkers
     cta = c[:grid * SLOTS].reshape(grid, SLOTS)
     phases = {}
-    for wg in range(2):
+    for wg in range(CONSUMERS):
         v = cta[:, wg * PER_WG:(wg + 1) * PER_WG].sum(axis=0)
         tile, blocks = v[TILE], v[BLOCKS]  # cycles and blocks summed over the warpgroup's four warps
         phases[f"warpgroup{wg}"] = {
@@ -116,8 +117,7 @@ def main(argv=None):
             "cycles_per_block_by_phase": {p: v[i] / blocks for i, p in enumerate(PHASES)},
             "blocks": blocks / 4, "hits": v[HITS], "hits_per_block": v[HITS] / (blocks / 4), "queue_full_waits": v[QWAIT],
         }
-    prod_total = cta[:, PROD:PROD + 2].sum(axis=0)
-    phases["producers_empty_wait_share"] = [cta[:, EMPTY + r].sum() / prod_total[r] for r in range(2)]
+    phases["producer_empty_wait_share"] = cta[:, EMPTY].sum() / cta[:, PROD].sum()
 
     hist = c[grid * SLOTS:grid * SLOTS + WALK]
     walk_len = min(WALK, ntiles // walkers)  # positions every CTA reaches

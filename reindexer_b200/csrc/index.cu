@@ -360,7 +360,7 @@ int ensureShadow(const rxgpu_index* ix, cudaStream_t st) {
 
 // One batch of queries on the candidate filter: the int8 query codes and their tensor map, prepared once, and the launch shape.
 struct TcBatch {
-	uint32_t nq, nqb, cluster, ngroups, nqPad, kchunks, queueSlots;
+	uint32_t nq, nqb, cluster, ngroups, nqPad, kchunks, stages, queueSlots;
 	int diag;     // the diagnostic instantiation taken (rxgpu_tc_diag), 0 = the production kernel
 	size_t smem;  // tc_smem_bytes + the candidate queues
 	int resident;
@@ -397,9 +397,10 @@ int tcPrepare(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float
 		return rc;
 	}
 	b.kfn = tcKernel(nqb, cluster);
-	b.queueSlots = tc_queue_slots(nqb, kchunks, kTcSmemLimit);
-	b.smem = tc_smem_bytes(nqb, kchunks) + tc_queue_bytes(b.queueSlots);
-	if (b.queueSlots == 0) {
+	b.stages = tc_ring_stages(nqb, kchunks, kTcSmemLimit);
+	b.queueSlots = tc_queue_slots(nqb, kchunks, b.stages, kTcSmemLimit);
+	b.smem = tc_smem_bytes(nqb, kchunks, b.stages) + tc_queue_bytes(b.queueSlots);
+	if (b.stages == 0 || b.queueSlots == 0) {
 		return fail(RXGPU_ERR_SYSTEM, "rxgpu: no room for the tensor-core filter's candidate queues");
 	}
 	b.diag = g_tc_diag.load();
@@ -481,6 +482,7 @@ int tcLaunch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const TcBatc
 	a.k1 = k1;
 	a.metric = ix->metric;
 	a.queue_slots = b.queueSlots;
+	a.stages = b.stages;
 	a.diag = g_tc_diag_buf;
 	// One launch serves G = min(groups left, resident) query groups with W = resident / G tile walkers each, so the G clusters of a
 	// walker read every row tile from HBM about once and from L2 otherwise (config 1: 8 blocks x 16 walkers = 128 CTAs, the shadow

@@ -40,21 +40,24 @@
 // the 128-row tiles w, w + W, w + 2W, ..., so every tile is visited once per query, and the G CTAs of one walker request the same
 // tiles at about the same time: the first read misses to HBM, the others hit L2, and nothing makes one CTA wait for another.
 //
-// Roles (384 threads = three warpgroups, 1 CTA per SM, persistent over 128-row tiles):
-//   warps 0, 1   producers: warp 0 loads the query block (NQ x dim int8 codes) once by TMA; warp w then streams the 64-row shadow
-//                blocks 2t + w of the walker's tiles t, one K chunk (64 rows x 128 codes = 8 KB) per stage, through the RING OF
-//                consumer warpgroup w (kTcStages stages each).  The shadow is stored TILED and PRE-SWIZZLED in HBM ([64-row block]
-//                [K chunk][64 x 128 B in the SWIZZLE_128B pattern]) so a stage is one contiguous 8 KB cp.async.bulk copy (row-major
-//                fp32 stays the source of truth; the shadow is private, derived).  In a cluster of two CTAs (optional; single CTAs
-//                are faster on the H100) each CTA fetches half of every stage and multicasts it to both, which own consecutive
-//                query blocks.
-//   warps 2, 3   bookkeepers: warp 2 + w serves the candidate queue of consumer warpgroup w (below): the row's own bound, the
+// Roles (512 threads = four warpgroups, 1 CTA per SM, persistent over 128-row tiles; every thread gets 128 registers, which the
+// consumers' int32 accumulators and block test fit; ptxas ignores a setmaxnreg split of 80 for warpgroup 0 and 144 for the
+// consumers "to maintain minimum register requirements", so the register file stays evenly split):
+//   warp 0       producer: loads the query block (NQ x dim int8 codes) once by TMA, then streams the walker's 64-row shadow blocks
+//                in BLOCK ORDER (below), one K chunk (64 rows x 128 codes = 8 KB) per stage, through ONE RING of up to kTcStages
+//                stages shared by all consumers.  The shadow is stored TILED and PRE-SWIZZLED in HBM ([64-row block][K chunk]
+//                [64 x 128 B in the SWIZZLE_128B pattern]) so a stage is one contiguous 8 KB cp.async.bulk copy (row-major fp32
+//                stays the source of truth; the shadow is private, derived).  In a cluster of two CTAs (optional; single CTAs are
+//                faster on the H100) each CTA fetches half of every stage and multicasts it to both, which own consecutive query
+//                blocks.
+//   warps 1-3    bookkeepers: warp 1 + w serves the candidate queue of consumer warpgroup w (below): the row's own bound, the
 //                append to the per-query candidate lists in HBM, the bound list and tau, off the MMA path.
-//   warpgroups 1, 2   consumers: warpgroup w multiplies its 64-row blocks with the whole query block (wgmma.m64nNQk32.s32.s8.s8,
-//                both operands from shared memory, exact int32 accumulators in registers), releases each stage as soon as its MMAs
-//                retired, then tests its 64 x NQ scores against tau and hands every hit to its bookkeeper through a queue in shared
-//                memory.  The two warpgroups take turns issuing a block's MMAs (ping-pong), so one warpgroup's epilogue overlaps
-//                the other's MMAs.
+//   warpgroups 1-3   consumers: a walker's 64-row blocks form one sequence i = 0, 1, 2, ..., block i being half i % 2 of the tile
+//                walker + (i / 2) W, and consumer warpgroup i % 3 owns block i.  It multiplies the block with the whole query block
+//                (wgmma.m64nNQk32.s32.s8.s8, both operands from shared memory, exact int32 accumulators in registers), releases each
+//                stage as soon as its MMAs retired, then tests its 64 x NQ scores against tau and hands every hit to its bookkeeper
+//                through a queue in shared memory.  The warpgroups take turns issuing their blocks' MMAs in block order, so each
+//                warpgroup's epilogue (drain, test, append) overlaps the two other warpgroups' MMAs.
 #pragma once
 #include <cuda.h>
 
@@ -65,10 +68,12 @@
 
 namespace rxgpu {
 
-constexpr int kTcThreads = 384;
-constexpr int kTcTileRows = 128;     // two 64-row blocks (wgmma M = 64), one per consumer warpgroup
+constexpr int kTcThreads = 512;
+constexpr int kTcConsumers = 3;      // consumer warpgroups, each with its own bookkeeper warp, queue and (thr, P, R) copies
+constexpr int kTcTileRows = 128;     // two 64-row blocks (wgmma M = 64)
 constexpr int kTcChunkK = 128;       // int8 codes per 128-byte swizzle row
-constexpr int kTcStages = 6;         // stages per consumer warpgroup ring
+constexpr int kTcStages = 12;        // ring stages (tc_ring_stages takes fewer only where 12 leave no room for the queues)
+constexpr int kTcStagesMin = 8;
 constexpr int kTcBlockBytes = 64 * kTcChunkK;               // 8 KB: one 64-row shadow block of one K chunk = one stage
 constexpr uint32_t kTcMaxNq = 128;   // queries per CTA (wgmma N <= 128 keeps the accumulators at <= 64 registers per thread)
 constexpr uint32_t kTcMaxK1 = 128;  // k + 1 <= 128: the bound list is scanned linearly under the per-query lock (larger k: staged)
@@ -100,14 +105,15 @@ struct TcArgs {
 	uint32_t k1;
 	int metric;                // kL2 / kIP / kCos
 	uint32_t queue_slots;      // records per candidate queue (tc_queue_slots; a power of two)
+	uint32_t stages;           // stages of the ring (tc_ring_stages)
 	unsigned long long* diag;  // diagnostic instantiations only (kDiag != 0): the counters of tc_diag_* below; unused otherwise
 };
 
 // Diagnostic instantiations of knn_tc_filter (template flag kDiag, 0 in every search; bench_tc_phases.py selects one through
 // rxgpu_tc_diag).  kTcDiagStamps stamps every phase of every tile with clock64(); the three ablations bound what the epilogue and the
 // row stream cost: kTcDiagNoRare compiles the rare path out (the block test stays, hits are only counted, tau never tightens),
-// kTcDiagNoFetch lets the producers cycle the barriers without fetching (the consumers multiply zeroed stages), and kTcDiagNoTest
-// compiles the block test and the rare path out (rings, MMAs, drain and both bar.syncs stay; the accumulators only feed an XOR sink
+// kTcDiagNoFetch lets the producer cycle the barriers without fetching (the consumers multiply zeroed stages), and kTcDiagNoTest
+// compiles the block test and the rare path out (ring, MMAs, turns, drain and both bar.syncs stay; the accumulators only feed an XOR sink
 // so the MMAs are kept).  Their candidate lists are meaningless; only the time and the counters are read.
 constexpr int kTcDiagStamps = 1;
 constexpr int kTcDiagNoRare = 2;
@@ -116,11 +122,11 @@ constexpr int kTcDiagNoTest = 4;
 // a.diag layout: [gridDim.x][kTcDiagSlots] per-CTA counters, then [kTcDiagWalk] hits per walk position (position i = the walker's
 // i-th tile, summed over all CTAs), then [gridDim.x][kTcDiagWalk / kTcDiagMarkEvery] %globaltimer marks taken when a CTA starts the
 // walk positions 0, kTcDiagMarkEvery, 2 kTcDiagMarkEvery, ...
-constexpr uint32_t kTcDiagSlots = 32;
+constexpr uint32_t kTcDiagSlots = 64;
 constexpr uint32_t kTcDiagWalk = 8192;
 constexpr uint32_t kTcDiagMarkEvery = 64;
 // per-CTA counters: consumer warpgroup w at w * kTcDgPerWg + (one of the phases below, in clock64 cycles summed over its four warps;
-// blocks, hits and queue waits are counts), producer ring r at kTcDgEmpty + r (cycles waiting on `empty`) and kTcDgProd + r (total)
+// blocks, hits and queue waits are counts), the producer at kTcDgEmpty (cycles waiting on `empty`) and kTcDgProd (total)
 enum : uint32_t {
 	kTcDgFull,     // waiting on full[stage]
 	kTcDgMma,      // the rest of the K loop: tau refresh, row constants, MMA issue, wgmma_wait<1>, stage release, handing the turn over
@@ -136,18 +142,18 @@ enum : uint32_t {
 	kTcDgHits,     // (query, row) pairs that passed the block test (count)
 	kTcDgQueueWait,  // enqueues that found the candidate queue full (count)
 	kTcDgPerWg,
-	kTcDgEmpty = 2 * kTcDgPerWg,
-	kTcDgProd = kTcDgEmpty + 2,
-	kTcDgRescored = kTcDgProd + 2,  // bookkeepers (both warps summed): rows whose exact distance they computed (count), ...
+	kTcDgEmpty = kTcConsumers * kTcDgPerWg,
+	kTcDgProd = kTcDgEmpty + 1,
+	kTcDgRescored = kTcDgProd + 1,  // bookkeepers (all three warps summed): rows whose exact distance they computed (count), ...
 	kTcDgInserts,                   // ... bound-list inserts attempted under the lock (count), ...
 	kTcDgRescoreCycles,             // ... and clock64 cycles spent computing those distances (stamped instantiation only)
 };
 static_assert(kTcDgRescoreCycles < kTcDiagSlots, "diagnostic counters fit their slots");
 
-// shared memory: query block, two stage rings, barriers, per-query constants, then per consumer warpgroup thresholds and (P, R)
-__host__ __device__ inline size_t tc_smem_bytes(uint32_t nq_block, uint32_t kchunks) {
-	return 1024 /*align slack*/ + size_t(nq_block) * kchunks * 128 + size_t(2 * kTcStages) * kTcBlockBytes + 256 /*barriers*/ +
-		   size_t(nq_block) * (16 /*qc*/ + 2 * (4 + 8) /*thr, pr per warpgroup*/) + 64;
+// shared memory: query block, the stage ring, barriers, per-query constants, then per consumer warpgroup thresholds and (P, R)
+__host__ __device__ inline size_t tc_smem_bytes(uint32_t nq_block, uint32_t kchunks, uint32_t stages = kTcStages) {
+	return 1024 /*align slack*/ + size_t(nq_block) * kchunks * 128 + size_t(stages) * kTcBlockBytes + 256 /*barriers*/ +
+		   size_t(nq_block) * (16 /*qc*/ + kTcConsumers * (4 + 8) /*thr, pr per warpgroup*/) + 64;
 }
 
 // ---- PTX wrappers -------------------------------------------------------------------------------------------------------------
@@ -337,8 +343,8 @@ __device__ __forceinline__ float2 tc_make_pr(int metric, float tau, float4 qc, f
 // ---- the candidate queue: consumers -> bookkeepers --------------------------------------------------------------------------------
 // A (query, row) pair that passes the block test is a hit.  The consumer warpgroup that found it only enqueues it: one shared-memory
 // atomicAdd takes a ticket, a 16-byte record (query in the block, row, x = float(I), ticket + 1) goes into the warpgroup's ring of
-// `slots` records, the last word stored with release semantics.  Its BOOKKEEPER warp (warp 2 for consumer warpgroup 0, warp 3 for
-// warpgroup 1; idle otherwise) takes the records in ticket order, up to 32 at a time, frees their slots, and runs the rare path off
+// `slots` records, the last word stored with release semantics.  Its BOOKKEEPER warp (warp 1 + w for consumer warpgroup w; idle
+// otherwise) takes the records in ticket order, up to 32 at a time, frees their slots, and runs the rare path off
 // the MMA path: the row's own bound, the candidate append, the bound list and tau.  A full ring makes the consumer wait until the
 // bookkeeper frees a slot; no hit is ever dropped.
 struct TcQueue {
@@ -347,14 +353,26 @@ struct TcQueue {
 	uint32_t done;        // consumer warps that finished their walk
 	uint32_t full_waits;  // diagnostic instantiations: enqueues that found the ring full
 };
-constexpr uint32_t kTcQueueMax = 512;  // records per consumer warpgroup at most (2 x 8 KB), ...
-constexpr uint32_t kTcQueueMin = 128;  // ... and at least: what tc_smem_bytes leaves free under the opt-in limit at every shape
-__host__ __device__ inline size_t tc_queue_bytes(uint32_t slots) { return 2 * sizeof(TcQueue) + size_t(2) * slots * 16; }
-// records per ring: the largest power of two in [kTcQueueMin, kTcQueueMax] whose rings fit beside the layout tc_smem_bytes counts
-// (0: none fits -- tcQueryBlock never picks such a shape)
-inline uint32_t tc_queue_slots(uint32_t nq_block, uint32_t kchunks, size_t limit) {
+constexpr uint32_t kTcQueueMax = 512;  // records per consumer warpgroup at most (3 x 8 KB), ...
+constexpr uint32_t kTcQueueMin = 128;  // ... and at least, at every shape tcQueryBlock picks
+__host__ __device__ inline size_t tc_queue_bytes(uint32_t slots) {
+	return kTcConsumers * sizeof(TcQueue) + size_t(kTcConsumers) * slots * 16;
+}
+// stages of the ring: kTcStages, or the most below it that leave kTcQueueMin records per queue (1153 to 1280 dims at a query block
+// of 96 are the only shapes of tcQueryBlock that need fewer: 11); 0 when even kTcStagesMin stages leave too little
+inline uint32_t tc_ring_stages(uint32_t nq_block, uint32_t kchunks, size_t limit) {
+	for (uint32_t s = kTcStages; s >= uint32_t(kTcStagesMin); --s) {
+		if (tc_smem_bytes(nq_block, kchunks, s) + tc_queue_bytes(kTcQueueMin) <= limit) {
+			return s;
+		}
+	}
+	return 0;
+}
+// records per queue: the largest power of two in [kTcQueueMin, kTcQueueMax] whose queues fit beside the layout tc_smem_bytes counts
+// (0: none fits)
+inline uint32_t tc_queue_slots(uint32_t nq_block, uint32_t kchunks, uint32_t stages, size_t limit) {
 	for (uint32_t s = kTcQueueMax; s >= kTcQueueMin; s /= 2) {
-		if (tc_smem_bytes(nq_block, kchunks) + tc_queue_bytes(s) <= limit) {
+		if (tc_smem_bytes(nq_block, kchunks, stages) + tc_queue_bytes(s) <= limit) {
 			return s;
 		}
 	}
@@ -475,9 +493,18 @@ __device__ __noinline__ float tc_rescore(const TcArgs& a, unsigned todo, uint32_
 // when its own lower bound d~ - err passes the tightest threshold the CTA knows for the query (NaN: appended); the appends of one
 // batch go to the candidate lists with one global atomicAdd per distinct query.  When the row's midpoint d~ beats that threshold
 // (and the seed does not hold the row already) the warp computes the row's EXACT distance d with the exact scan's arithmetic; a d
-// below the threshold goes into the bound list, and the threshold that comes back is published to the (P, R) of BOTH consumer
-// warpgroups.  A consumer may read a looser threshold meanwhile (a concurrent store of another writer may even replace a tighter one):
+// below the threshold goes into the bound list, and the threshold that comes back is published to the (P, R) of EVERY consumer
+// warpgroup.  A consumer may read a looser threshold meanwhile (a concurrent store of another writer may even replace a tighter one):
 // every threshold ever published is a valid upper bound of the query's final k1-th distance, so the test stays certified.
+template <int kNq>
+__device__ __forceinline__ float tc_min_thr(const float* s_thr, uint32_t ql) {  // the tightest threshold of the consumer warpgroups
+	float t = s_thr[ql];
+#pragma unroll
+	for (int w = 1; w < kTcConsumers; ++w) {
+		t = fminf(t, s_thr[w * kNq + ql]);
+	}
+	return t;
+}
 template <int kNq, int kDiag>
 __device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, const uint4* rec, uint32_t slots, uint32_t q0, const float4* s_qc,
 											  float* s_thr, float2* s_pr, float l2eps, int lane, unsigned long long* dg) {
@@ -517,7 +544,7 @@ __device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, cons
 			const float2 de = tc_row_bound(a, x, qc, rc);
 			d = de.x;
 			err = de.y;
-			tau = fminf(s_thr[ql], s_thr[kNq + ql]);
+			tau = tc_min_thr<kNq>(s_thr, ql);
 		}
 		const bool append = active && !(d - err > tau);
 		const unsigned peers = __match_any_sync(0xffffffffu, append ? ql : ~0u);
@@ -546,12 +573,12 @@ __device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, cons
 					rescore_cycles += clock64() - c0;
 				}
 			}
-			if (rescore && dx < fminf(s_thr[ql], s_thr[kNq + ql])) {  // the threshold may have dropped while the batch was rescored
+			if (rescore && dx < tc_min_thr<kNq>(s_thr, ql)) {  // the threshold may have dropped while the batch was rescored
 				if constexpr (kDiag != 0) {
 					++n_inserts;
 				}
 				const float nt = tc_bound_insert(a, q0 + ql, dx);
-				for (uint32_t w = 0; w < 2; ++w) {
+				for (uint32_t w = 0; w < kTcConsumers; ++w) {
 					if (nt < s_thr[w * kNq + ql]) {
 						s_thr[w * kNq + ql] = nt;
 						s_pr[w * kNq + ql] = tc_make_pr(a.metric, nt, s_qc[ql], l2eps);
@@ -593,18 +620,19 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 	unsigned char* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // offset arithmetic keeps the shared window
 	constexpr uint32_t kQchunkBytes = kNq * 128;                       // one K-chunk of the query block: kNq rows x 128 B
 	unsigned char* s_q = base;                                         // [kchunks][kNq][128 B], swizzled by TMA
-	unsigned char* s_rows = s_q + size_t(a.kchunks) * kQchunkBytes;    // [2 rings][stages][64][128 B]   (1024-aligned: kNq % 8 == 0)
-	uint64_t* bars = reinterpret_cast<uint64_t*>(s_rows + size_t(2 * kTcStages) * kTcBlockBytes);
-	uint64_t* full_bar = bars;                       // [2][stages] TMA -> MMA
-	uint64_t* empty_bar = bars + 2 * kTcStages;      // [2][stages] MMA (the consumer warps of the ring in every CTA of the cluster) -> TMA
-	uint64_t* q_bar = bars + 4 * kTcStages;          // queries resident
+	unsigned char* s_rows = s_q + size_t(a.kchunks) * kQchunkBytes;    // [stages][64][128 B]   (1024-aligned: kNq % 8 == 0)
+	const uint32_t nstages = a.stages;
+	uint64_t* bars = reinterpret_cast<uint64_t*>(s_rows + size_t(nstages) * kTcBlockBytes);
+	uint64_t* full_bar = bars;                       // [stages] TMA -> MMA
+	uint64_t* empty_bar = bars + kTcStages;          // [stages] MMA (the consumer warps of the stage's block in every CTA of the cluster) -> TMA
+	uint64_t* q_bar = bars + 2 * kTcStages;          // queries resident
 	float* s_ab = reinterpret_cast<float*>(q_bar + 1);                 // (a*, b*) of the block bound
 	float4* s_qc = reinterpret_cast<float4*>(bars + 32);               // [kNq] (s_q, r_q, n_q, 1 / k_q)
-	float* s_thr = reinterpret_cast<float*>(s_qc + kNq);               // [2][kNq] current tau (map space), per consumer warpgroup
-	float2* s_pr = reinterpret_cast<float2*>(s_thr + 2 * kNq);         // [2][kNq] (P, R) of the candidate test
-	TcQueue* s_queue = reinterpret_cast<TcQueue*>(s_pr + 2 * kNq);    // [2] candidate queue of each consumer warpgroup
-	uint4* s_rec = reinterpret_cast<uint4*>(s_queue + 2);              // [2][queue_slots] their records (beyond tc_smem_bytes)
-	static_assert(4 * kTcStages + 2 <= 32, "barriers and (a*, b*) fit in front of the per-query constants");
+	float* s_thr = reinterpret_cast<float*>(s_qc + kNq);               // [3][kNq] current tau (map space), per consumer warpgroup
+	float2* s_pr = reinterpret_cast<float2*>(s_thr + kTcConsumers * kNq);  // [3][kNq] (P, R) of the candidate test
+	TcQueue* s_queue = reinterpret_cast<TcQueue*>(s_pr + kTcConsumers * kNq);  // [3] candidate queue of each consumer warpgroup
+	uint4* s_rec = reinterpret_cast<uint4*>(s_queue + kTcConsumers);  // [3][queue_slots] their records (beyond tc_smem_bytes)
+	static_assert(2 * kTcStages + 2 <= 32, "barriers and (a*, b*) fit in front of the per-query constants");
 
 	const int warp = __shfl_sync(0xffffffffu, int(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;  // provably warp-uniform
 	const uint32_t ntiles = (a.n + kTcTileRows - 1) / kTcTileRows;
@@ -617,20 +645,22 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 	const float l2eps = tc_l2eps(a.dim);
 
 	if (threadIdx.x == 0) {
-		for (int s = 0; s < 2 * kTcStages; ++s) {
+		for (uint32_t s = 0; s < nstages; ++s) {
 			mbar_init(&full_bar[s], 1);
-			mbar_init(&empty_bar[s], 4 * kCluster);  // the four consumer warps of the ring's warpgroup in every CTA that reads the stage
+			mbar_init(&empty_bar[s], 4 * kCluster);  // the four warps of the warpgroup that owns the stage's block, in every CTA that reads it
 		}
 		mbar_init(q_bar, 1);
 		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 		s_ab[0] = s_ab[1] = 0.f;
-		s_queue[0] = s_queue[1] = TcQueue{0u, 0u, 0u, 0u};
+		for (int w = 0; w < kTcConsumers; ++w) {
+			s_queue[w] = TcQueue{0u, 0u, 0u, 0u};
+		}
 	}
-	for (uint32_t i = threadIdx.x; i < 2 * a.queue_slots; i += blockDim.x) {
+	for (uint32_t i = threadIdx.x; i < kTcConsumers * a.queue_slots; i += blockDim.x) {
 		s_rec[i].w = 0u;  // no ticket yet (a record of ticket t carries t + 1)
 	}
 	if constexpr (kDiag == kTcDiagNoFetch) {  // the stages the consumers multiply without a fetch hold zero codes
-		for (uint32_t i = threadIdx.x; i < 2 * kTcStages * kTcBlockBytes / 16; i += blockDim.x) {
+		for (uint32_t i = threadIdx.x; i < nstages * kTcBlockBytes / 16; i += blockDim.x) {
 			reinterpret_cast<uint4*>(s_rows)[i] = make_uint4(0u, 0u, 0u, 0u);
 		}
 		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -647,33 +677,37 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		}
 		s_qc[i] = qc;
 		const float2 pr = valid ? tc_make_pr(a.metric, thr, qc, l2eps) : make_float2(0.f, -INFINITY);  // padding queries never match
-		s_thr[i] = s_thr[kNq + i] = thr;
-		s_pr[i] = s_pr[kNq + i] = pr;
+		for (int w = 0; w < kTcConsumers; ++w) {
+			s_thr[w * kNq + i] = thr;
+			s_pr[w * kNq + i] = pr;
+		}
 	}
 	__syncthreads();
 	if constexpr (kCluster > 1) {
 		cluster_sync_all();  // the peers' barriers exist before anything of ours can signal them
 	}
+	// the walker's 64-row blocks i = 0, 1, ..., nblocks - 1: block i is half i % 2 of the tile walker + (i / 2) walkers, shadow block
+	// 2 (walker + (i / 2) walkers) + i % 2; its K chunk kc is the (i kchunks + kc)-th stage the producer fills
+	const uint32_t nblocks = walker < ntiles ? 2 * ((ntiles - walker + walkers - 1) / walkers) : 0u;
 
-	if (warp < 2) {
-		// ===== TMA producer of ring `warp`: the whole warp walks the loop, one elected lane issues (operands stay in uniform registers)
-		const uint32_t ring = uint32_t(warp);
-		if (ring == 0 && elect_one_sync()) {
+	if (warp == 0) {
+		// ===== TMA producer: the whole warp walks the loop, one elected lane issues (operands stay in uniform registers)
+		if (elect_one_sync()) {
 			mbar_expect_tx(q_bar, a.kchunks * kQchunkBytes);
 			for (uint32_t kc = 0; kc < a.kchunks; ++kc) {
 				tma_load_2d(s_q + size_t(kc) * kQchunkBytes, &map_queries, q_bar, int32_t(kc * kTcChunkK), int32_t(q0));
 			}
 		}
 		__syncwarp();
-		uint64_t* full = full_bar + ring * kTcStages;
-		uint64_t* empty = empty_bar + ring * kTcStages;
-		unsigned char* ring_smem = s_rows + size_t(ring) * kTcStages * kTcBlockBytes;
+		uint64_t* full = full_bar;
+		uint64_t* empty = empty_bar;
+		unsigned char* ring_smem = s_rows;
 		uint32_t stage = 0, phase = 0;
 		[[maybe_unused]] long long t_empty = 0;
 		[[maybe_unused]] const long long t_start = clk();
-		for (uint32_t t = walker; t < ntiles; t += walkers) {
-			// the 64-row shadow block 2t + ring, its K chunks 8 KB apart in HBM
-			const unsigned char* src = a.shadow + size_t(2 * t + ring) * a.kchunks * kTcBlockBytes;
+		for (uint32_t i = 0; i < nblocks; ++i) {
+			// the walker's block i, its K chunks 8 KB apart in HBM
+			const unsigned char* src = a.shadow + size_t(2 * (walker + (i >> 1) * walkers) + (i & 1u)) * a.kchunks * kTcBlockBytes;
 			for (uint32_t kc = 0; kc < a.kchunks; ++kc) {
 				[[maybe_unused]] const long long c0 = clk();
 				mbar_wait(&empty[stage], phase ^ 1);
@@ -696,7 +730,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 					}
 				}
 				__syncwarp();
-				if (++stage == kTcStages) {
+				if (++stage == nstages) {
 					stage = 0;
 					phase ^= 1;
 				}
@@ -704,25 +738,25 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		}
 		if constexpr (kStamp) {
 			if (lane == 0) {
-				atomicAdd(&dg[kTcDgEmpty + ring], (unsigned long long)t_empty);
-				atomicAdd(&dg[kTcDgProd + ring], (unsigned long long)(clk() - t_start));
+				atomicAdd(&dg[kTcDgEmpty], (unsigned long long)t_empty);
+				atomicAdd(&dg[kTcDgProd], (unsigned long long)(clk() - t_start));
 			}
 		}
 	} else if (warp < 4) {
-		// ===== bookkeeper of consumer warpgroup warp - 2 =====
-		const uint32_t wg = uint32_t(warp) - 2;
+		// ===== bookkeeper of consumer warpgroup warp - 1 =====
+		const uint32_t wg = uint32_t(warp) - 1;
 		tc_bookkeeper<kNq, kDiag>(a, s_queue + wg, s_rec + wg * a.queue_slots, a.queue_slots, q0, s_qc, s_thr, s_pr, l2eps, lane, dg);
 	} else {
-		// ===== consumer warpgroup wg: the 64-row blocks 2t + wg of the walker's tiles t, through ring wg =====
+		// ===== consumer warpgroup wg: the walker's blocks i = wg, wg + 3, wg + 6, ... =====
 		const uint32_t wg = uint32_t(warp) / 4 - 1, wtid = threadIdx.x - 128 * (wg + 1);
 		float* thr = s_thr + wg * kNq;
 		float2* pr = s_pr + wg * kNq;
 		TcQueue* qu = s_queue + wg;
 		uint4* rec = s_rec + wg * a.queue_slots;
 		const uint32_t slots = a.queue_slots;
-		uint64_t* full = full_bar + wg * kTcStages;
-		uint64_t* empty = empty_bar + wg * kTcStages;
-		const unsigned char* ring_smem = s_rows + size_t(wg) * kTcStages * kTcBlockBytes;
+		uint64_t* full = full_bar;
+		uint64_t* empty = empty_bar;
+		const unsigned char* ring_smem = s_rows;
 		// accumulator fragment of wgmma.m64nN: d[4j + {0,1}] = (row r0, query 8j + 2c + {0,1}), d[4j + {2,3}] = the same for row r0 + 8
 		const uint32_t r0 = (wtid >> 5) * 16 + (lane >> 2), c2 = 2 * (lane & 3);
 		const uint32_t my_q = wtid;  // the query whose threshold this thread refreshes from the global list
@@ -739,22 +773,22 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 			}
 		};
 		mbar_wait(q_bar, 0);
-		uint32_t stage = 0, phase = 0;
 		[[maybe_unused]] long long dt[kTcDgPerWg] = {};  // kStamp: this warp's cycles per phase (kTcDg*)
 		[[maybe_unused]] unsigned long long nhits = 0;
 		[[maybe_unused]] uint32_t sink = 0;  // kTcDiagNoTest
-		for (uint32_t t = walker; t < ntiles; t += walkers) {
-			[[maybe_unused]] const uint32_t walk = (t - walker) / walkers;
+		for (uint32_t blk = wg; blk < nblocks; blk += kTcConsumers) {
+			const uint32_t t = walker + (blk >> 1) * walkers, half = blk & 1u;
+			[[maybe_unused]] const uint32_t walk = blk >> 1;
 			[[maybe_unused]] long long s0 = clk(), s1, s2, s3, s4, s5;
 			if constexpr (kStamp) {
-				if (wg == 0 && wtid == 0 && walk % kTcDiagMarkEvery == 0 && walk < kTcDiagWalk) {
+				if (half == 0 && wtid == 0 && walk % kTcDiagMarkEvery == 0 && walk < kTcDiagWalk) {
 					unsigned long long now;
 					asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
 					a.diag[size_t(gridDim.x) * kTcDiagSlots + kTcDiagWalk + size_t(blockIdx.x) * (kTcDiagWalk / kTcDiagMarkEvery) +
 						   walk / kTcDiagMarkEvery] = now;
 				}
 			}
-			// refresh tau from the other CTAs: the global load was issued during the PREVIOUS tile, so its latency is hidden
+			// refresh tau from the other CTAs: the global load was issued during the PREVIOUS block, so its latency is hidden
 			if (my_q < nq_valid) {
 				const float tn = ord_float(tau_ahead);
 				if (tn < thr[my_q]) {
@@ -763,23 +797,32 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 				}
 				tau_ahead = a.tau[q0 + my_q];
 			}
-			const uint32_t row0 = (2 * t + wg) * 64 + r0, row1 = row0 + 8;
+			const uint32_t row0 = (2 * t + half) * 64 + r0, row1 = row0 + 8;
 			const float4 rc0 = a.rowc[row0], rc1 = a.rowc[row1];  // rows are padded to whole tiles; consumed after the MMAs
 			int acc[kNq / 2];
 #pragma unroll
 			for (int i = 0; i < kNq / 2; ++i) {
 				acc[i] = 0;
 			}
-			// Warpgroup turns (ping-pong): the two consumer warpgroups take turns issuing a block's MMAs, so one's block test runs
-			// under the other's MMAs instead of both testing at once while the tensor pipe idles.  Warpgroup w waits on named barrier
-			// 3 + w, which the other warpgroup arrives on once it has issued its block's last chunk.  No deadlock: both warpgroups walk
-			// the same tiles (block 2t + wg of every tile t), so their turns alternate 0, 1, 0, 1, ...; warpgroup 0 takes the first turn
-			// without waiting, and warpgroup 1 does not hand over after its last block, so no arrival is left pending at exit.  The
-			// producers and the bookkeepers never wait on a turn.  In a cluster of two each CTA orders its own warpgroups in the same
-			// order, and a stage shared with the peer only waits on the peer's same warpgroup at an earlier point of that order.
+			// Warpgroup turns: the three consumer warpgroups issue their blocks' MMAs in block order, so each one's drain, test and
+			// append run under the two others' MMAs instead of all of them testing at once while the tensor pipe idles.  The owner of
+			// block blk waits on named barrier 4 + blk % 3 (its own), except for block 0; the owner of block blk - 1 arrives on it
+			// once it has issued that block's last chunk, and only if block blk exists, so every wait has exactly one arrival and no
+			// arrival is left pending at exit, whatever the walker's block count (0, 1, 2 or any residue mod 3).  A barrier never
+			// holds two pending arrivals: the arrival for block j needs block j - 1 issued, which needs block j - 1's wait completed,
+			// which needs block j - 2 issued and so block j - 3's wait completed -- the previous use of the same barrier.  No
+			// deadlock: the producer fills the ring strictly in block order and a consumer consumes in the same order, so by induction
+			// over the global chunk index g = blk kchunks + kc every chunk below g is issued; the stage chunk g needs was then released
+			// (chunk g - stages is released when chunk g - stages + 1 of the same block is issued, or by the drain of a block's last
+			// chunk, which waits on nothing), so chunk g arrives, and its owner's turn came with the last chunk of block blk - 1.  The
+			// producer and the bookkeepers never wait on a turn.  In a cluster of two both CTAs walk the same blocks in the same order
+			// with the same owners, and the induction runs over the chunks of both: a stage goes back to a producer once the owning
+			// warpgroup of every CTA released it.
+			const uint32_t g0 = blk * a.kchunks;
+			uint32_t stage = g0 % nstages, phase = (g0 / nstages) & 1u;
 			[[maybe_unused]] const long long c_turn = clk();
-			if (wg == 1 || t != walker) {
-				asm volatile("bar.sync %0, 256;" ::"r"(3 + wg) : "memory");
+			if (blk != 0) {
+				asm volatile("bar.sync %0, 256;" ::"r"(4 + wg) : "memory");
 			}
 			if constexpr (kStamp) {
 				dt[kTcDgTurn] += clk() - c_turn;
@@ -806,14 +849,14 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 					}
 				}
 				prev = stage;
-				if (++stage == kTcStages) {
+				if (++stage == nstages) {
 					stage = 0;
 					phase ^= 1;
 				}
 			}
-			// hand the turn over once the last chunk is issued, before it retires (warpgroup 1: unless this was its last block)
-			if (wg == 0 || t + walkers < ntiles) {
-				asm volatile("bar.arrive %0, 256;" ::"r"(3 + (wg ^ 1)) : "memory");
+			// hand the turn to the owner of block blk + 1 once the last chunk is issued, before it retires (if that block exists)
+			if (blk + 1 < nblocks) {
+				asm volatile("bar.arrive %0, 256;" ::"r"(4 + (wg + 1) % kTcConsumers) : "memory");
 			}
 			s1 = clk();
 			wgmma_wait<0>();
@@ -898,7 +941,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 					}
 				}
 			}
-			__syncwarp();  // the rare path diverges (per-lane queue waits): reconverge before the .aligned wgmma of the next tile
+			__syncwarp();  // the rare path diverges (per-lane queue waits): reconverge before the .aligned wgmma of the next block
 			s5 = clk();
 			asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // nobody still reads (P, R) when the next refresh writes them
 			if constexpr (kStamp) {
@@ -943,7 +986,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 	}
 	__syncthreads();  // every bookkeeper has drained its queue
 	if constexpr (kStamp) {
-		if (threadIdx.x < 2) {
+		if (threadIdx.x < kTcConsumers) {
 			dg[threadIdx.x * kTcDgPerWg + kTcDgQueueWait] = s_queue[threadIdx.x].full_waits;
 		}
 	}
