@@ -351,6 +351,16 @@ int rxgpu_ivf_search_knn_large_k(const rxgpu_index*, uint32_t nq, const float* q
  * dist < radius in map space (strict; IP / Cosine radius negated by the caller), best first; *out_n = total number of matches. */
 int rxgpu_ivf_search_range(const rxgpu_index*, const float* query /* host */, float radius, uint32_t nprobe, uint64_t max_out,
 						   float* out_dist, uint64_t* out_label, uint64_t* out_n);
+/* A batch of IVF range searches.  radius[q] is in map space, exactly as for rxgpu_ivf_search_range.  Per query q the result is identical
+ * to rxgpu_ivf_search_range(queries + q*dim, radius[q], nprobe, max_out, ...): out_n[q] = total matches, and the best
+ * min(out_n[q], max_out) matches, best first in the order of hitLessByLabel (distance, then label), go into row q of
+ * out_dist / out_label (nq x max_out); the rest of a row is not written.  A NaN or -inf radius matches nothing, +inf every probed row.
+ * One coarse pass and one key pass over the probed lists serve the batch; each query's matches are counted, kept and sorted on the
+ * device (DESIGN.md §3.5), and no query is answered twice.  Same errors as rxgpu_ivf_search_range; device memory exhausted:
+ * RXGPU_ERR_SYSTEM.  rxgpu_last_search_stats: launches = all kernel launches, passes = 1, tc_fallbacks = 0. */
+int rxgpu_ivf_search_range_batch(const rxgpu_index*, uint32_t nq, const float* queries /* nq x dim, host */,
+								 const float* radius /* nq, map space */, uint32_t nprobe, uint64_t max_out,
+								 float* out_dist, uint64_t* out_label, uint64_t* out_n /* nq */);
 
 /* Mutable lists -- what IvfIndex::upsert / del do once the index is trained (ivf_index.cc:87-132: map_->add_with_ids(1, vec, &id),
  * map_->remove_ids(IDSelectorArray{1, &id})): rxgpu_ivf_create attaches EMPTY lists to an empty index (the rows then live in the lists:

@@ -170,6 +170,7 @@ _SIGNATURES = {
     "rxgpu_ivf_search_knn": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, C.c_uint32, C.c_uint32, _f32p, _u64p, _u32p]),
     "rxgpu_ivf_search_knn_large_k": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, C.c_uint32, C.c_uint32, _f32p, _u64p, _u32p]),
     "rxgpu_ivf_search_range": (C.c_int, [C.c_void_p, _f32p, C.c_float, C.c_uint32, C.c_uint64, _f32p, _u64p, C.POINTER(C.c_uint64)]),
+    "rxgpu_ivf_search_range_batch": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, _f32p, C.c_uint32, C.c_uint64, _f32p, _u64p, _u64p]),
     "rxgpu_ft_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_uint32, C.c_uint32, _u32p, _f32p, _u8p, C.c_int]),
     "rxgpu_ft_destroy": (None, [C.c_void_p]),
     "rxgpu_ft_add_postings": (C.c_int, [C.c_void_p, C.POINTER(FtPostings), _u32p]),
@@ -570,6 +571,20 @@ class GpuBruteforceSearch:
         _check(self._lib.rxgpu_ivf_search_range(self._h, _p(q, _f32p), radius, nprobe, max_out, _p(d, _f32p), _p(l, _u64p), C.byref(n)))
         m = min(n.value, max_out)
         return d[:m], l[:m], n.value
+
+    def ivf_search_range_batch(self, queries, radii, nprobe: int, max_out: int):
+        """rxgpu_ivf_search_range_batch.  queries: [nq, dim]; radii: a scalar or [nq] (map space, as ivf_search_range).  Returns
+        (dists [nq, max_out], labels [nq, max_out], counts [nq]): row q holds the best min(counts[q], max_out) matches of query q,
+        best-first, and counts[q] is its total number of matches."""
+        q = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, self.dim)
+        nq = q.shape[0]
+        r = np.ascontiguousarray(np.broadcast_to(np.asarray(radii, dtype=np.float32), (nq,)))
+        d = np.zeros((nq, max(max_out, 1)), np.float32)
+        l = np.zeros((nq, max(max_out, 1)), np.uint64)
+        c = np.zeros(nq, np.uint64)
+        _check(self._lib.rxgpu_ivf_search_range_batch(self._h, nq, _p(q, _f32p), _p(r, _f32p), nprobe, max_out, _p(d, _f32p), _p(l, _u64p),
+                                                      _p(c, _u64p)))
+        return d[:, :max_out], l[:, :max_out], c
 
     # -- bench / test support ------------------------------------------------------------------------------------------
     def append_synth(self, seed: int, first_row: int, n: int):

@@ -12,6 +12,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <limits>
 #include <memory>
 #include <mutex>
 #include <new>
@@ -26,6 +27,7 @@
 #include "knn_scan.cuh"
 #include "knn_tc.cuh"
 #include "ivf_select.cuh"
+#include "ivf_range.cuh"
 
 using namespace rxgpu;
 
@@ -1893,6 +1895,12 @@ struct rxgpu_ivf_device {
 	DevBuf<int> d_seg_begin, d_seg_end;
 	DevBuf<SelState> d_sel_state;
 	DevBuf<unsigned char> d_cub;
+	// range batch (rxgpu_ivf_search_range_batch), beside the key workspace and survivors above: radius per query, a chunk's key tiles
+	// (query, tile), its matches per query, a sub-chunk's survivor and output offsets
+	DevBuf<float> d_radius;
+	DevBuf<uint2> d_tiles;
+	DevBuf<uint32_t> d_range_n;
+	DevBuf<int> d_range_seg;
 	// mutable lists (rxgpu_ivf_create / _add / _remove): every list owns a region [begin, begin + cap) of a row slab; size <= cap
 	bool own = false;
 	float* rows = nullptr;       // [slab_rows][pitch]
@@ -1939,6 +1947,87 @@ int ivfLaunchCoarse(const rxgpu_index* ix, rxgpu_ivf_device* h, uint32_t nq, uin
 																		ix->metric == RXGPU_COS ? h->cnorm.p : nullptr, h->d_work.p);
 	}
 	RX_CUDA(cudaGetLastError());
+	return 0;
+}
+
+// the prologue of the key pass (rxgpu_ivf_search_knn_large_k, rxgpu_ivf_search_range_batch), under h->mtx: the coarse quantiser over
+// the nq queries, probed rows per query (h->d_qrows, and rows on the host) and their exclusive scan, each query's first key
+// (h->d_qoff; off[q] on the host, off[nq] = all probed rows).  3 launches.
+int ivfProbedRows(const rxgpu_index* ix, rxgpu_ivf_device* h, uint32_t nq, const float* queries, uint32_t nprobe, cudaStream_t st,
+				  std::vector<uint64_t>& rows, std::vector<uint64_t>& off) {
+	RX_CUDA(h->d_q.ensure(size_t(nq) * ix->dim));
+	RX_CUDA(h->d_work.ensure(size_t(nq) * nprobe));
+	RX_CUDA(h->d_qrows.ensure(nq));
+	RX_CUDA(h->d_qoff.ensure(nq));
+	RX_CUDA(cudaMemcpyAsync(h->d_q.p, queries, size_t(nq) * ix->dim * 4, cudaMemcpyHostToDevice, st));
+	if (int rc = ivfLaunchCoarse(ix, h, nq, nprobe, st)) {
+		return rc;
+	}
+	ivf_probe_rows_kernel<<<(nq + 7u) / 8u, 256, 0, st>>>(h->d_work.p, nq, nprobe, h->d_qrows.p);
+	RX_CUDA(cudaGetLastError());
+	size_t cubBytes = 0;
+	RX_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, cubBytes, h->d_qrows.p, h->d_qoff.p, int(nq), st));
+	RX_CUDA(h->d_cub.ensure(cubBytes));
+	RX_CUDA(cub::DeviceScan::ExclusiveSum(h->d_cub.p, cubBytes, h->d_qrows.p, h->d_qoff.p, int(nq), st));
+	rows.assign(nq, 0);
+	off.assign(size_t(nq) + 1, 0);
+	RX_CUDA(cudaMemcpyAsync(rows.data(), h->d_qrows.p, size_t(nq) * 8, cudaMemcpyDeviceToHost, st));
+	RX_CUDA(cudaStreamSynchronize(st));
+	for (uint32_t q = 0; q < nq; ++q) {
+		off[q + 1] = off[q] + rows[q];
+	}
+	return 0;
+}
+
+// the query chunk [q0, return value): at most kIvfKeyCap keys and slotsPerQuery * queries <= kIvfSlotCap; a query above the key cap is a
+// chunk of its own
+uint32_t ivfChunkEnd(const std::vector<uint64_t>& off, uint32_t q0, uint64_t slotsPerQuery) {
+	const uint32_t nq = uint32_t(off.size() - 1);
+	uint32_t q1 = q0 + 1;
+	while (q1 < nq && off[q1 + 1] - off[q0] <= kIvfKeyCap && uint64_t(q1 + 1 - q0) * slotsPerQuery <= kIvfSlotCap) {
+		++q1;
+	}
+	return q1;
+}
+
+// the key pass of the chunk [q0, q0 + cq) (nkeys > 0): the exact scan in work-item key mode, one CTA per (query, probed list), every
+// probed row's key to h->d_keys at the chunk's slot.  2 launches.
+int ivfKeyPass(const rxgpu_index* ix, rxgpu_ivf_device* h, uint32_t nq, uint32_t nprobe, uint32_t q0, uint32_t cq, uint64_t nkeys,
+			   cudaStream_t st) {
+	RX_CUDA(h->d_keys.ensure(std::max<uint64_t>(nkeys, 1)));
+	RX_CUDA(h->d_work_chunk.ensure(size_t(cq) * nprobe));
+	ivf_key_plan_kernel<<<(cq + 7u) / 8u, 256, 0, st>>>(h->d_work.p, nq, nprobe, q0, cq, h->d_qoff.p, h->d_work_chunk.p);
+	RX_CUDA(cudaGetLastError());
+	ScanArgs a{};
+	a.rows = h->own ? h->rows : ix->d_rows;
+	a.norm_coefs = ix->metric != RXGPU_COS ? nullptr : h->own ? h->norms : ix->d_norms;
+	a.queries = h->d_q.p;
+	a.pitch = ix->pitch;
+	a.dim = ix->dim;
+	a.nq = 1;
+	a.k1 = 1;
+	a.mode = kModeTopK;
+	a.work = h->d_work_chunk.p;
+	a.nwork = cq * nprobe;
+	a.lists = h->d_keys.p;
+	unsigned grid = 0;
+	RX_CUDA((launchScanQ<1, true>(ix, a, (ix->dim + 127u) / 128u, &grid, st, false)));
+	return 0;
+}
+
+// survivors h->d_sel_ord / d_sel_label [n items, nseg segments [begin[i], end[i])) into (distance, label) order, in place: stable radix
+// sorts by label, then by the ordered distance word (through d_sel_ord2 / d_sel_label2).  2 launches.
+int ivfSortSurvivors(rxgpu_ivf_device* h, int n, int nseg, int* begin, int* end, cudaStream_t st) {
+	size_t sortBytes = 0, sortBytes2 = 0;
+	RX_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, sortBytes, h->d_sel_label.p, h->d_sel_label2.p, h->d_sel_ord.p,
+													 h->d_sel_ord2.p, n, nseg, begin, end, 0, 64, st));
+	RX_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, sortBytes2, h->d_sel_ord2.p, h->d_sel_ord.p, h->d_sel_label2.p,
+													 h->d_sel_label.p, n, nseg, begin, end, 0, 32, st));
+	RX_CUDA(h->d_cub.ensure(std::max(sortBytes, sortBytes2)));
+	RX_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(h->d_cub.p, sortBytes, h->d_sel_label.p, h->d_sel_label2.p, h->d_sel_ord.p,
+													 h->d_sel_ord2.p, n, nseg, begin, end, 0, 64, st));
+	RX_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(h->d_cub.p, sortBytes2, h->d_sel_ord2.p, h->d_sel_ord.p, h->d_sel_label2.p,
+													 h->d_sel_label.p, n, nseg, begin, end, 0, 32, st));
 	return 0;
 }
 }  // namespace
@@ -2133,45 +2222,21 @@ int rxgpu_ivf_search_knn_large_k(const rxgpu_index* ix, uint32_t nq, const float
 	}
 	std::lock_guard<std::mutex> lck(h->mtx);
 	cudaStream_t st = ix->stream;
-	const size_t nwork = size_t(nq) * nprobe;
-	RX_CUDA(h->d_q.ensure(size_t(nq) * ix->dim));
-	RX_CUDA(h->d_work.ensure(nwork));
-	RX_CUDA(h->d_qrows.ensure(nq));
-	RX_CUDA(h->d_qoff.ensure(nq));
-	RX_CUDA(cudaMemcpyAsync(h->d_q.p, queries, size_t(nq) * ix->dim * 4, cudaMemcpyHostToDevice, st));
-	if (int rc = ivfLaunchCoarse(ix, h, nq, nprobe, st)) {
-		return rc;
-	}
-	// probed rows per query and their exclusive scan: each query's first key
-	ivf_probe_rows_kernel<<<(nq + 7u) / 8u, 256, 0, st>>>(h->d_work.p, nq, nprobe, h->d_qrows.p);
-	RX_CUDA(cudaGetLastError());
-	size_t cubBytes = 0;
-	RX_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, cubBytes, h->d_qrows.p, h->d_qoff.p, int(nq), st));
-	RX_CUDA(h->d_cub.ensure(cubBytes));
-	RX_CUDA(cub::DeviceScan::ExclusiveSum(h->d_cub.p, cubBytes, h->d_qrows.p, h->d_qoff.p, int(nq), st));
 	uint32_t launches = 3;  // coarse quantiser, probed rows, their scan (one CUB call)
 	try {
-		std::vector<uint64_t> rows(nq), off(size_t(nq) + 1, 0);
-		RX_CUDA(cudaMemcpyAsync(rows.data(), h->d_qrows.p, size_t(nq) * 8, cudaMemcpyDeviceToHost, st));
-		RX_CUDA(cudaStreamSynchronize(st));
-		for (uint32_t q = 0; q < nq; ++q) {
-			off[q + 1] = off[q] + rows[q];
+		std::vector<uint64_t> rows, off;
+		if (int rc = ivfProbedRows(ix, h, nq, queries, nprobe, st, rows, off)) {
+			return rc;
 		}
 		const uint64_t* labels = h->own ? h->labels : ix->d_labels;
-		const uint32_t nch = (ix->dim + 127u) / 128u;
 		std::vector<uint32_t> ord, cnt;
 		std::vector<uint64_t> lab;
 		// query chunks: at most kIvfKeyCap keys and kIvfSlotCap survivor slots each; a query above the key cap is a chunk of its own
 		for (uint32_t q0 = 0, q1 = 0; q0 < nq; q0 = q1) {
-			q1 = q0 + 1;
-			while (q1 < nq && off[q1 + 1] - off[q0] <= kIvfKeyCap && uint64_t(q1 + 1 - q0) * k <= kIvfSlotCap) {
-				++q1;
-			}
+			q1 = ivfChunkEnd(off, q0, k);
 			const uint32_t cq = q1 - q0;
 			const uint64_t nkeys = off[q1] - off[q0];
 			const size_t slots = size_t(cq) * k;
-			RX_CUDA(h->d_keys.ensure(std::max<uint64_t>(nkeys, 1)));
-			RX_CUDA(h->d_work_chunk.ensure(size_t(cq) * nprobe));
 			RX_CUDA(h->d_sel_ord.ensure(slots));
 			RX_CUDA(h->d_sel_ord2.ensure(slots));
 			RX_CUDA(h->d_sel_label.ensure(slots));
@@ -2181,23 +2246,9 @@ int rxgpu_ivf_search_knn_large_k(const rxgpu_index* ix, uint32_t nq, const float
 			RX_CUDA(h->d_seg_end.ensure(cq));
 			RX_CUDA(cudaMemsetAsync(h->d_sel_count.p, 0, size_t(cq) * 4, st));
 			if (nkeys) {
-				// key pass: the exact scan in work-item key mode, one CTA per (query, probed list)
-				ivf_key_plan_kernel<<<(cq + 7u) / 8u, 256, 0, st>>>(h->d_work.p, nq, nprobe, q0, cq, h->d_qoff.p, h->d_work_chunk.p);
-				RX_CUDA(cudaGetLastError());
-				ScanArgs a{};
-				a.rows = h->own ? h->rows : ix->d_rows;
-				a.norm_coefs = ix->metric != RXGPU_COS ? nullptr : h->own ? h->norms : ix->d_norms;
-				a.queries = h->d_q.p;
-				a.pitch = ix->pitch;
-				a.dim = ix->dim;
-				a.nq = 1;
-				a.k1 = 1;
-				a.mode = kModeTopK;
-				a.work = h->d_work_chunk.p;
-				a.nwork = cq * nprobe;
-				a.lists = h->d_keys.p;
-				unsigned grid = 0;
-				RX_CUDA((launchScanQ<1, true>(ix, a, nch, &grid, st, false)));
+				if (int rc = ivfKeyPass(ix, h, nq, nprobe, q0, cq, nkeys, st)) {
+					return rc;
+				}
 				ivf_select_cta_kernel<<<cq, kIvfSelThreads, 0, st>>>(h->d_keys.p, h->d_qoff.p + q0, h->d_qrows.p + q0, off[q0], k, labels,
 																  h->d_sel_ord.p, h->d_sel_label.p, h->d_sel_count.p);
 				RX_CUDA(cudaGetLastError());
@@ -2226,16 +2277,9 @@ int rxgpu_ivf_search_knn_large_k(const rxgpu_index* ix, uint32_t nq, const float
 				// order the survivors by (distance, label): stable radix sorts by label, then by the ordered distance word
 				ivf_sort_bounds_kernel<<<(cq + 255u) / 256u, 256, 0, st>>>(h->d_sel_count.p, k, cq, h->d_seg_begin.p, h->d_seg_end.p);
 				RX_CUDA(cudaGetLastError());
-				size_t sortBytes = 0, sortBytes2 = 0;
-				RX_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, sortBytes, h->d_sel_label.p, h->d_sel_label2.p, h->d_sel_ord.p,
-																 h->d_sel_ord2.p, int(slots), int(cq), h->d_seg_begin.p, h->d_seg_end.p, 0, 64, st));
-				RX_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(nullptr, sortBytes2, h->d_sel_ord2.p, h->d_sel_ord.p, h->d_sel_label2.p,
-																 h->d_sel_label.p, int(slots), int(cq), h->d_seg_begin.p, h->d_seg_end.p, 0, 32, st));
-				RX_CUDA(h->d_cub.ensure(std::max(sortBytes, sortBytes2)));
-				RX_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(h->d_cub.p, sortBytes, h->d_sel_label.p, h->d_sel_label2.p, h->d_sel_ord.p,
-																 h->d_sel_ord2.p, int(slots), int(cq), h->d_seg_begin.p, h->d_seg_end.p, 0, 64, st));
-				RX_CUDA(cub::DeviceSegmentedRadixSort::SortPairs(h->d_cub.p, sortBytes2, h->d_sel_ord2.p, h->d_sel_ord.p, h->d_sel_label2.p,
-																 h->d_sel_label.p, int(slots), int(cq), h->d_seg_begin.p, h->d_seg_end.p, 0, 32, st));
+				if (int rc = ivfSortSurvivors(h, int(slots), int(cq), h->d_seg_begin.p, h->d_seg_end.p, st)) {
+					return rc;
+				}
 				launches += 3;
 			}
 			ord.resize(slots);
@@ -2345,6 +2389,152 @@ int rxgpu_ivf_search_range(const rxgpu_index* ix, const float* query, float radi
 			out_dist[j] = res[j].dist;
 			out_label[j] = res[j].label;
 		}
+	} catch (const std::bad_alloc&) {
+		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
+	}
+	return 0;
+}
+
+int rxgpu_ivf_search_range_batch(const rxgpu_index* ix, uint32_t nq, const float* queries, const float* radius, uint32_t nprobe,
+								 uint64_t max_out, float* out_dist, uint64_t* out_label, uint64_t* out_n) {
+	if (int rc = checkIndex(ix)) {
+		return rc;
+	}
+	g_stats = rxgpu_search_stats{};
+	if (nq == 0) {
+		return 0;
+	}
+	if (!queries || !radius || !out_n || (max_out && (!out_dist || !out_label))) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: null argument");
+	}
+	rxgpu_ivf_device* h = ix->ivf;
+	if (!h) {
+		return fail(RXGPU_ERR_LOGIC, "rxgpu: no IVF lists imported into this index");
+	}
+	if (h->index_version != ix->version) {
+		return fail(RXGPU_ERR_LOGIC, "rxgpu: the index changed after the IVF lists were imported");
+	}
+	nprobe = std::max(1u, std::min(nprobe, h->nlist));
+	if (int rc = ivfCheckCoarseSmem(ix, h)) {
+		return rc;
+	}
+	std::lock_guard<std::mutex> lck(h->mtx);
+	cudaStream_t st = ix->stream;
+	uint32_t launches = 3;  // coarse quantiser, probed rows, their scan
+	try {
+		std::vector<uint64_t> rows, off;
+		if (int rc = ivfProbedRows(ix, h, nq, queries, nprobe, st, rows, off)) {
+			return rc;
+		}
+		RX_CUDA(h->d_radius.ensure(nq));
+		RX_CUDA(cudaMemcpyAsync(h->d_radius.p, radius, size_t(nq) * 4, cudaMemcpyHostToDevice, st));
+		const uint64_t* labels = h->own ? h->labels : ix->d_labels;
+		std::vector<uint2> tiles;
+		std::vector<size_t> tileAt;
+		std::vector<uint32_t> cnt;
+		std::vector<int> plan;
+		std::vector<float> dist;
+		std::vector<uint64_t> lab;
+		// the key chunks of the any-k select (no survivor slots to bound yet: a query's matches are counted before they are kept)
+		for (uint32_t q0 = 0, q1 = 0; q0 < nq; q0 = q1) {
+			q1 = ivfChunkEnd(off, q0, 0);
+			const uint32_t cq = q1 - q0;
+			const uint64_t nkeys = off[q1] - off[q0];
+			if (nkeys == 0) {
+				std::fill(out_n + q0, out_n + q1, uint64_t(0));
+				continue;
+			}
+			if (int rc = ivfKeyPass(ix, h, nq, nprobe, q0, cq, nkeys, st)) {
+				return rc;
+			}
+			tiles.clear();
+			tileAt.assign(size_t(cq) + 1, 0);
+			for (uint32_t qi = 0; qi < cq; ++qi) {
+				for (uint64_t j = 0; j * kIvfRangeTile < rows[q0 + qi]; ++j) {
+					tiles.push_back(make_uint2(qi, uint32_t(j)));
+				}
+				tileAt[qi + 1] = tiles.size();
+			}
+			RX_CUDA(h->d_tiles.ensure(tiles.size()));
+			RX_CUDA(h->d_range_n.ensure(cq));
+			RX_CUDA(h->d_sel_count.ensure(cq));
+			RX_CUDA(cudaMemcpyAsync(h->d_tiles.p, tiles.data(), tiles.size() * sizeof(uint2), cudaMemcpyHostToDevice, st));
+			RX_CUDA(cudaMemsetAsync(h->d_range_n.p, 0, size_t(cq) * 4, st));
+			RX_CUDA(cudaMemsetAsync(h->d_sel_count.p, 0, size_t(cq) * 4, st));
+			ivf_range_count_kernel<<<unsigned(tiles.size()), kIvfRangeThreads, 0, st>>>(
+				h->d_keys.p, h->d_qoff.p + q0, h->d_qrows.p + q0, off[q0], h->d_radius.p + q0, h->d_tiles.p, h->d_range_n.p);
+			RX_CUDA(cudaGetLastError());
+			launches += 3;  // key plan, key scan, count
+			cnt.resize(cq);
+			RX_CUDA(cudaMemcpyAsync(cnt.data(), h->d_range_n.p, size_t(cq) * 4, cudaMemcpyDeviceToHost, st));
+			RX_CUDA(cudaStreamSynchronize(st));
+			for (uint32_t qi = 0; qi < cq; ++qi) {
+				out_n[q0 + qi] = cnt[qi];
+			}
+			if (max_out == 0) {
+				continue;
+			}
+			// survivor sub-chunks of at most kIvfSlotCap matches; a query with more is a sub-chunk of its own
+			for (uint32_t s0 = 0, s1 = 0; s0 < cq; s0 = s1) {
+				uint64_t total = cnt[s0];
+				for (s1 = s0 + 1; s1 < cq && total + cnt[s1] <= kIvfSlotCap; ++s1) {
+					total += cnt[s1];
+				}
+				if (total == 0) {
+					continue;
+				}
+				if (total > uint64_t(std::numeric_limits<int>::max())) {  // the segmented sorts count items in an int
+					return fail(RXGPU_ERR_PARAMS, "rxgpu: more than 2^31 - 1 range matches for one IVF query");
+				}
+				const uint32_t ns = s1 - s0;
+				plan.assign(2 * (size_t(ns) + 1), 0);
+				int* seg = plan.data();     // survivors of query s0 + i: [seg[i], seg[i + 1])
+				int* pack = seg + ns + 1;   // its best min(matches, max_out) in the packed output: [pack[i], pack[i + 1])
+				int longest = 0;
+				for (uint32_t i = 0; i < ns; ++i) {
+					const int m = int(std::min<uint64_t>(cnt[s0 + i], max_out));
+					seg[i + 1] = seg[i] + int(cnt[s0 + i]);
+					pack[i + 1] = pack[i] + m;
+					longest = std::max(longest, m);
+				}
+				RX_CUDA(h->d_range_seg.ensure(plan.size()));
+				RX_CUDA(h->d_sel_ord.ensure(total));
+				RX_CUDA(h->d_sel_ord2.ensure(total));
+				RX_CUDA(h->d_sel_label.ensure(total));
+				RX_CUDA(h->d_sel_label2.ensure(total));
+				RX_CUDA(cudaMemcpyAsync(h->d_range_seg.p, plan.data(), plan.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+				int* dseg = h->d_range_seg.p;
+				const int* dpack = dseg + ns + 1;
+				ivf_range_emit_kernel<<<unsigned(tileAt[s1] - tileAt[s0]), kIvfRangeThreads, 0, st>>>(
+					h->d_keys.p, h->d_qoff.p + q0, h->d_qrows.p + q0, off[q0], h->d_radius.p + q0, h->d_tiles.p + tileAt[s0], s0, dseg, labels,
+					h->d_sel_count.p, h->d_sel_ord.p, h->d_sel_label.p);
+				RX_CUDA(cudaGetLastError());
+				if (int rc = ivfSortSurvivors(h, int(total), int(ns), dseg, dseg + 1, st)) {
+					return rc;
+				}
+				// the packed output goes to the sorts' second buffers, free again once the sorts are done
+				float* pdist = reinterpret_cast<float*>(h->d_sel_ord2.p);
+				const dim3 gg(ns, unsigned(std::min(1024, (longest + 255) / 256)));
+				ivf_range_gather_kernel<<<gg, 256, 0, st>>>(h->d_sel_ord.p, h->d_sel_label.p, dseg, dpack, pdist, h->d_sel_label2.p);
+				RX_CUDA(cudaGetLastError());
+				launches += 4;  // emit, two sorts, gather
+				dist.resize(size_t(pack[ns]));
+				lab.resize(size_t(pack[ns]));
+				RX_CUDA(cudaMemcpyAsync(dist.data(), pdist, dist.size() * 4, cudaMemcpyDeviceToHost, st));
+				RX_CUDA(cudaMemcpyAsync(lab.data(), h->d_sel_label2.p, lab.size() * 8, cudaMemcpyDeviceToHost, st));
+				RX_CUDA(cudaStreamSynchronize(st));
+				for (uint32_t i = 0; i < ns; ++i) {
+					const size_t at = size_t(q0 + s0 + i) * max_out;
+					std::copy(dist.begin() + pack[i], dist.begin() + pack[i + 1], out_dist + at);
+					std::copy(lab.begin() + pack[i], lab.begin() + pack[i + 1], out_label + at);
+				}
+			}
+		}
+		const uint64_t probed = off[nq];
+		g_stats.launches = launches;
+		g_stats.passes = 1;
+		// as rxgpu_ivf_search_knn_large_k: rows read once; each key written once and read once
+		g_stats.algorithmic_bytes = probed * ix->dim * 4 + (ix->metric == RXGPU_COS ? probed * 4 : 0) + probed * 16;
 	} catch (const std::bad_alloc&) {
 		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
 	}

@@ -4,8 +4,8 @@
 // clone, RebuildCentroids read its inverted lists and direct map through operator->), the four calls on the query/update path --
 //   search(1, key, k, dists, ids, &IVFSearchParameters{nprobe})      range_search(1, key, radius, &result, &params)
 //   add_with_ids(1, vec[, norm], &id)                                 remove_ids(IDSelectorArray{1, &id})
-// -- are served by librxgpu (include/rxgpu.h: rxgpu_ivf_create / _add / _remove / _search_knn_large_k / _search_range).  The device lists are
-// filled once, from the trained index, by the first search; after that every upsert / delete patches them in place (the list number
+// -- are served by librxgpu (include/rxgpu.h: rxgpu_ivf_create / _add / _remove / _search_knn_large_k / _search_range, and
+// _search_range_batch for range_search with n > 1).  The device lists are filled once, from the trained index, by the first search; after that every upsert / delete patches them in place (the list number
 // is read back from FAISS' direct map, so both sides agree on the assignment bit for bit).  Distances follow FAISS' conventions
 // (L2: squared distance ascending; inner product / cosine: +similarity descending, labels -1 past the end).
 // Meant to be dropped into cpp_src/core/index/float_vector/; compiled only where the reference tree is available
@@ -124,20 +124,27 @@ public:
 		const bool similarity = cpu_->metric_type != faiss::METRIC_L2;
 		std::vector<std::vector<float>> d(n);
 		std::vector<std::vector<uint64_t>> l(n);
-		for (faiss::idx_t q = 0; q < n; ++q) {
-			uint64_t total = 0;
-			d[q].resize(256);
-			l[q].resize(256);
-			const float r = similarity ? -radius : radius;  // map space: dist < r
-			check(rxgpu_ivf_search_range(gpu_, x + size_t(q) * cpu_->d, r, nprobe, d[q].size(), d[q].data(), l[q].data(), &total));
-			if (total > d[q].size()) {
+		if (n > 1) {  // one coarse pass and one scan of the probed lists for the whole batch
+			rangeBatch(n, x, similarity ? -radius : radius, nprobe, d, l);
+			for (faiss::idx_t q = 0; q < n; ++q) {
+				result->lims[q] = d[q].size();
+			}
+		} else {
+			for (faiss::idx_t q = 0; q < n; ++q) {
+				uint64_t total = 0;
+				d[q].resize(256);
+				l[q].resize(256);
+				const float r = similarity ? -radius : radius;  // map space: dist < r
+				check(rxgpu_ivf_search_range(gpu_, x + size_t(q) * cpu_->d, r, nprobe, d[q].size(), d[q].data(), l[q].data(), &total));
+				if (total > d[q].size()) {
+					d[q].resize(total);
+					l[q].resize(total);
+					check(rxgpu_ivf_search_range(gpu_, x + size_t(q) * cpu_->d, r, nprobe, d[q].size(), d[q].data(), l[q].data(), &total));
+				}
 				d[q].resize(total);
 				l[q].resize(total);
-				check(rxgpu_ivf_search_range(gpu_, x + size_t(q) * cpu_->d, r, nprobe, d[q].size(), d[q].data(), l[q].data(), &total));
+				result->lims[q] = total;
 			}
-			d[q].resize(total);
-			l[q].resize(total);
-			result->lims[q] = total;
 		}
 		result->do_allocation();  // turns the counts in lims into offsets and allocates labels / distances
 		for (faiss::idx_t q = 0; q < n; ++q) {
@@ -152,6 +159,42 @@ public:
 	const std::string& LastDeviceError() const noexcept { return lastError_; }
 
 private:
+	// n queries in one rxgpu_ivf_search_range_batch with room for 256 matches each, then one more batch of only the queries with more,
+	// with room for the largest of them; r in map space.  d[q] / l[q] receive all matches of query q, best first.
+	void rangeBatch(faiss::idx_t n, const float* x, float r, uint32_t nprobe, std::vector<std::vector<float>>& d,
+					std::vector<std::vector<uint64_t>>& l) const {
+		const size_t dim = cpu_->d;
+		uint64_t room = 256;
+		std::vector<float> rad(n, r), bd(size_t(n) * room);
+		std::vector<uint64_t> bl(size_t(n) * room), cnt(n);
+		check(rxgpu_ivf_search_range_batch(gpu_, uint32_t(n), x, rad.data(), nprobe, room, bd.data(), bl.data(), cnt.data()));
+		std::vector<faiss::idx_t> more;
+		uint64_t most = 0;
+		for (faiss::idx_t q = 0; q < n; ++q) {
+			if (cnt[q] > room) {
+				more.push_back(q);
+				most = std::max(most, cnt[q]);
+				continue;
+			}
+			d[q].assign(bd.begin() + size_t(q) * room, bd.begin() + size_t(q) * room + cnt[q]);
+			l[q].assign(bl.begin() + size_t(q) * room, bl.begin() + size_t(q) * room + cnt[q]);
+		}
+		if (more.empty()) {
+			return;
+		}
+		room = most;
+		std::vector<float> mq(more.size() * dim);
+		for (size_t i = 0; i < more.size(); ++i) {
+			std::copy(x + size_t(more[i]) * dim, x + size_t(more[i] + 1) * dim, mq.begin() + i * dim);
+		}
+		bd.assign(more.size() * room, 0.f);
+		bl.assign(more.size() * room, 0);
+		check(rxgpu_ivf_search_range_batch(gpu_, uint32_t(more.size()), mq.data(), rad.data(), nprobe, room, bd.data(), bl.data(), cnt.data()));
+		for (size_t i = 0; i < more.size(); ++i) {
+			d[more[i]].assign(bd.begin() + i * room, bd.begin() + i * room + cnt[i]);
+			l[more[i]].assign(bl.begin() + i * room, bl.begin() + i * room + cnt[i]);
+		}
+	}
 	static void check(int rc) {
 		if (rc != RXGPU_OK) {
 			throw std::runtime_error(rxgpu_last_error());
