@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Where the int8 filter launch spends its time at config 1 (10M x 768 fp32, inner product, k = 10, batch of 1024 queries).
 
-  python bench_tc_phases.py [--rows N] [--queries 1024] [--runs 5] [--out FILE]
+  python bench_tc_phases.py [--rows N] [--queries 1024] [--runs 5] [--cluster 1|2|4] [--out FILE]
 
 Runs the batch through the diagnostic instantiations of knn_tc_filter (knn_tc.cuh: kTcDiag*, selected with rxgpu_tc_diag; the
 searches themselves never take them) and prints one JSON line with
@@ -16,7 +16,8 @@ searches themselves never take them) and prints one JSON line with
                 ablations: (a) the rare path compiled out (block test kept, hits only counted), (b) the producer not fetching
                 (the consumers multiply zeroed stages; the barriers still cycle) and (c) the block test and the rare path compiled
                 out (ring, MMAs, turns, drain and bar.syncs kept): the MMA path's own floor.
-Clock stamps are cycles of the SM clock; the card, its power limit and the SM clock samples of the timed runs are in the line.
+--cluster C runs every instantiation in clusters of C CTAs that share each row stage by TMA multicast (rxgpu_set_tensor_core_filter
+3 / 4 / 5); the default is single CTAs.  Clock stamps are cycles of the SM clock; the card, its power limit and the SM clock samples of the timed runs are in the line.
 """
 import argparse
 import ctypes
@@ -49,6 +50,7 @@ def main(argv=None):
     ap.add_argument("--rows", type=int, default=ROWS_FULL)
     ap.add_argument("--queries", type=int, default=1024)
     ap.add_argument("--runs", type=int, default=5)
+    ap.add_argument("--cluster", type=int, default=1, choices=[1, 2, 4], help="CTAs per cluster sharing every row stage")
     ap.add_argument("--out", default=None, help="also write the JSON line (with the full hit histogram and marks) here")
     args = ap.parse_args(argv)
 
@@ -63,7 +65,7 @@ def main(argv=None):
     lib = B.lib()
     idx = rx.GpuBruteforceSearch(rx.IP, DIM, args.rows)
     idx.append_synth(SEED, 0, args.rows)
-    idx.set_tensor_core_filter(3)  # single CTAs, as the searches run by default
+    idx.set_tensor_core_filter({1: 3, 2: 4, 4: 5}[args.cluster])
     queries = bench_queries(args.queries)
     counters = torch.zeros(MAX_CTAS * SLOTS + WALK + MAX_CTAS * (WALK // MARK_EVERY), dtype=torch.int64, device="cuda:0")
 
@@ -76,7 +78,7 @@ def main(argv=None):
         st = rx.last_search_stats()
         lib.rxgpu_set_profile(0)
         B._check(lib.rxgpu_tc_diag(0, None))
-        if st["tc_used"] != 1 or st["scan_launches"] != 1 or st["tc_kernel"] != 1 + mode:
+        if st["tc_used"] != 1 or st["scan_launches"] != 1 or st["tc_kernel"] != 1 + mode or st["tc_cluster"] != args.cluster:
             raise SystemExit(f"bench_tc_phases.py: expected one filter launch, got {st}")
         return st["scan_kernel_ms"], st
 
@@ -101,11 +103,15 @@ def main(argv=None):
         print(json.dumps({name: launches[name], "clocks": clocks[name]}), file=sys.stderr, flush=True)
 
     c, st = stamped
-    # the launch shape of index.cu's tcLaunch at one CTA per SM: G query groups x W walkers, the counters laid out by its grid
+    # the launch shape of index.cu's tcLaunch: G query groups (C query blocks each) x W walkers x C CTAs.  The G C CTAs of a walker
+    # walk its 2 (its tiles) blocks each, so over the whole grid the blocks add up to 2 ntiles G C: the grid is the first multiple of
+    # G C whose CTAs' block counters (per warp, four warps per warpgroup) reach that sum
     ntiles = (args.rows + 127) // 128
-    groups = (args.queries + 127) // 128
-    walkers = min(torch.cuda.get_device_properties(0).multi_processor_count // groups, ntiles)
-    grid = groups * walkers
+    C = args.cluster
+    groups = ((args.queries + 127) // 128 + C - 1) // C
+    per_cta = c[:MAX_CTAS * SLOTS].reshape(MAX_CTAS, SLOTS)[:, [wg * PER_WG + BLOCKS for wg in range(CONSUMERS)]].sum(axis=1) / 4
+    grid = next(g for g in range(groups * C, MAX_CTAS + 1, groups * C) if per_cta[:g].sum() >= 2 * ntiles * groups * C)
+    walkers = grid // (groups * C)
     cta = c[:grid * SLOTS].reshape(grid, SLOTS)
     phases = {}
     for wg in range(CONSUMERS):
@@ -130,7 +136,7 @@ def main(argv=None):
     tiles_per_cta = ntiles / walkers
     spreads = []
     for w in range(walkers):
-        m = marks[w * groups:(w + 1) * groups]  # cid = walker * G + group (single CTAs)
+        m = marks[w * groups * C:(w + 1) * groups * C]  # CTA (walker * G + group) * C + rank in the cluster
         n = int(min(np.count_nonzero(row) for row in m))
         if n < 2:
             continue
@@ -138,7 +144,7 @@ def main(argv=None):
         for t in np.linspace(m[:, 0].max(), m[:, n - 1].min(), 16):
             reached = [np.interp(t, row[:n], pos) for row in m]
             spreads.append(max(reached) - min(reached))
-    drift = {"walkers": walkers, "ctas_per_walker": groups, "tiles_per_cta": tiles_per_cta,
+    drift = {"walkers": walkers, "ctas_per_walker": groups * C, "tiles_per_cta": tiles_per_cta,
              "spread_tiles_median": float(np.median(spreads)) if spreads else None,
              "spread_tiles_p90": float(np.percentile(spreads, 90)) if spreads else None,
              "spread_tiles_max": float(np.max(spreads)) if spreads else None}
@@ -148,7 +154,7 @@ def main(argv=None):
     ops = 2.0 * args.rows * DIM * args.queries
     line = {
         "workload": f"int8 filter launch, {args.rows} x {DIM}, inner product, k = {K}, batch of {args.queries}",
-        "card": card(), "grid": grid,
+        "card": card(), "cluster": C, "grid": grid,
         "launches": launches,
         "ablation_ceiling_no_rare_path_speedup": prod_ms / launches["no_rare_path"]["median_ms"],
         "ablation_floor_no_fetch_speedup": prod_ms / launches["no_fetch"]["median_ms"],

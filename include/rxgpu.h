@@ -546,7 +546,8 @@ void rxgpu_last_search_stats(rxgpu_search_stats* out);
 /* large query batches: int8 tensor-core filter (exact integer dot products of per-row scaled codes, certified by per-row
  * residual norms) + exact fp32 re-rank (results identical to the exact scan).
  * mode 0 = automatic (batches >= 64 queries on >= 100k rows, k <= 1023), 1 = whenever possible, 2 = never;
- * 3 / 4 = as 1 with single CTAs (the default) / clusters of up to two CTAs sharing every row tile; all give the same bits. */
+ * 3 / 4 / 5 = as 1 with single CTAs / clusters of up to two / clusters of up to four CTAs sharing every row tile (TMA multicast);
+ * 0 and 1 take clusters of up to two on indexes of >= 2^23 rows and single CTAs below; all give the same bits. */
 int rxgpu_set_tensor_core_filter(rxgpu_index*, int mode);
 /* process-wide switch: bracket every scan-kernel launch with CUDA events (used by bench.py for the roofline figure) */
 int rxgpu_set_profile(int on);
@@ -554,7 +555,7 @@ int rxgpu_set_profile(int on);
  * (1 = per-phase clock stamps, 2 = rare path compiled out, 3 = producers not fetching, 4 = block test and rare path compiled out;
  * 0 = the production kernel again) and adds its counters to the zeroed device buffer d_counters (knn_tc.cuh: kTcDiag*).  Modes 2
  * to 4 return meaningless results; only query
- * blocks of 128 and single CTAs are served.  A mode other than 0 is refused (RXGPU_ERR_LOGIC) unless the environment has
+ * blocks of 128 are served, in the cluster shape the index's rxgpu_set_tensor_core_filter mode picks.  A mode other than 0 is refused (RXGPU_ERR_LOGIC) unless the environment has
  * RXGPU_TC_DIAG=1, and a search a diagnostic instantiation answered reports tc_kernel = 1 + mode in its statistics. */
 int rxgpu_tc_diag(int mode, void* d_counters);
 

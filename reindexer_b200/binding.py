@@ -594,7 +594,8 @@ class GpuBruteforceSearch:
         _check(self._lib.rxgpu_set_query_tile(self._h, qt))
 
     def set_tensor_core_filter(self, mode: int):
-        """0 = auto, 1 = whenever possible, 2 = never (exact fp32 scan only)"""
+        """0 = auto, 1 = whenever possible, 2 = never (exact fp32 scan only); 3 / 4 / 5 = as 1 in single CTAs / clusters of up to
+        two / clusters of up to four CTAs that share every row tile (0 and 1: clusters of up to two on >= 2^23 rows)"""
         _check(self._lib.rxgpu_set_tensor_core_filter(self._h, mode))
 
 

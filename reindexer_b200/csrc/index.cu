@@ -267,22 +267,27 @@ constexpr uint32_t kStageCapPerK1 = 64;
 uint32_t stageSeedRows(uint32_t k1) { return kStageSeedPerK1 * k1; }
 uint32_t stageCandCap(uint32_t k1) { return std::min<uint32_t>(1u << 18, std::max<uint32_t>(4096u, kStageCapPerK1 * k1)); }
 
-// knn_tc_filter<query block, cluster size>: one instantiation per wgmma N and per cluster shape
+// knn_tc_filter<query block, cluster size>: one instantiation per wgmma N and per cluster shape (C = 1, 2, 4)
 using TcKernel = void (*)(const CUtensorMap, const TcArgs);
+int tcClusterIndex(uint32_t cluster) { return cluster == 4 ? 2 : cluster == 2 ? 1 : 0; }
 TcKernel tcKernel(uint32_t nqb, uint32_t cluster) {
-	static const TcKernel table[4][2] = {{knn_tc_filter<32, 1>, knn_tc_filter<32, 2>},
-										 {knn_tc_filter<64, 1>, knn_tc_filter<64, 2>},
-										 {knn_tc_filter<96, 1>, knn_tc_filter<96, 2>},
-										 {knn_tc_filter<128, 1>, knn_tc_filter<128, 2>}};
-	return table[nqb / 32 - 1][cluster == 2 ? 1 : 0];
+	static const TcKernel table[4][3] = {{knn_tc_filter<32, 1>, knn_tc_filter<32, 2>, knn_tc_filter<32, 4>},
+										 {knn_tc_filter<64, 1>, knn_tc_filter<64, 2>, knn_tc_filter<64, 4>},
+										 {knn_tc_filter<96, 1>, knn_tc_filter<96, 2>, knn_tc_filter<96, 4>},
+										 {knn_tc_filter<128, 1>, knn_tc_filter<128, 2>, knn_tc_filter<128, 4>}};
+	return table[nqb / 32 - 1][tcClusterIndex(cluster)];
 }
 // rxgpu_tc_diag: the diagnostic instantiation every filter launch of this process takes instead (0 = none), and its counters
 std::atomic<int> g_tc_diag{0};
 unsigned long long* g_tc_diag_buf = nullptr;
-TcKernel tcDiagKernel(int mode) {
-	static const TcKernel table[4] = {knn_tc_filter<128, 1, kTcDiagStamps>, knn_tc_filter<128, 1, kTcDiagNoRare>,
-									  knn_tc_filter<128, 1, kTcDiagNoFetch>, knn_tc_filter<128, 1, kTcDiagNoTest>};
+template <int kCluster>
+TcKernel tcDiagKernelC(int mode) {
+	static const TcKernel table[4] = {knn_tc_filter<128, kCluster, kTcDiagStamps>, knn_tc_filter<128, kCluster, kTcDiagNoRare>,
+									  knn_tc_filter<128, kCluster, kTcDiagNoFetch>, knn_tc_filter<128, kCluster, kTcDiagNoTest>};
 	return table[mode - 1];
+}
+TcKernel tcDiagKernel(int mode, uint32_t cluster) {
+	return cluster == 4 ? tcDiagKernelC<4>(mode) : cluster == 2 ? tcDiagKernelC<2>(mode) : tcDiagKernelC<1>(mode);
 }
 
 uint32_t tcQueryBlock(uint32_t nq, uint32_t kchunks) {
@@ -360,6 +365,26 @@ int ensureShadow(const rxgpu_index* ix, cudaStream_t st) {
 	return 0;
 }
 
+// Cluster shape by default (rxgpu_set_tensor_core_filter modes 0 and 1), measured on an H100 80GB HBM3 (700 W limit) at config 1
+// (DESIGN 3.2): clusters of up to two, 69.0-69.5 k queries/s against 65.9-66.1 k with single CTAs and 65.5-66.1 k with clusters of
+// four (30 clusters of four are resident: 120 CTAs instead of 128).  Multicast halves the row bytes the SMs read from L2, but a
+// cluster waits for its slowest CTA; that pays only on long walks: at 2^22 rows the launch took 5.76 ms in clusters of two against
+// 5.67 ms in single CTAs, so indexes below kTcClusterMinRows rows keep single CTAs.
+constexpr uint32_t kTcClusterDefault = 2;
+constexpr uint64_t kTcClusterMinRows = 1u << 23;
+// The cluster size of a batch of nblocks query blocks: a cluster owns C consecutive blocks, and a block count that is not a multiple
+// of C is padded with blocks of no valid queries, which walk every row for nothing.  The largest C <= cmax whose padding is at most
+// one block, and fewer blocks than the batch has (one block is never paired with a padding block).
+uint32_t tcClusterSize(uint32_t nblocks, uint32_t ntiles, uint32_t cmax) {
+	for (uint32_t c = cmax; c > 1; c /= 2) {
+		const uint32_t pad = (c - nblocks % c) % c;
+		if (ntiles >= 2 && pad <= 1 && pad < nblocks) {
+			return c;
+		}
+	}
+	return 1;
+}
+
 // One batch of queries on the candidate filter: the int8 query codes and their tensor map, prepared once, and the launch shape.
 struct TcBatch {
 	uint32_t nq, nqb, cluster, ngroups, nqPad, kchunks, stages, queueSlots;
@@ -377,12 +402,10 @@ int tcPrepare(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float
 	const uint32_t pitchQ = ix->pitch_q, kchunks = pitchQ / kTcChunkK;
 	const uint32_t nqb = tcQueryBlock(nq, kchunks);
 	const uint32_t ntiles = uint32_t((ix->size + kTcTileRows - 1) / kTcTileRows);
-	// single CTAs by default: measured on an H100 80GB HBM3 (400 W limit) at config 1, 34.8 k queries/s against 19.9 k with clusters of
-	// two -- a multicast stage waits for the slowest consumer of the cluster, while CTAs that share row tiles through L2 never wait
-	const uint32_t clusterMax = ix->tc_cluster_max ? ix->tc_cluster_max : 1u;
-	// a cluster of two owns two consecutive query blocks; an odd block count is padded with a block of no valid queries
-	const uint32_t cluster = clusterMax >= 2 && nq > nqb && ntiles >= 2 ? 2u : 1u;
-	const uint32_t ngroups = ((nq + nqb - 1) / nqb + cluster - 1) / cluster;
+	const uint32_t nblocks = (nq + nqb - 1) / nqb;
+	const uint32_t cmax = ix->tc_cluster_max ? ix->tc_cluster_max : ix->size >= kTcClusterMinRows ? kTcClusterDefault : 1u;
+	const uint32_t cluster = tcClusterSize(nblocks, ntiles, cmax);
+	const uint32_t ngroups = (nblocks + cluster - 1) / cluster;
 	const uint32_t nqPad = ngroups * cluster * nqb;
 	RX_CUDA(ws.d_qcodes.ensure(size_t(nqPad) * pitchQ));
 	RX_CUDA(ws.d_qc.ensure(nqPad));
@@ -407,10 +430,10 @@ int tcPrepare(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float
 	}
 	b.diag = g_tc_diag.load();
 	if (const int diag = b.diag) {
-		if (nqb != 128 || cluster != 1) {
-			return fail(RXGPU_ERR_PARAMS, "rxgpu: the diagnostic filter instantiations take query blocks of 128 and single CTAs");
+		if (nqb != 128) {
+			return fail(RXGPU_ERR_PARAMS, "rxgpu: the diagnostic filter instantiations take query blocks of 128");
 		}
-		b.kfn = tcDiagKernel(diag);
+		b.kfn = tcDiagKernel(diag, cluster);
 	}
 	RX_CUDA(raiseSmemCeilingOnce(b.kfn, ix->device, int(kTcSmemLimit)));
 	cudaLaunchConfig_t cfg{};
@@ -1218,11 +1241,11 @@ int rxgpu_set_query_tile(rxgpu_index* ix, uint32_t qt) {
 	return 0;
 }
 int rxgpu_set_tensor_core_filter(rxgpu_index* ix, int mode) {
-	if (!ix || mode < 0 || mode > 4) {
-		return fail(RXGPU_ERR_PARAMS, "rxgpu: tensor-core filter mode must be 0..4");
+	if (!ix || mode < 0 || mode > 5) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: tensor-core filter mode must be 0..5");
 	}
 	ix->tc_mode = uint32_t(mode >= 3 ? 1 : mode);
-	ix->tc_cluster_max = mode == 4 ? 2u : 0u;
+	ix->tc_cluster_max = mode == 3 ? 1u : mode == 4 ? 2u : mode == 5 ? 4u : 0u;
 	return 0;
 }
 int rxgpu_tc_diag(int mode, void* d_counters) {

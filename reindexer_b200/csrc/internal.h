@@ -239,7 +239,7 @@ struct rxgpu_index {
 		}
 	}
 	uint32_t tc_mode = 0;  // 0 auto, 1 force on, 2 off
-	uint32_t tc_cluster_max = 0;  // 0 = up to 4 CTAs per cluster
+	uint32_t tc_cluster_max = 0;  // most CTAs per cluster (1, 2 or 4); 0 = the default shape (index.cu: kTcClusterDefault)
 
 	~rxgpu_index() {
 		cudaSetDevice(device);

@@ -36,9 +36,10 @@
 //                 the exact range scan.  Certification needs no upper bound here, only that lb never exceeds d.
 //
 // Launch shape: one grid covers G query groups (a group = one query block of NQ queries per CTA of a cluster) with W tile walkers
-// each, G x W <= the clusters resident at once (config 1: 8 blocks x 16 walkers = 128 CTAs, one launch per batch).  Walker w visits
-// the 128-row tiles w, w + W, w + 2W, ..., so every tile is visited once per query, and the G CTAs of one walker request the same
-// tiles at about the same time: the first read misses to HBM, the others hit L2, and nothing makes one CTA wait for another.
+// each, G x W <= the clusters resident at once (config 1, clusters of two: 4 groups x 16 walkers x 2 = 128 CTAs, one launch per
+// batch).  Walker w visits the 128-row tiles w, w + W, w + 2W, ..., so every tile is visited once per query, and the G clusters of
+// one walker request the same tiles at about the same time: the first read misses to HBM, the others hit L2, and nothing makes one
+// cluster wait for another.
 //
 // Roles (512 threads = four warpgroups, 1 CTA per SM, persistent over 128-row tiles; every thread gets 128 registers, which the
 // consumers' int32 accumulators and block test fit; ptxas ignores a setmaxnreg split of 80 for warpgroup 0 and 144 for the
@@ -47,9 +48,9 @@
 //                in BLOCK ORDER (below), one K chunk (64 rows x 128 codes = 8 KB) per stage, through ONE RING of up to kTcStages
 //                stages shared by all consumers.  The shadow is stored TILED and PRE-SWIZZLED in HBM ([64-row block][K chunk]
 //                [64 x 128 B in the SWIZZLE_128B pattern]) so a stage is one contiguous 8 KB cp.async.bulk copy (row-major fp32
-//                stays the source of truth; the shadow is private, derived).  In a cluster of two CTAs (optional; single CTAs are
-//                faster on the H100) each CTA fetches half of every stage and multicasts it to both, which own consecutive query
-//                blocks.
+//                stays the source of truth; the shadow is private, derived).  In a cluster of C = 2 or 4 CTAs, which own C
+//                consecutive query blocks, each CTA fetches 1/C of every stage and multicasts it to all C, so the cluster reads
+//                each row byte from L2 once instead of C times.
 //   warps 1-3    bookkeepers: warp 1 + w serves the candidate queue of consumer warpgroup w (below): the row's own bound, the
 //                append to the per-query candidate lists in HBM, the bound list and tau, off the MMA path.
 //   warpgroups 1-3   consumers: a walker's 64-row blocks form one sequence i = 0, 1, 2, ..., block i being half i % 2 of the tile
@@ -180,11 +181,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 		"r"(parity)
 		: "memory");
 }
-// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster (the CTA itself included)
+// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster (the CTA itself included).  The default
+// (CTA-scope) semantics: a consumer signals with it that its wgmma reads of a stage retired, and nothing it wrote has to become
+// visible to the peer.  A cluster-scope release made every arrival wait for this thread's outstanding memory operations
+// (DESIGN 3.2: 3.7x / 6.7x slower launches in clusters of two / four, the MMA-only floor included).
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
 	uint32_t remote;
 	asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-	asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+	asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int32_t x, int32_t y) {
 	asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
@@ -605,8 +609,7 @@ template <int kNq, int kCluster, int kDiag = 0>
 __global__ void __launch_bounds__(kTcThreads, 1)
 	knn_tc_filter(const __grid_constant__ CUtensorMap map_queries, const __grid_constant__ TcArgs a) {
 	static_assert(kNq % 32 == 0 && kNq <= int(kTcMaxNq), "query block");
-	static_assert(kCluster == 1 || kCluster == 2, "a stage is split in 1 or 2 equal copies");
-	static_assert(kDiag == 0 || kCluster == 1, "the diagnostic instantiations are single CTAs");
+	static_assert(kCluster == 1 || kCluster == 2 || kCluster == 4, "a stage is split in 1, 2 or 4 equal copies");
 	constexpr bool kStamp = kDiag == kTcDiagStamps;
 	auto clk = [] {  // 0 outside the stamped instantiation, where every stamp and sum below folds away
 		if constexpr (kStamp) {
@@ -763,13 +766,13 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		unsigned int tau_ahead = my_q < nq_valid ? a.tau[q0 + my_q] : 0u;
 		const bool l2 = a.metric == kL2;
 		const float ka = (1.f + 0x1p-7f) * s_ab[0], kb = (1.f + 0x1p-7f) * s_ab[1];  // 2^-8 of e, and 2^-8 for the rounding of M_v
-		auto release = [&](uint32_t st) {  // this warp is done with stage st in every CTA that reads it
+		auto release = [&](uint32_t st) {  // this warp is done with stage st in every CTA that reads it: lane c signals CTA c
 			if constexpr (kCluster == 1) {
-				mbar_arrive(&empty[st]);
-			} else {
-				for (uint32_t c = 0; c < uint32_t(kCluster); ++c) {
-					mbar_arrive_cluster(&empty[st], c);
+				if (lane == 0) {
+					mbar_arrive(&empty[st]);
 				}
+			} else if (lane < kCluster) {
+				mbar_arrive_cluster(&empty[st], uint32_t(lane));
 			}
 		};
 		mbar_wait(q_bar, 0);
@@ -815,9 +818,15 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 			// over the global chunk index g = blk kchunks + kc every chunk below g is issued; the stage chunk g needs was then released
 			// (chunk g - stages is released when chunk g - stages + 1 of the same block is issued, or by the drain of a block's last
 			// chunk, which waits on nothing), so chunk g arrives, and its owner's turn came with the last chunk of block blk - 1.  The
-			// producer and the bookkeepers never wait on a turn.  In a cluster of two both CTAs walk the same blocks in the same order
-			// with the same owners, and the induction runs over the chunks of both: a stage goes back to a producer once the owning
-			// warpgroup of every CTA released it.
+			// producer and the bookkeepers never wait on a turn.  In a cluster of C CTAs all of them walk the same blocks in the same
+			// order with the same owners, the turns and the bookkeepers stay per CTA, and the induction runs over the chunks of all C:
+			// if every chunk below g is issued in every CTA, then chunk g - stages was released in every CTA (its owner releases it
+			// in all C CTAs -- lane c of each of its four warps arrives on `empty` of CTA c, 4 C arrivals per phase -- once its own
+			// MMAs on it retired), so every producer's wait on that stage's `empty` completes and each issues its 1/C of chunk g into
+			// all C CTAs; `full` of chunk g then completes in every CTA (one local expect_tx arrival, C parts of complete_tx, some of
+			// which may land before the expect_tx: the transaction count may go transiently negative), and each owner's turn came
+			// as in one CTA.  A peer that is ahead waits only on barriers our side will arrive on; no CTA leaves before the exit
+			// cluster sync, so no multicast or remote arrival targets a CTA that has exited.
 			const uint32_t g0 = blk * a.kchunks;
 			uint32_t stage = g0 % nstages, phase = (g0 / nstages) & 1u;
 			[[maybe_unused]] const long long c_turn = clk();
@@ -844,9 +853,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 				wgmma_commit();
 				if (kc > 0) {  // the previous chunk's MMAs have retired: its stage goes back to the producer
 					wgmma_wait<1>();
-					if (lane == 0) {
-						release(prev);
-					}
+					release(prev);
 				}
 				prev = stage;
 				if (++stage == nstages) {
@@ -860,9 +867,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 			}
 			s1 = clk();
 			wgmma_wait<0>();
-			if (lane == 0) {
-				release(prev);
-			}
+			release(prev);
 			s2 = clk();
 			asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // the refreshed (P, R) of all queries are visible
 			s3 = clk();
