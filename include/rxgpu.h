@@ -336,7 +336,8 @@ int rxgpu_hnsw_search_knn_sq8(const rxgpu_index*, uint32_t nq, const float* quer
  * probed lists with the exact-scan kernel (fused top-k per list) + one merge.  Cosine: queries pre-normalised, rows and centroids
  * carry their norm coefficients like the reference's patched FAISS (IndexFlatCosine, IndexIVFFlat(..., is_cosine)).
  * Results best-first in map space (L2: squared distance; IP / Cosine: -inner product / -cos), bit-equal distances ordered by label;
- * out_count[q] = min(k, rows in the probed lists).  k <= 256, nprobe <= 1024, at most 16384 centroids. */
+ * out_count[q] = min(k, rows in the probed lists).  k <= 256, nprobe <= 1024, at most 131072 centroids (the reference's bound;
+ * 131073 and more: errParams), dim <= 51200 (the coarse pass stages a query in shared memory). */
 int rxgpu_ivf_import(rxgpu_index*, uint32_t nlist, const float* centroids /* nlist x dim, host */, const uint64_t* list_sizes /* nlist */);
 int rxgpu_ivf_search_knn(const rxgpu_index*, uint32_t nq, const float* queries /* host */, uint32_t k, uint32_t nprobe, float* out_dist,
 						 uint64_t* out_label, uint32_t* out_count);

@@ -6,6 +6,7 @@
 
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_segmented_radix_sort.cuh>
+#include <cub/device/device_segmented_sort.cuh>
 
 #include <algorithm>
 #include <atomic>
@@ -28,6 +29,7 @@
 #include "knn_tc.cuh"
 #include "ivf_select.cuh"
 #include "ivf_range.cuh"
+#include "ivf_coarse.cuh"
 
 using namespace rxgpu;
 
@@ -1949,33 +1951,74 @@ void ivfRelease(rxgpu_ivf_device* p) { delete p; }
 }  // namespace rxgpu
 
 namespace {
-size_t ivfCoarseSmem(const rxgpu_index* ix, const rxgpu_ivf_device* h) { return size_t((ix->dim + 127u) / 128u) * 512 + size_t(h->nlist) * 8; }
-int ivfCheckCoarseSmem(const rxgpu_index* ix, const rxgpu_ivf_device* h) {
-	if (ivfCoarseSmem(ix, h) > 200 * 1024) {
-		return fail(RXGPU_ERR_PARAMS, "rxgpu: dimension / centroid count exceeds the coarse quantiser's shared memory");
+// the coarse pass stages one query (at least) in shared memory: dim <= 51 200
+int ivfCheckCoarseSmem(const rxgpu_index* ix) {
+	if (coarse_smem_bytes(1, ix->dim) > kCoarseSmemMax) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: dimension exceeds the coarse quantiser's shared memory");
 	}
 	return 0;
 }
-// the coarse quantiser over the nq queries in h->d_q: work items of the list scans in h->d_work, probe-major
-int ivfLaunchCoarse(const rxgpu_index* ix, rxgpu_ivf_device* h, uint32_t nq, uint32_t nprobe, cudaStream_t st) {
-	const size_t coarseSmem = ivfCoarseSmem(ix, h);
-	if (ix->metric == RXGPU_L2) {
-		RX_CUDA(raiseSmemCeilingOnce(ivf_coarse_kernel<true>, ix->device, 200 * 1024));
-		ivf_coarse_kernel<true><<<nq, kScanThreads, coarseSmem, st>>>(h->centroids.p, ix->pitch, ix->dim, h->nlist, h->d_q.p, nq, nprobe,
-																	   h->list_begin.p, h->own ? h->list_end.p : nullptr, nullptr, h->d_work.p);
-	} else {
-		RX_CUDA(raiseSmemCeilingOnce(ivf_coarse_kernel<false>, ix->device, 200 * 1024));
-		ivf_coarse_kernel<false><<<nq, kScanThreads, coarseSmem, st>>>(h->centroids.p, ix->pitch, ix->dim, h->nlist, h->d_q.p, nq, nprobe,
-																		h->list_begin.p, h->own ? h->list_end.p : nullptr,
-																		ix->metric == RXGPU_COS ? h->cnorm.p : nullptr, h->d_work.p);
+template <bool kIsL2, int QT>
+cudaError_t launchCoarseDist(const rxgpu_index* ix, rxgpu_ivf_device* h, dim3 grid, size_t smem, const float* queries, uint32_t cq,
+							 const float* cnorm, cudaStream_t st) {
+	if (cudaError_t e = raiseSmemCeilingOnce(ivf_coarse_dist_kernel<kIsL2, QT>, ix->device, int(kCoarseSmemMax))) {
+		return e;
 	}
-	RX_CUDA(cudaGetLastError());
+	ivf_coarse_dist_kernel<kIsL2, QT><<<grid, kScanThreads, smem, st>>>(h->centroids.p, ix->pitch, ix->dim, h->nlist, queries, cq, cnorm,
+																		 h->d_keys.p);
+	return cudaGetLastError();
+}
+// the coarse quantiser over the nq queries in h->d_q (ivf_coarse.cuh): work items of the list scans in h->d_work, probe-major.  Per
+// query chunk of at most kIvfKeyCap keys: distances, select, sort, emit (4 launches, counted in g_stats with the centroid bytes, read
+// once per query tile).  The chunk's keys go to h->d_keys, its survivors to h->d_sel_label: the key pass and the selects that follow
+// reuse them.  A batch stages kCoarseTile queries per tile (dim <= 3 200), one query stages itself alone.
+int ivfLaunchCoarse(const rxgpu_index* ix, rxgpu_ivf_device* h, uint32_t nq, uint32_t nprobe, cudaStream_t st) {
+	const uint32_t nlist = h->nlist;
+	const int qt = nq > 1 && coarse_smem_bytes(kCoarseTile, ix->dim) <= kCoarseSmemMax ? kCoarseTile : 1;
+	const size_t smem = coarse_smem_bytes(qt, ix->dim);
+	const uint32_t chunk = uint32_t(std::max<uint64_t>(1, kIvfKeyCap / nlist));
+	const uint32_t cqMax = std::min(nq, chunk);
+	RX_CUDA(h->d_keys.ensure(size_t(cqMax) * nlist));
+	RX_CUDA(h->d_sel_label.ensure(size_t(cqMax) * nprobe));
+	RX_CUDA(h->d_seg_begin.ensure(cqMax));
+	RX_CUDA(h->d_seg_end.ensure(cqMax));
+	const float* cnorm = ix->metric == RXGPU_COS ? h->cnorm.p : nullptr;
+	const uint32_t groups = (nlist + kCoarseRows - 1) / kCoarseRows;
+	for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
+		const uint32_t cq = std::min(chunk, nq - q0);
+		const uint32_t tiles = (cq + qt - 1) / qt;
+		// query tiles fastest: the CTAs in flight share centroid slices through L2; about 4 CTAs per SM over the whole grid
+		const uint32_t slices = std::max(1u, std::min((groups + kScanWarps - 1) / kScanWarps, (uint32_t(ix->sm_count) * 4 + tiles - 1) / tiles));
+		const dim3 grid(tiles, slices);
+		const float* qs = h->d_q.p + size_t(q0) * ix->dim;
+		if (ix->metric == RXGPU_L2) {
+			RX_CUDA(qt == 1 ? (launchCoarseDist<true, 1>(ix, h, grid, smem, qs, cq, cnorm, st))
+							: (launchCoarseDist<true, kCoarseTile>(ix, h, grid, smem, qs, cq, cnorm, st)));
+		} else {
+			RX_CUDA(qt == 1 ? (launchCoarseDist<false, 1>(ix, h, grid, smem, qs, cq, cnorm, st))
+							: (launchCoarseDist<false, kCoarseTile>(ix, h, grid, smem, qs, cq, cnorm, st)));
+		}
+		ivf_coarse_select_kernel<<<cq, kIvfSelThreads, 0, st>>>(h->d_keys.p, nlist, nprobe, h->d_sel_label.p, h->d_seg_begin.p, h->d_seg_end.p);
+		RX_CUDA(cudaGetLastError());
+		// the keys are spent once the survivors are out: they are the sort's second buffer
+		cub::DoubleBuffer<uint64_t> sorted(h->d_sel_label.p, h->d_keys.p);
+		const int n = int(size_t(cq) * nprobe);
+		size_t sortBytes = 0;
+		RX_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, sortBytes, sorted, n, int(cq), h->d_seg_begin.p, h->d_seg_end.p, st));
+		RX_CUDA(h->d_cub.ensure(sortBytes));
+		RX_CUDA(cub::DeviceSegmentedSort::SortKeys(h->d_cub.p, sortBytes, sorted, n, int(cq), h->d_seg_begin.p, h->d_seg_end.p, st));
+		ivf_coarse_emit_kernel<<<unsigned((size_t(n) + 255) / 256), 256, 0, st>>>(sorted.Current(), nq, nprobe, q0, cq, h->list_begin.p,
+																				  h->own ? h->list_end.p : nullptr, h->d_work.p);
+		RX_CUDA(cudaGetLastError());
+		g_stats.launches += 4;
+		g_stats.algorithmic_bytes += uint64_t(tiles) * nlist * ix->dim * 4;
+	}
 	return 0;
 }
 
 // the prologue of the key pass (rxgpu_ivf_search_knn_large_k, rxgpu_ivf_search_range_batch), under h->mtx: the coarse quantiser over
 // the nq queries, probed rows per query (h->d_qrows, and rows on the host) and their exclusive scan, each query's first key
-// (h->d_qoff; off[q] on the host, off[nq] = all probed rows).  3 launches.
+// (h->d_qoff; off[q] on the host, off[nq] = all probed rows).  2 launches after the coarse pass's.
 int ivfProbedRows(const rxgpu_index* ix, rxgpu_ivf_device* h, uint32_t nq, const float* queries, uint32_t nprobe, cudaStream_t st,
 				  std::vector<uint64_t>& rows, std::vector<uint64_t>& off) {
 	RX_CUDA(h->d_q.ensure(size_t(nq) * ix->dim));
@@ -2064,8 +2107,8 @@ int rxgpu_ivf_import(rxgpu_index* ix, uint32_t nlist, const float* centroids, co
 	if (!centroids || !list_sizes || nlist == 0) {
 		return fail(RXGPU_ERR_PARAMS, "rxgpu: null argument");
 	}
-	if (nlist > 16384) {
-		return fail(RXGPU_ERR_PARAMS, "rxgpu: at most 16384 IVF centroids on the device path");
+	if (nlist > kIvfMaxCentroids) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: at most 131072 IVF centroids (the reference's centroids_count bound)");
 	}
 	try {
 		std::vector<uint32_t> begin(size_t(nlist) + 1, 0u);
@@ -2133,7 +2176,7 @@ int rxgpu_ivf_search_knn(const rxgpu_index* ix, uint32_t nq, const float* querie
 	if (nprobe > 256u * kMergeOwn) {
 		return fail(RXGPU_ERR_PARAMS, "rxgpu: nprobe exceeds the merge fan-in (1024)");
 	}
-	if (int rc = ivfCheckCoarseSmem(ix, h)) {
+	if (int rc = ivfCheckCoarseSmem(ix)) {
 		return rc;
 	}
 	std::lock_guard<std::mutex> lck(h->mtx);
@@ -2184,7 +2227,7 @@ int rxgpu_ivf_search_knn(const rxgpu_index* ix, uint32_t nq, const float* querie
 	m.mode = kModeTopK;
 	knn_merge_lists<<<nq, 256, 0, st>>>(m);
 	RX_CUDA(cudaGetLastError());
-	g_stats.launches = 3;
+	g_stats.launches += 2;  // list scans, merge (the coarse pass counts its own)
 	g_stats.passes = 1;
 	try {
 		std::vector<float> hd(size_t(nq) * k);
@@ -2240,12 +2283,12 @@ int rxgpu_ivf_search_knn_large_k(const rxgpu_index* ix, uint32_t nq, const float
 	if (k <= kMaxFusedK1 && nprobe <= 256u * kMergeOwn) {  // what the fused per-list top-k serves: that path, same bits
 		return rxgpu_ivf_search_knn(ix, nq, queries, k, nprobe, out_dist, out_label, out_count);
 	}
-	if (int rc = ivfCheckCoarseSmem(ix, h)) {
+	if (int rc = ivfCheckCoarseSmem(ix)) {
 		return rc;
 	}
 	std::lock_guard<std::mutex> lck(h->mtx);
 	cudaStream_t st = ix->stream;
-	uint32_t launches = 3;  // coarse quantiser, probed rows, their scan (one CUB call)
+	uint32_t launches = 2;  // probed rows, their scan (one CUB call); the coarse pass counts its own
 	try {
 		std::vector<uint64_t> rows, off;
 		if (int rc = ivfProbedRows(ix, h, nq, queries, nprobe, st, rows, off)) {
@@ -2324,10 +2367,10 @@ int rxgpu_ivf_search_knn_large_k(const rxgpu_index* ix, uint32_t nq, const float
 			}
 		}
 		const uint64_t probed = off[nq];
-		g_stats.launches = launches;
+		g_stats.launches += launches;
 		g_stats.passes = 1;
 		// rows read once; each key written once and read once by the select
-		g_stats.algorithmic_bytes = probed * ix->dim * 4 + (ix->metric == RXGPU_COS ? probed * 4 : 0) + probed * 16;
+		g_stats.algorithmic_bytes += probed * ix->dim * 4 + (ix->metric == RXGPU_COS ? probed * 4 : 0) + probed * 16;
 	} catch (const std::bad_alloc&) {
 		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
 	}
@@ -2352,7 +2395,7 @@ int rxgpu_ivf_search_range(const rxgpu_index* ix, const float* query, float radi
 		return fail(RXGPU_ERR_LOGIC, "rxgpu: the index changed after the IVF lists were imported");
 	}
 	nprobe = std::max(1u, std::min(nprobe, h->nlist));
-	if (int rc = ivfCheckCoarseSmem(ix, h)) {
+	if (int rc = ivfCheckCoarseSmem(ix)) {
 		return rc;
 	}
 	std::lock_guard<std::mutex> lck(h->mtx);
@@ -2364,7 +2407,6 @@ int rxgpu_ivf_search_range(const rxgpu_index* ix, const float* query, float radi
 	if (int rc = ivfLaunchCoarse(ix, h, 1, nprobe, st)) {
 		return rc;
 	}
-	g_stats.launches = 1;
 	uint64_t cap = std::max<uint64_t>(h->d_range.n, 1u << 14);
 	unsigned long long total = 0;
 	for (;;) {  // like the brute-force range search: grow the result buffer and rescan when it was too small
@@ -2438,12 +2480,12 @@ int rxgpu_ivf_search_range_batch(const rxgpu_index* ix, uint32_t nq, const float
 		return fail(RXGPU_ERR_LOGIC, "rxgpu: the index changed after the IVF lists were imported");
 	}
 	nprobe = std::max(1u, std::min(nprobe, h->nlist));
-	if (int rc = ivfCheckCoarseSmem(ix, h)) {
+	if (int rc = ivfCheckCoarseSmem(ix)) {
 		return rc;
 	}
 	std::lock_guard<std::mutex> lck(h->mtx);
 	cudaStream_t st = ix->stream;
-	uint32_t launches = 3;  // coarse quantiser, probed rows, their scan
+	uint32_t launches = 2;  // probed rows, their scan; the coarse pass counts its own
 	try {
 		std::vector<uint64_t> rows, off;
 		if (int rc = ivfProbedRows(ix, h, nq, queries, nprobe, st, rows, off)) {
@@ -2554,10 +2596,10 @@ int rxgpu_ivf_search_range_batch(const rxgpu_index* ix, uint32_t nq, const float
 			}
 		}
 		const uint64_t probed = off[nq];
-		g_stats.launches = launches;
+		g_stats.launches += launches;
 		g_stats.passes = 1;
 		// as rxgpu_ivf_search_knn_large_k: rows read once; each key written once and read once
-		g_stats.algorithmic_bytes = probed * ix->dim * 4 + (ix->metric == RXGPU_COS ? probed * 4 : 0) + probed * 16;
+		g_stats.algorithmic_bytes += probed * ix->dim * 4 + (ix->metric == RXGPU_COS ? probed * 4 : 0) + probed * 16;
 	} catch (const std::bad_alloc&) {
 		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
 	}

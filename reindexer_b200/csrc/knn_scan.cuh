@@ -450,7 +450,7 @@ __global__ void __launch_bounds__(256) knn_merge_lists(const MergeArgs a) {
 }
 
 // ---- one exact distance outside the scan ------------------------------------------------------------------------------------
-// The per-row arithmetic of knn_scan_warp for every other exact fp32 distance (knn_rerank, the IVF coarse quantiser, the int8
+// The per-row arithmetic of knn_scan_warp for every other exact fp32 distance (knn_rerank, the IVF coarse pass, the int8
 // filter's seed and its bookkeepers): lane l accumulates float4 #l of every 128-float chunk, chunk after chunk, with sequential FMAs
 // (x, y, z, w); an xor butterfly adds the lanes; then the sign (inner product, cosine) and the row's Cosine norm coefficient
 // (norm_coefs != nullptr).  So a row's distance has the same bits on every path: the tie rule needs that, and the filter's bound list
@@ -525,73 +525,6 @@ __device__ __forceinline__ float row_dist_warp(const float4* rows4, uint32_t pit
 	float d[1][1];
 	row_dists_warp<kIsL2, 1, 1>(rows4, pitch4, nch, r, q, norm_coefs, lane, d);
 	return d[0][0];
-}
-
-// ---- IVF ----------------------------------------------------------------------------------------------------------------
-// coarse quantiser (faiss::IndexIVF::search -> quantizer->search(nprobe), IndexIVF.cpp): one CTA per query computes the distance to
-// every centroid (a warp per centroid) and selects the nprobe nearest under (distance, centroid id); then it emits the work items
-// of the list scan, probe-major: work[p * nq + q] = (q, list_begin[c], list_begin[c + 1], c)
-template <bool kIsL2>
-__global__ void __launch_bounds__(kScanThreads) ivf_coarse_kernel(const float* centroids, uint32_t pitch, uint32_t dim, uint32_t nlist,
-																  const float* queries, uint32_t nq, uint32_t nprobe, const uint32_t* list_begin, const uint32_t* list_end,
-																  const float* centroid_norm_coefs, uint4* work) {
-	extern __shared__ __align__(16) unsigned char smem_raw[];
-	__shared__ uint64_t s_best[kScanWarps];
-	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-	const uint32_t nch = (dim + 127u) / 128u, dp4 = nch * 32u, pitch4 = pitch >> 2;
-	float4* sq4 = reinterpret_cast<float4*>(smem_raw);
-	uint64_t* keys = reinterpret_cast<uint64_t*>(smem_raw + size_t(dp4) * 16);
-	const uint32_t q = blockIdx.x;
-	{
-		float* sq = reinterpret_cast<float*>(sq4);
-		for (uint32_t c = threadIdx.x; c < dp4 * 4; c += blockDim.x) {
-			sq[c] = c < dim ? queries[size_t(q) * dim + c] : 0.f;
-		}
-	}
-	__syncthreads();
-	const float4* rows4 = reinterpret_cast<const float4*>(centroids);
-	for (uint32_t c = warp; c < nlist; c += kScanWarps) {
-		// IndexFlatCosine: knn_cosine = IP * norm coefficient of the centroid
-		const float d = row_dist_warp<kIsL2>(rows4, pitch4, nch, c, sq4, centroid_norm_coefs, lane);
-		if (lane == 0) {
-			keys[c] = make_key(d, c);
-		}
-	}
-	__syncthreads();
-	uint64_t last = 0;
-	for (uint32_t p = 0; p < nprobe; ++p) {  // keys are unique: select strictly increasing keys
-		uint64_t best = kKeyNone;
-		for (uint32_t c = threadIdx.x; c < nlist; c += blockDim.x) {
-			const uint64_t kx = keys[c];
-			if ((p == 0 || kx > last) && kx < best) {
-				best = kx;
-			}
-		}
-#pragma unroll
-		for (int off = 16; off > 0; off >>= 1) {
-			const uint64_t o = __shfl_xor_sync(0xffffffffu, best, off);
-			best = o < best ? o : best;
-		}
-		if (lane == 0) {
-			s_best[warp] = best;
-		}
-		__syncthreads();
-		best = s_best[0];
-#pragma unroll
-		for (int w = 1; w < kScanWarps; ++w) {
-			best = s_best[w] < best ? s_best[w] : best;
-		}
-		__syncthreads();
-		if (threadIdx.x == 0) {
-			uint4 w = make_uint4(q, 0, 0, 0xFFFFFFFFu);  // fewer centroids than nprobe: an empty range
-			if (best != kKeyNone) {
-				const uint32_t c = uint32_t(best);
-				w = make_uint4(q, list_begin[c], list_end ? list_end[c] : list_begin[c + 1], c);
-			}
-			work[size_t(p) * nq + q] = w;
-		}
-		last = best;
-	}
 }
 
 // ---- maintenance kernels ------------------------------------------------------------------------------------------------
