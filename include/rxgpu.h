@@ -15,7 +15,8 @@
  *  - labels are FloatVectorId::AsNumber() = rowId << 32 | arrayIdx (core/index/float_vector/float_vector_id.h:11).
  *  - threading: searches are re-entrant and may run concurrently from many host threads ("Read-only concurrency
  *    expected", hnswlib/hnswalg.h:1977); mutators are called by one thread at a time and never concurrently with
- *    searches on the same handle (the namespace lock guarantees that in the reference).
+ *    searches on the same handle (the namespace lock guarantees that in the reference).  An HNSW streaming session
+ *    is advanced by one thread at a time, though not always the same one; different sessions may run concurrently.
  *  - there is NO CPU fallback: every compute entry point fails with errSystem when no CUDA device is usable.
  */
 #ifndef RXGPU_H

@@ -1769,6 +1769,9 @@ int rxgpu_hnsw_stream_next(rxgpu_hnsw_stream* s, uint32_t batch_size, float* out
 	if (smem > 200 * 1024) {
 		return fail(RXGPU_ERR_PARAMS, "rxgpu: dimension exceeds the shared-memory budget of the streaming HNSW kernel");
 	}
+	// Sessions and the searches under h->mtx share the maintenance stream without a lock.  That is safe: the kernel reads only the
+	// graph and rows, which no search writes, and writes only this session's own buffers, and the stream synchronise below completes
+	// it before any of them is read.  Other calls' work on the stream can only delay that synchronise, never reach these buffers.
 	cudaStream_t st = ix->stream;
 	if (ix->metric == RXGPU_L2) {
 		RX_CUDA(raiseSmemCeilingOnce(hnsw_stream_kernel<true>, ix->device, 200 * 1024));

@@ -1288,6 +1288,7 @@ int rxgpu_search_knn_device(const rxgpu_index* ix, uint32_t nq, const float* d_q
 	WsLease lease(ix);
 	Workspace& ws = *lease.ws;
 	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ix->stream;
+	lease.st = st;
 	if (ix->size == 0) {
 		RX_CUDA(cudaMemsetAsync(d_out_count, 0, nq * sizeof(uint32_t), st));
 		RX_CUDA(cudaStreamSynchronize(st));
@@ -1311,6 +1312,7 @@ int rxgpu_search_tie_rows_device(const rxgpu_index* ix, const float* d_query, fl
 	}
 	WsLease lease(ix);
 	cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : ix->stream;
+	lease.st = st;
 	if (ix->size == 0) {
 		RX_CUDA(cudaMemsetAsync(d_out_count, 0, sizeof(uint32_t), st));
 		RX_CUDA(cudaStreamSynchronize(st));
@@ -1400,6 +1402,7 @@ static int searchKnnHost(const rxgpu_index* ix, uint32_t nq, const float* querie
 		RX_CUDA(cudaStreamCreateWithFlags(&ws.stream, cudaStreamNonBlocking));
 	}
 	cudaStream_t st = ws.stream;
+	lease.st = st;
 	const size_t qn = size_t(nq) * ix->dim, on = size_t(nq) * k1;
 	RX_CUDA(ws.d_queries.ensure(qn));
 	RX_CUDA(ws.h_queries.ensure(qn));
@@ -1564,6 +1567,7 @@ static int searchRangeHost(const rxgpu_index* ix, const float* query, float radi
 		RX_CUDA(cudaStreamCreateWithFlags(&ws.stream, cudaStreamNonBlocking));
 	}
 	cudaStream_t st = ws.stream;
+	lease.st = st;
 	RX_CUDA(ws.d_queries.ensure(ix->dim));
 	RX_CUDA(cudaMemcpyAsync(ws.d_queries.p, query, ix->dim * sizeof(float), cudaMemcpyHostToDevice, st));
 	if (int rc = scanRangeExact(ix, ws, st, ws.d_queries.p, radius, res)) {
@@ -1693,6 +1697,7 @@ static int searchRangeBatchHost(const rxgpu_index* ix, uint32_t nq, const float*
 		RX_CUDA(cudaStreamCreateWithFlags(&ws.stream, cudaStreamNonBlocking));
 	}
 	cudaStream_t st = ws.stream;
+	lease.st = st;
 	const size_t qn = size_t(nq) * ix->dim;
 	RX_CUDA(ws.d_queries.ensure(qn));
 	RX_CUDA(ws.h_queries.ensure(qn));

@@ -276,9 +276,14 @@ struct rxgpu_index {
 
 namespace rxgpu {
 
+// The workspace's buffers are used on whichever stream the call enqueues on (ws.stream, the caller's stream, ix->stream or a
+// communicator's), so stream order alone does not keep the next lease-holder off them.  A call that returns early after a launch (an
+// allocation or launch error) would hand back buffers a kernel may still be writing: the lease synchronises the call's stream `st`
+// before the workspace goes back to the pool.  On success the call has synchronised it already, so this waits for nothing.
 struct WsLease {
 	const rxgpu_index* idx;
 	std::unique_ptr<Workspace> ws;
+	cudaStream_t st = nullptr;  // set by the call once it has picked its stream
 	explicit WsLease(const rxgpu_index* i) : idx(i) {
 		{
 			std::lock_guard<std::mutex> lck(idx->ws_mtx);
@@ -292,6 +297,9 @@ struct WsLease {
 		}
 	}
 	~WsLease() {
+		if (st) {
+			cudaStreamSynchronize(st);
+		}
 		std::lock_guard<std::mutex> lck(idx->ws_mtx);
 		idx->ws_free.emplace_back(std::move(ws));
 	}

@@ -475,6 +475,7 @@ int rxgpu_sharded_search_knn(rxgpu_comm* c, const rxgpu_index* ix, uint32_t nq, 
 	try {
 		cudaStream_t st = c->stream;
 		WsLease lease(ix);
+		lease.st = st;
 		Workspace& ws = *lease.ws;
 		const PayloadLayout lay(nq, k1);
 		const uint32_t R = uint32_t(c->nranks);
@@ -663,6 +664,7 @@ int rxgpu_sharded_search_range_batch(rxgpu_comm* c, const rxgpu_index* ix, uint3
 				d_q = c->d_queries.p;
 			}
 			WsLease lease(ix);
+			lease.st = st;
 			const RangeEmit emit = [&](uint32_t q, const std::vector<Hit>& hits) {
 				c->h_r_n.p[q] = hits.size();
 				kept[q] = uint32_t(std::min<uint64_t>(hits.size(), max_out));
