@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Where the int8 filter launch spends its time at config 1 (10M x 768 fp32, inner product, k = 10, batch of 1024 queries).
 
-  python bench_tc_phases.py [--rows N] [--queries 1024] [--runs 5] [--cluster 1|2|4] [--out FILE]
+  python bench_tc_phases.py [--rows N] [--queries 1024] [--runs 5] [--cluster 1|2|4] [--metric ip|l2|cosine] [--out FILE]
 
 Runs the batch through the diagnostic instantiations of knn_tc_filter (knn_tc.cuh: kTcDiag*, selected with rxgpu_tc_diag; the
 searches themselves never take them) and prints one JSON line with
@@ -17,7 +17,7 @@ searches themselves never take them) and prints one JSON line with
                 (the consumers multiply zeroed stages; the barriers still cycle) and (c) the block test and the rare path compiled
                 out (ring, MMAs, turns, drain and bar.syncs kept): the MMA path's own floor.
 --cluster C runs every instantiation in clusters of C CTAs that share each row stage by TMA multicast (rxgpu_set_tensor_core_filter
-3 / 4 / 5); the default is single CTAs.  Clock stamps are cycles of the SM clock; the card, its power limit and the SM clock samples of the timed runs are in the line.
+3 / 4 / 5); the default is single CTAs.  --metric runs the same rows and queries as an L2 or a Cosine index instead.  Clock stamps are cycles of the SM clock; the card, its power limit and the SM clock samples of the timed runs are in the line.
 """
 import argparse
 import ctypes
@@ -42,6 +42,7 @@ TILE, BLOCKS, HITS, QWAIT, PER_WG = 8, 9, 10, 11, 12
 CONSUMERS = 3  # consumer warpgroups, each followed by PER_WG counters; then the producer's
 EMPTY, PROD = CONSUMERS * PER_WG, CONSUMERS * PER_WG + 1
 MODES = {"production": 0, "stamped": 1, "no_rare_path": 2, "no_fetch": 3, "mma_only": 4}
+METRICS = {"ip": ("IP", "inner product"), "l2": ("L2", "L2"), "cosine": ("COS", "cosine")}
 MAX_CTAS = 1024
 
 
@@ -51,6 +52,7 @@ def main(argv=None):
     ap.add_argument("--queries", type=int, default=1024)
     ap.add_argument("--runs", type=int, default=5)
     ap.add_argument("--cluster", type=int, default=1, choices=[1, 2, 4], help="CTAs per cluster sharing every row stage")
+    ap.add_argument("--metric", default="ip", choices=list(METRICS))
     ap.add_argument("--out", default=None, help="also write the JSON line (with the full hit histogram and marks) here")
     args = ap.parse_args(argv)
 
@@ -63,7 +65,7 @@ def main(argv=None):
     if rx.device_count() < 1:
         raise SystemExit("bench_tc_phases.py: no CUDA device -- librxgpu has no CPU fallback")
     lib = B.lib()
-    idx = rx.GpuBruteforceSearch(rx.IP, DIM, args.rows)
+    idx = rx.GpuBruteforceSearch(getattr(rx, METRICS[args.metric][0]), DIM, args.rows)
     idx.append_synth(SEED, 0, args.rows)
     idx.set_tensor_core_filter({1: 3, 2: 4, 4: 5}[args.cluster])
     queries = bench_queries(args.queries)
@@ -153,7 +155,7 @@ def main(argv=None):
     prod_ms = launches["production"]["median_ms"]
     ops = 2.0 * args.rows * DIM * args.queries
     line = {
-        "workload": f"int8 filter launch, {args.rows} x {DIM}, inner product, k = {K}, batch of {args.queries}",
+        "workload": f"int8 filter launch, {args.rows} x {DIM}, {METRICS[args.metric][1]}, k = {K}, batch of {args.queries}",
         "card": card(), "cluster": C, "grid": grid,
         "launches": launches,
         "ablation_ceiling_no_rare_path_speedup": prod_ms / launches["no_rare_path"]["median_ms"],

@@ -4,6 +4,7 @@
 // There is no CPU fallback anywhere in this file: without a usable CUDA device every compute entry point fails.
 #include <cuda_runtime.h>
 
+#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_segmented_radix_sort.cuh>
 #include <cub/device/device_segmented_sort.cuh>
@@ -322,47 +323,140 @@ bool tcEligible(const rxgpu_index* ix, uint32_t nq, uint32_t k1, int mode) {
 	return mode == kModeTopK && k1 <= kTcStagedMaxK1 && tcServes(ix, nq);
 }
 
-// int8 shadow + per-row constants, brought up to date when the rows changed since the last large-batch search
+// The shadow is rebuilt whole, sorted, once its dead and unsorted slots pass 1 / kShadowResortDiv of the slots; the slot capacity
+// leaves that much room for appended rows beyond the row capacity.
+constexpr uint32_t kShadowResortDiv = 8;
+
+void releaseShadow(const rxgpu_index* ix) {
+	cudaFree(ix->d_shadow);
+	cudaFree(ix->d_rowc);
+	cudaFree(ix->d_slot_row);
+	cudaFree(ix->d_row_slot);
+	cudaFree(ix->d_blockc);
+	ix->d_shadow = nullptr;
+	ix->d_rowc = nullptr;
+	ix->d_slot_row = nullptr;
+	ix->d_row_slot = nullptr;
+	ix->d_blockc = nullptr;
+}
+
+// The slot order of a full build: the rows sorted by tc_sort_keys (stable, so ties keep the row order), slot s = the s-th row of it
+int sortShadowSlots(const rxgpu_index* ix, cudaStream_t st, uint32_t n) {
+	uint64_t *keys = nullptr, *keys_sorted = nullptr;
+	uint32_t* vals = nullptr;
+	void* temp = nullptr;
+	size_t temp_bytes = 0;
+	const int end_bit = ix->metric == RXGPU_L2 ? 64 : 32;  // IP and Cosine keys have no bucket
+	cudaError_t e = cudaMalloc(&keys, size_t(n) * 8);
+	if (e == cudaSuccess) e = cudaMalloc(&keys_sorted, size_t(n) * 8);
+	if (e == cudaSuccess) e = cudaMalloc(&vals, size_t(n) * 4);
+	if (e == cudaSuccess) {
+		tc_sort_keys<<<unsigned((uint64_t(n) * 32 + 255) / 256), 256, 0, st>>>(ix->d_rows, ix->pitch, ix->dim, n,
+																				 ix->metric == RXGPU_COS ? ix->d_norms : nullptr, ix->metric, keys, vals);
+		e = cub::DeviceRadixSort::SortPairs(nullptr, temp_bytes, keys, keys_sorted, vals, ix->d_slot_row, n, 0, end_bit, st);
+	}
+	if (e == cudaSuccess) e = cudaMalloc(&temp, temp_bytes);
+	if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(temp, temp_bytes, keys, keys_sorted, vals, ix->d_slot_row, n, 0, end_bit, st);
+	if (e == cudaSuccess) {
+		tc_invert_slots<<<(n + 255) / 256, 256, 0, st>>>(ix->d_slot_row, n, ix->d_row_slot);
+		e = cudaGetLastError();
+	}
+	if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+	cudaFree(keys);
+	cudaFree(keys_sorted);
+	cudaFree(vals);
+	cudaFree(temp);
+	RX_CUDA(e);
+	g_stats.launches += 3;
+	return 0;
+}
+
+// int8 shadow + per-slot and per-block constants, brought up to date when the rows changed since the last large-batch search.  A full
+// build sorts the rows into slots (knn_tc.cuh: tc_block_threshold); otherwise only what the mutations since then touched: rows
+// rewritten in place are reconverted in their own slots, appended rows take new slots at the end, the slots of rows past the new size
+// die.  The block constants are then recomputed over all slots.
 int ensureShadow(const rxgpu_index* ix, cudaStream_t st) {
 	std::lock_guard<std::mutex> lck(ix->tc_mtx);
 	const uint32_t pitchQ = (ix->dim + kTcChunkK - 1) / kTcChunkK * kTcChunkK;
 	if (!ix->d_shadow) {
 		const size_t cap = (size_t(ix->capacity ? ix->capacity : 1) + kTcTileRows - 1) / kTcTileRows * kTcTileRows;  // whole tiles
-		RX_CUDA(cudaMalloc(&ix->d_shadow, cap * pitchQ));
-		RX_CUDA(cudaMalloc(reinterpret_cast<void**>(&ix->d_rowc), cap * sizeof(float4)));
+		const size_t slotCap = (cap + cap / kShadowResortDiv + kTcTileRows - 1) / kTcTileRows * kTcTileRows;
+		RX_CUDA(cudaMalloc(&ix->d_shadow, slotCap * pitchQ));
+		RX_CUDA(cudaMalloc(reinterpret_cast<void**>(&ix->d_rowc), slotCap * sizeof(float4)));
+		RX_CUDA(cudaMalloc(reinterpret_cast<void**>(&ix->d_slot_row), slotCap * sizeof(uint32_t)));
+		RX_CUDA(cudaMalloc(reinterpret_cast<void**>(&ix->d_row_slot), cap * sizeof(uint32_t)));
+		RX_CUDA(cudaMalloc(reinterpret_cast<void**>(&ix->d_blockc), slotCap / 64 * 2 * sizeof(float4)));
 		ix->pitch_q = pitchQ;
+		ix->shadow_slot_cap = slotCap;
 		ix->shadow_version = ~0ull;
 		ix->shadow_dirty_all = true;
 		ix->shadow_dirty.clear();
 	}
 	if (ix->shadow_version != ix->version) {
-		// only the rows the mutations since the last search rewrote (an upsert, a swap-remove, an appended run), unless the log gave up
+		const uint32_t size = uint32_t(ix->size), old = ix->shadow_rows;
 		auto convert = [&](uint32_t b, uint32_t e) {
 			const unsigned blocks = unsigned((uint64_t(e - b) * 32 + 255) / 256);
-			tc_convert_rows<<<blocks, 256, 0, st>>>(ix->d_rows, ix->pitch, ix->dim, b, e, static_cast<unsigned char*>(ix->d_shadow),
+			tc_convert_rows<<<blocks, 256, 0, st>>>(ix->d_rows, ix->pitch, ix->dim, b, e, ix->d_row_slot, static_cast<unsigned char*>(ix->d_shadow),
 													pitchQ / kTcChunkK, ix->metric == RXGPU_COS ? ix->d_norms : nullptr, ix->d_rowc);
+			g_stats.launches += 1;
 		};
-		if (ix->shadow_dirty_all) {
-			if (ix->size) {
-				convert(0, uint32_t(ix->size));
-			}
-		} else {
+		bool full = ix->shadow_dirty_all;
+		if (!full) {
+			const uint32_t kept = std::min(old, size), added = size - kept, gone = old - kept;
+			uint64_t rewritten = 0;
 			for (const auto& r : ix->shadow_dirty) {
-				const uint32_t e = uint32_t(std::min<uint64_t>(r.second, ix->size));
-				if (r.first < e) {
-					convert(r.first, e);
+				rewritten += r.first < kept ? std::min(r.second, kept) - r.first : 0u;
+			}
+			const uint64_t slots = uint64_t(ix->shadow_slots) + added;
+			full = slots > ix->shadow_slot_cap ||
+				   (uint64_t(ix->shadow_dead) + gone + ix->shadow_unsorted + added + rewritten) * kShadowResortDiv > slots;
+			if (!full) {
+				if (gone) {
+					tc_kill_rows<<<(gone + 255) / 256, 256, 0, st>>>(kept, old, ix->d_row_slot, ix->d_slot_row, ix->d_rowc);
+					g_stats.launches += 1;
 				}
+				for (const auto& r : ix->shadow_dirty) {
+					if (r.first < kept) {
+						convert(r.first, std::min(r.second, kept));
+					}
+				}
+				if (added) {
+					tc_assign_slots<<<(added + 255) / 256, 256, 0, st>>>(kept, size, ix->shadow_slots, ix->d_slot_row, ix->d_row_slot);
+					g_stats.launches += 1;
+					convert(kept, size);
+				}
+				ix->shadow_slots = uint32_t(slots);
+				ix->shadow_dead += gone;
+				ix->shadow_unsorted += uint32_t(added + rewritten);
 			}
 		}
+		if (full) {
+			if (size) {
+				if (int rc = sortShadowSlots(ix, st, size)) {
+					return rc;
+				}
+				convert(0, size);
+			}
+			ix->shadow_slots = size;
+			ix->shadow_dead = 0;
+			ix->shadow_unsorted = 0;
+		}
+		ix->shadow_rows = size;
 		ix->shadow_dirty_all = false;
 		ix->shadow_dirty.clear();
-		// rows past the end, up to whole tiles, have all-zero constants (their codes are never tested: the kernel masks rows >= n)
-		const uint64_t padded = (ix->size + kTcTileRows - 1) / kTcTileRows * kTcTileRows;
-		RX_CUDA(cudaMemsetAsync(ix->d_rowc + ix->size, 0, size_t(padded - ix->size) * sizeof(float4), st));
+		// slots past the end, up to whole tiles, have all-zero constants (their codes are never tested: the kernel masks slots >= n)
+		const uint32_t slots = ix->shadow_slots;
+		const uint64_t padded = (uint64_t(slots) + kTcTileRows - 1) / kTcTileRows * kTcTileRows;
+		RX_CUDA(cudaMemsetAsync(ix->d_rowc + slots, 0, size_t(padded - slots) * sizeof(float4), st));
+		const uint32_t nblocks = uint32_t(padded / 64);
+		if (nblocks) {
+			tc_block_consts<<<(nblocks * 32 + 255) / 256, 256, 0, st>>>(ix->d_rowc, ix->d_slot_row, slots, nblocks,
+																		   1.f - tc_l2eps(ix->dim), ix->metric, ix->d_blockc);
+			g_stats.launches += 1;
+		}
 		RX_CUDA(cudaGetLastError());
 		RX_CUDA(cudaStreamSynchronize(st));
 		ix->shadow_version = ix->version;
-		g_stats.launches += 1;
 	}
 	return 0;
 }
@@ -463,7 +557,7 @@ int tcPrepare(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float
 	return 0;
 }
 
-// The filter launches of a prepared batch over the rows [0, nrows), with the thresholds already in ws.d_tau: the rows whose certified
+// The filter launches of a prepared batch over the shadow's slots [0, nrows), with the thresholds already in ws.d_tau: the rows whose certified
 // lower bound is at or below the query's threshold tau go to ws.d_cand_rows[q][candCap], and ws.d_cand_count[q] counts them all (also
 // past candCap: an overflowed list).  fixedTau: init_rows = UINT32_MAX keeps every row out of the bound list, so tau never moves
 // (knn_tc.cuh header comment) and k1 is not used; otherwise tau tightens to the k1-th best exact distance of the bound list that
@@ -490,6 +584,8 @@ int tcLaunch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const TcBatc
 	TcArgs a{};
 	a.shadow = static_cast<const unsigned char*>(ix->d_shadow);
 	a.rowc = ix->d_rowc;
+	a.slot_row = ix->d_slot_row;
+	a.blockc = ix->d_blockc;
 	a.qc = ws.d_qc.p;
 	a.tau = ws.d_tau.p;
 	a.ub_list = fixedTau ? nullptr : ws.d_ub_list.p;
@@ -564,7 +660,7 @@ int tcFilter(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float*
 			ws.d_qf.p, nq, k1, ix->metric, ws.d_tau.p, ws.d_ub_list.p, ws.d_ub_lock.p);
 		g_stats.launches += 1;
 	}
-	return tcLaunch(ix, ws, st, b, k1, candCap, uint32_t(ix->size), h_tau != nullptr);
+	return tcLaunch(ix, ws, st, b, k1, candCap, ix->shadow_slots, h_tau != nullptr);
 }
 
 // knn_rerank's range mode over the candidate lists: CTA b keeps the candidates of query q = qsel[b] (b without qsel) with
@@ -632,19 +728,22 @@ int scanTopKStaged(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const 
 	s.out_label = d_out_label;
 	s.out_count = d_out_count;
 	s.neg_zero = ix->metric != RXGPU_L2;
+	// the stages filter growing prefixes of the shadow's slots (sorted, so not the seed's rows); the last one covers every slot
+	const uint32_t slots = ix->shadow_slots;
+	uint32_t prefix = rows;
 	do {
-		rows = uint32_t(std::min<uint64_t>(size, uint64_t(rows) * kStageRatio));
-		if (int rc = tcLaunch(ix, ws, st, b, k1, cap, rows, true)) {
+		prefix = uint32_t(std::min<uint64_t>(slots, uint64_t(prefix) * kStageRatio));
+		if (int rc = tcLaunch(ix, ws, st, b, k1, cap, prefix, true)) {
 			return rc;
 		}
 		if (int rc = rerankRange(ix, ws, st, d_queries, nq, nq, nullptr, cap, ws.d_radius.p, ws.d_range.p, ws.d_range_n.p)) {
 			return rc;
 		}
-		s.last = rows == size;
+		s.last = prefix == slots;
 		knn_select_topk<<<nq, kSelThreads, 0, st>>>(s);
 		RX_CUDA(cudaGetLastError());
 		g_stats.launches += 1;
-	} while (rows < size);
+	} while (prefix < slots);
 	RX_CUDA(cudaMemcpyAsync(ws.h_cand_count.p, ws.d_cand_count.p, size_t(nq) * 4, cudaMemcpyDeviceToHost, st));
 	RX_CUDA(cudaMemcpyAsync(ws.h_stage_status.p, ws.d_stage_status.p, size_t(nq) * 4, cudaMemcpyDeviceToHost, st));
 	RX_CUDA(cudaMemcpyAsync(ws.h_reranked.p, ws.d_reranked.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
@@ -1024,10 +1123,8 @@ int rxgpu_index_resize(rxgpu_index* ix, uint64_t new_capacity) {
 	ix->d_norms = norms;
 	ix->capacity = new_capacity;
 	if (ix->d_shadow) {  // rebuilt lazily at the new capacity
-		cudaFree(ix->d_shadow);
-		cudaFree(ix->d_rowc);
-		ix->d_shadow = nullptr;
-		ix->d_rowc = nullptr;
+		std::lock_guard<std::mutex> lck(ix->tc_mtx);
+		releaseShadow(ix);
 	}
 	try {
 		if (ix->flags & RXGPU_FLAG_HOST_MIRROR) {

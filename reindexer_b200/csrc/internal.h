@@ -215,9 +215,19 @@ struct rxgpu_index {
 
 	// tensor-core filter state, built lazily by the first large-batch search: int8 shadow of the rows + per-row constants
 	mutable std::mutex tc_mtx;
-	mutable void* d_shadow = nullptr;  // int8 codes, [capacity / 64 blocks][pitch_q / 128 chunks][64 x 128 B], knn_tc.cuh
-	mutable float4* d_rowc = nullptr;  // [capacity] (scale, residual norm, norm, Cosine coefficient) of every row
+	// The shadow holds the rows in SLOT order: sorted by the block test's row factors at a full build (ensureShadow), rows appended
+	// since then in new slots at the end, the slots of vanished rows dead (knn_tc.cuh: kTcDeadSlot).
+	mutable void* d_shadow = nullptr;  // int8 codes, [slot capacity / 64 blocks][pitch_q / 128 chunks][64 x 128 B], knn_tc.cuh
+	mutable float4* d_rowc = nullptr;  // [slot capacity] (scale, residual norm, norm, Cosine coefficient) of every slot's row
+	mutable uint32_t* d_slot_row = nullptr;  // [slot capacity] the row of a slot, kTcDeadSlot for none
+	mutable uint32_t* d_row_slot = nullptr;  // [capacity] the slot of a row
+	mutable float4* d_blockc = nullptr;      // [slot capacity / 64][2] tc_block_consts
 	mutable uint32_t pitch_q = 0;      // bytes of codes per row, dim rounded up to 128
+	mutable uint64_t shadow_slot_cap = 0;    // slots allocated (whole tiles)
+	mutable uint32_t shadow_slots = 0;       // slots in use, dead ones included
+	mutable uint32_t shadow_rows = 0;        // rows the shadow holds (the index size when it was last brought up to date)
+	mutable uint32_t shadow_unsorted = 0;    // slots appended or rewritten since the last full build
+	mutable uint32_t shadow_dead = 0;        // dead slots
 	mutable uint64_t shadow_version = ~0ull;
 	// rows rewritten since the shadow was last brought up to date (the mutations log them beside `version`): ensureShadow converts
 	// only these; the log gives up (full rebuild) beyond kShadowLogMax ranges
@@ -265,9 +275,10 @@ struct rxgpu_index {
 		if (d_shadow) {
 			cudaFree(d_shadow);
 		}
-		if (d_rowc) {
-			cudaFree(d_rowc);
-		}
+		cudaFree(d_rowc);
+		cudaFree(d_slot_row);
+		cudaFree(d_row_slot);
+		cudaFree(d_blockc);
 		if (stream) {
 			cudaStreamDestroy(stream);
 		}

@@ -81,15 +81,17 @@ constexpr uint32_t kTcMaxK1 = 128;  // k + 1 <= 128: the bound list is scanned l
 constexpr float kTcL2Eps = 1e-5f;
 
 struct TcArgs {
-	const unsigned char* shadow;  // int8 codes, [64-row block][K chunk][64 rows x 128 B, SWIZZLE_128B pattern pre-applied]
-	const float4* rowc;        // [rows padded to whole tiles] (s_v, r_v, n_v, c_v): scale, residual norm, norm, Cosine coefficient
-								// (1 for IP / L2); zero beyond n
+	const unsigned char* shadow;  // int8 codes by SLOT, [64-slot block][K chunk][64 slots x 128 B, SWIZZLE_128B pattern pre-applied]
+	const float4* rowc;        // [slots padded to whole tiles] (s_v, r_v, n_v, c_v) of the slot's row: scale, residual norm, norm,
+								// Cosine coefficient (1 for IP / L2); zero for dead slots and beyond n
+	const uint32_t* slot_row;  // [slots] the row a slot holds (kTcDeadSlot: none)
+	const float4* blockc;      // [64-slot blocks][2] the block test's row factors of every block (tc_block_consts)
 	const float4* qc;          // [nq_total] (s_q, r_q, n_q, 1 / max(s_q, tiny)) of tc_prepare_queries
 	unsigned int* tau;         // [nq_total] ordered-uint of the current threshold (map space), shared by all CTAs
 	float* ub_list;            // [nq_total][kTcMaxK1] the bound list: the k1 smallest exact distances of the rows inserted by any CTA
 							   // (guarded by ub_lock)
 	unsigned int* ub_lock;     // [nq_total]
-	uint32_t init_rows;        // rows [0, init_rows) are already represented in ub_list by tc_init_tau (never insert them twice)
+	uint32_t init_rows;        // ROWS [0, init_rows) are already represented in ub_list by tc_init_tau (never insert them twice)
 	const float* rows;         // fp32 rows [n][pitch] and the Cosine norm coefficients (nullptr otherwise): the bookkeepers' exact
 	const float* norm_coefs;   // distances of the rows they insert into the bound list
 	const float* qf;           // [nq_total][kchunks * 128] fp32 queries, zero padded (tc_prepare_queries)
@@ -97,7 +99,7 @@ struct TcArgs {
 	uint32_t* cand_rows;       // [nq_total][cand_cap]
 	unsigned int* cand_count;  // [nq_total]
 	uint32_t cand_cap;
-	uint32_t n;                // rows
+	uint32_t n;                // slots: a prefix of the shadow's slots (all of them, or a stage's prefix)
 	uint32_t dim;
 	uint32_t kchunks;          // padded dim / 128
 	uint32_t nq_total;         // queries in the whole batch
@@ -130,8 +132,8 @@ constexpr uint32_t kTcDiagMarkEvery = 64;
 // blocks, hits and queue waits are counts), the producer at kTcDgEmpty (cycles waiting on `empty`) and kTcDgProd (total)
 enum : uint32_t {
 	kTcDgFull,     // waiting on full[stage]
-	kTcDgMma,      // the rest of the K loop: tau refresh, row constants, MMA issue, wgmma_wait<1>, stage release, handing the turn over
-	kTcDgDrain,    // wgmma_wait<0> and the last release
+	kTcDgMma,      // the rest of the K loop: tau refresh, block constants, MMA issue, wgmma_wait<1>, stage release, handing the turn over
+	kTcDgDrain,    // wgmma_wait<0>, the last release and the block thresholds
 	kTcDgBar1,     // the first bar.sync
 	kTcDgTest,     // the block test: the branch-free loop that builds the hit mask
 	kTcDgAppend,   // the vote on the hit masks and the enqueues of the hits (their waits on a full queue included)
@@ -151,10 +153,10 @@ enum : uint32_t {
 };
 static_assert(kTcDgRescoreCycles < kTcDiagSlots, "diagnostic counters fit their slots");
 
-// shared memory: query block, the stage ring, barriers, per-query constants, then per consumer warpgroup thresholds and (P, R)
+// shared memory: query block, the stage ring, barriers, per-query constants, then per consumer warpgroup thresholds and block thresholds
 __host__ __device__ inline size_t tc_smem_bytes(uint32_t nq_block, uint32_t kchunks, uint32_t stages = kTcStages) {
 	return 1024 /*align slack*/ + size_t(nq_block) * kchunks * 128 + size_t(stages) * kTcBlockBytes + 256 /*barriers*/ +
-		   size_t(nq_block) * (16 /*qc*/ + kTcConsumers * (4 + 8) /*thr, pr per warpgroup*/) + 64;
+		   size_t(nq_block) * (16 /*qc*/ + kTcConsumers * (4 + 4) /*thr, block threshold per warpgroup*/) + 64;
 }
 
 // ---- PTX wrappers -------------------------------------------------------------------------------------------------------------
@@ -326,16 +328,47 @@ __device__ __forceinline__ void wgmma_s8(int (&d)[N / 2], uint64_t adesc, uint64
 	}
 }
 
-// The candidate test lb <= tau on the raw accumulator I, for every score one int -> float conversion (I2FP.F32.S32, an ALU-pipe
-// instruction on sm_90), two (L2: three) FFMAs and one compare.  The block bound e <= n_q M_v, with
+// The candidate test lb <= tau.  The block bound e <= n_q M_v, with
 //   M_v = c_v (a* r_v + b* n_v),   a* >= (1 + 2^-8) (n_q + r_q) / n_q,   b* >= (1 + 2^-8) (r_q + (D + 16) 2^-23 n_q) / n_q
 // (a*, b*: the largest over the CTA's query block, computed once per launch), makes the per-row and the per-query factors separate;
-// dividing the test by k_q = s_q (1 for an all-zero query, whose codes are zero) gives, with x = float(I) and S_v = s_v c_v,
+// dividing the test by k_q = s_q (1 for an all-zero query, whose codes are zero) gives, with x = I and S_v = s_v c_v,
 //   IP, Cosine  x S_v + P M_v + R >= 0               P = n_q / k_q   R = tau / k_q
 //   L2          x S_v + P M_v - Z W_v + R >= 0       Z = 1 / k_q     R = (tau - (1 - eps) n_q^2) / (2 k_q)    W_v = (1 - eps) n_v^2 / 2
-// The test is evaluated as "not below zero", so an overflow to NaN (magnitudes far outside the data the exact scan handles) lets
-// the row through to the bookkeeper, which decides with the per-query bound e(q, v) and no division.
-__device__ __forceinline__ float tc_l2eps(uint32_t dim) { return kTcL2Eps + float(dim + 1) * 0x1p-23f; }
+// For S_v > 0 this is x >= T(q, v) = -R u_v - P (a* rho_v + b* nu_v) + Z w_v with u_v = 1 / S_v, rho_v = r_v / s_v, nu_v = n_v / s_v
+// (c_v cancels) and w_v = W_v / S_v (0 for IP and Cosine); P, a*, b*, Z >= 0.  The shadow stores the rows SORTED so that the 64 rows
+// of a slot block have nearly equal factors (ensureShadow: by S_v descending; L2 first by coarse buckets of n_v^2), and tc_block_consts
+// keeps per block u_lo <= u_v <= u_hi, rho_hi >= rho_v, nu_hi >= nu_v, w_lo <= w_v <= w_hi over its live rows, each rounded outwards
+// from fp64 with directed rounding, so with real arithmetic
+//   T_B(q) = min(-R u_lo, -R u_hi) - P (a* rho_hi + b* nu_hi) + Z w_lo  <=  T(q, v)   for every live row v of the block.
+// The consumer evaluates T_B once per (query, block) in fp32: about ten roundings, each at most 2^-24 of
+//   mag = |R| u_hi + P (a* rho_hi + b* nu_hi) + Z w_hi,
+// so the computed value is within 2^-20 mag of T_B; it subtracts slack = 2^-18 mag + 1, rounds down to an int and clamps to
+// [-2^30, 2^30] (|I| < 2^25 at every accepted dim; +inf only when tau = -inf or a positive term overflows while the others stay
+// finite, so the true T_B is far above 2^25 too).  A score then passes when I >= that integer: one integer compare, no conversion.
+// Blocks holding a live row with S_v <= 0 (an all-zero row, a zero-norm Cosine row) or any non-finite factor pass every pair
+// (threshold -2^30), and so does a NaN threshold, as "not below zero" lets NaN through in the exact form; a block with no live slot
+// passes none.  The bookkeeper then decides every hit with the row's own bound e(q, v), exactly as before.
+__host__ __device__ __forceinline__ float tc_l2eps(uint32_t dim) { return kTcL2Eps + float(dim + 1) * 0x1p-23f; }
+constexpr uint32_t kTcDeadSlot = 0xFFFFFFFFu;
+constexpr int kTcPassAll = -(1 << 30), kTcPassNone = 1 << 30;
+// tc_block_consts' record of one 64-slot block: (u_lo, u_hi, rho_hi, nu_hi), (w_lo, w_hi, flag, 0); flag 1 = every pair passes,
+// -1 = no live slot (no pair passes), 0 = T_B applies
+__device__ __forceinline__ int tc_block_threshold(float R, float P, float Z, float ka, float kb, float4 b0, float4 b1) {
+	if (b1.z != 0.f) {
+		return b1.z > 0.f ? kTcPassAll : kTcPassNone;
+	}
+	const float m = P * fmaf(ka, b0.z, kb * b0.w);
+	const float t = fminf(-R * b0.x, -R * b0.y) - m + Z * b1.x;
+	if (t == INFINITY) {  // tau = -inf (a query that admits nothing), or a positive term beyond fp32 with the others finite
+		return kTcPassNone;
+	}
+	const float mag = fmaf(fabsf(R), b0.y, fmaf(Z, b1.y, m));
+	const float f = t - fmaf(mag, 0x1p-18f, 1.f);
+	if (!(f >= -0x1p30f)) {  // NaN included
+		return kTcPassAll;
+	}
+	return f > 0x1p30f ? kTcPassNone : int(floorf(f));
+}
 __device__ __forceinline__ float2 tc_make_pr(int metric, float tau, float4 qc, float l2eps) {  // qc = (s_q, r_q, n_q, 1 / k_q)
 	const float p = qc.z * qc.w;
 	if (metric != kL2) {
@@ -346,10 +379,10 @@ __device__ __forceinline__ float2 tc_make_pr(int metric, float tau, float4 qc, f
 
 // ---- the candidate queue: consumers -> bookkeepers --------------------------------------------------------------------------------
 // A (query, row) pair that passes the block test is a hit.  The consumer warpgroup that found it only enqueues it: one shared-memory
-// atomicAdd takes a ticket, a 16-byte record (query in the block, row, x = float(I), ticket + 1) goes into the warpgroup's ring of
+// atomicAdd takes a ticket, a 16-byte record (query in the block, slot, x = float(I), ticket + 1) goes into the warpgroup's ring of
 // `slots` records, the last word stored with release semantics.  Its BOOKKEEPER warp (warp 1 + w for consumer warpgroup w; idle
 // otherwise) takes the records in ticket order, up to 32 at a time, frees their slots, and runs the rare path off
-// the MMA path: the row's own bound, the candidate append, the bound list and tau.  A full ring makes the consumer wait until the
+// the MMA path: the slot's row, its own bound, the candidate append, the bound list and tau.  A full ring makes the consumer wait until the
 // bookkeeper frees a slot; no hit is ever dropped.
 struct TcQueue {
 	uint32_t tail;        // tickets taken by the consumers
@@ -393,7 +426,7 @@ __device__ __forceinline__ void st_release_shared(uint32_t* p, uint32_t v) {
 }
 
 // consumer side: returns whether the ring was full (the caller waited)
-__device__ __forceinline__ bool tc_enqueue(TcQueue* qu, uint4* rec, uint32_t slots, uint32_t q, uint32_t row, float x) {
+__device__ __forceinline__ bool tc_enqueue(TcQueue* qu, uint4* rec, uint32_t slots, uint32_t q, uint32_t slot, float x) {
 	const uint32_t t = atomicAdd(&qu->tail, 1u);
 	bool waited = false;
 	while (t - ld_acquire_shared(&qu->head) >= slots) {  // the bookkeeper has not read the record this slot held yet
@@ -402,21 +435,21 @@ __device__ __forceinline__ bool tc_enqueue(TcQueue* qu, uint4* rec, uint32_t slo
 	}
 	uint4* r = rec + (t & (slots - 1));
 	r->x = q;
-	r->y = row;
+	r->y = slot;
 	r->z = __float_as_uint(x);
 	st_release_shared(&r->w, t + 1);
 	return waited;
 }
 
-// the hits of one accumulator quad (h = bits 0..3 for (row0, q), (row0, q + 1), (row1, q), (row1, q + 1)), out of line: inlined at
+// the hits of one accumulator quad (h = bits 0..3 for (slot0, q), (slot0, q + 1), (slot1, q), (slot1, q + 1)), out of line: inlined at
 // each of the kNq / 8 quads of the unrolled append loop it only spreads the consumer loop over more instruction cache
-__device__ __noinline__ bool tc_enqueue_quad(TcQueue* qu, uint4* rec, uint32_t slots, uint32_t h, uint32_t q, uint32_t row0, uint32_t row1,
+__device__ __noinline__ bool tc_enqueue_quad(TcQueue* qu, uint4* rec, uint32_t slots, uint32_t h, uint32_t q, uint32_t slot0, uint32_t slot1,
 											 float x0, float x1, float x2, float x3) {
 	bool waited = false;
-	if (h & 1u) waited |= tc_enqueue(qu, rec, slots, q, row0, x0);
-	if (h & 2u) waited |= tc_enqueue(qu, rec, slots, q + 1, row0, x1);
-	if (h & 4u) waited |= tc_enqueue(qu, rec, slots, q, row1, x2);
-	if (h & 8u) waited |= tc_enqueue(qu, rec, slots, q + 1, row1, x3);
+	if (h & 1u) waited |= tc_enqueue(qu, rec, slots, q, slot0, x0);
+	if (h & 2u) waited |= tc_enqueue(qu, rec, slots, q + 1, slot0, x1);
+	if (h & 4u) waited |= tc_enqueue(qu, rec, slots, q, slot1, x2);
+	if (h & 8u) waited |= tc_enqueue(qu, rec, slots, q + 1, slot1, x3);
 	return waited;
 }
 
@@ -493,12 +526,13 @@ __device__ __noinline__ float tc_rescore(const TcArgs& a, unsigned todo, uint32_
 	return mine;
 }
 
-// Bookkeeper warp of one consumer warpgroup's queue, until every consumer warp is done and the ring is empty.  A row is appended
+// Bookkeeper warp of one consumer warpgroup's queue, until every consumer warp is done and the ring is empty.  A hit's slot is mapped
+// to its row (a dead slot is dropped); the row is appended
 // when its own lower bound d~ - err passes the tightest threshold the CTA knows for the query (NaN: appended); the appends of one
 // batch go to the candidate lists with one global atomicAdd per distinct query.  When the row's midpoint d~ beats that threshold
 // (and the seed does not hold the row already) the warp computes the row's EXACT distance d with the exact scan's arithmetic; a d
-// below the threshold goes into the bound list, and the threshold that comes back is published to the (P, R) of EVERY consumer
-// warpgroup.  A consumer may read a looser threshold meanwhile (a concurrent store of another writer may even replace a tighter one):
+// below the threshold goes into the bound list, and the threshold that comes back is published to the threshold of EVERY consumer
+// warpgroup, which turns it into its next block thresholds.  A consumer may read a looser threshold meanwhile (a concurrent store of another writer may even replace a tighter one):
 // every threshold ever published is a valid upper bound of the query's final k1-th distance, so the test stays certified.
 template <int kNq>
 __device__ __forceinline__ float tc_min_thr(const float* s_thr, uint32_t ql) {  // the tightest threshold of the consumer warpgroups
@@ -511,7 +545,7 @@ __device__ __forceinline__ float tc_min_thr(const float* s_thr, uint32_t ql) {  
 }
 template <int kNq, int kDiag>
 __device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, const uint4* rec, uint32_t slots, uint32_t q0, const float4* s_qc,
-											  float* s_thr, float2* s_pr, float l2eps, int lane, unsigned long long* dg) {
+											  float* s_thr, int lane, unsigned long long* dg) {
 	[[maybe_unused]] unsigned long long n_rescored = 0, n_inserts = 0;
 	[[maybe_unused]] long long rescore_cycles = 0;
 	uint32_t head = 0;
@@ -525,8 +559,8 @@ __device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, cons
 			__nanosleep(256);
 			continue;
 		}
-		const bool active = uint32_t(lane) < n;
-		uint32_t ql = 0, row = 0;
+		bool active = uint32_t(lane) < n;
+		uint32_t ql = 0, slot = 0;
 		float x = 0.f;
 		if (active) {
 			const uint32_t t = head + lane;
@@ -534,7 +568,7 @@ __device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, cons
 			while (ld_acquire_shared(&r->w) != t + 1) {  // the consumer holding ticket t has not stored its record yet
 			}
 			ql = r->x;
-			row = r->y;
+			slot = r->y;
 			x = __uint_as_float(r->z);
 		}
 		__syncwarp();
@@ -542,9 +576,11 @@ __device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, cons
 		if (lane == 0) {
 			st_release_shared(&qu->head, head);  // the records are read: their slots go back to the consumers
 		}
+		const uint32_t row = active ? a.slot_row[slot] : kTcDeadSlot;
+		active = active && row != kTcDeadSlot;
 		float d = 0.f, err = 0.f, tau = 0.f;
 		if (active) {
-			const float4 qc = s_qc[ql], rc = a.rowc[row];
+			const float4 qc = s_qc[ql], rc = a.rowc[slot];
 			const float2 de = tc_row_bound(a, x, qc, rc);
 			d = de.x;
 			err = de.y;
@@ -585,7 +621,6 @@ __device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, cons
 				for (uint32_t w = 0; w < kTcConsumers; ++w) {
 					if (nt < s_thr[w * kNq + ql]) {
 						s_thr[w * kNq + ql] = nt;
-						s_pr[w * kNq + ql] = tc_make_pr(a.metric, nt, s_qc[ql], l2eps);
 					}
 				}
 			}
@@ -632,8 +667,8 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 	float* s_ab = reinterpret_cast<float*>(q_bar + 1);                 // (a*, b*) of the block bound
 	float4* s_qc = reinterpret_cast<float4*>(bars + 32);               // [kNq] (s_q, r_q, n_q, 1 / k_q)
 	float* s_thr = reinterpret_cast<float*>(s_qc + kNq);               // [3][kNq] current tau (map space), per consumer warpgroup
-	float2* s_pr = reinterpret_cast<float2*>(s_thr + kTcConsumers * kNq);  // [3][kNq] (P, R) of the candidate test
-	TcQueue* s_queue = reinterpret_cast<TcQueue*>(s_pr + kTcConsumers * kNq);  // [3] candidate queue of each consumer warpgroup
+	int* s_tb = reinterpret_cast<int*>(s_thr + kTcConsumers * kNq);    // [3][kNq] the block thresholds of each warpgroup's current block
+	TcQueue* s_queue = reinterpret_cast<TcQueue*>(s_tb + kTcConsumers * kNq);  // [3] candidate queue of each consumer warpgroup
 	uint4* s_rec = reinterpret_cast<uint4*>(s_queue + kTcConsumers);  // [3][queue_slots] their records (beyond tc_smem_bytes)
 	static_assert(2 * kTcStages + 2 <= 32, "barriers and (a*, b*) fit in front of the per-query constants");
 
@@ -679,10 +714,9 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 			atomicMax(reinterpret_cast<unsigned int*>(&s_ab[1]), __float_as_uint(qc.y / qc.z + delta));
 		}
 		s_qc[i] = qc;
-		const float2 pr = valid ? tc_make_pr(a.metric, thr, qc, l2eps) : make_float2(0.f, -INFINITY);  // padding queries never match
 		for (int w = 0; w < kTcConsumers; ++w) {
 			s_thr[w * kNq + i] = thr;
-			s_pr[w * kNq + i] = pr;
+			s_tb[w * kNq + i] = kTcPassNone;  // padding queries never match; valid ones are set before every block test
 		}
 	}
 	__syncthreads();
@@ -748,12 +782,12 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 	} else if (warp < 4) {
 		// ===== bookkeeper of consumer warpgroup warp - 1 =====
 		const uint32_t wg = uint32_t(warp) - 1;
-		tc_bookkeeper<kNq, kDiag>(a, s_queue + wg, s_rec + wg * a.queue_slots, a.queue_slots, q0, s_qc, s_thr, s_pr, l2eps, lane, dg);
+		tc_bookkeeper<kNq, kDiag>(a, s_queue + wg, s_rec + wg * a.queue_slots, a.queue_slots, q0, s_qc, s_thr, lane, dg);
 	} else {
 		// ===== consumer warpgroup wg: the walker's blocks i = wg, wg + 3, wg + 6, ... =====
 		const uint32_t wg = uint32_t(warp) / 4 - 1, wtid = threadIdx.x - 128 * (wg + 1);
 		float* thr = s_thr + wg * kNq;
-		float2* pr = s_pr + wg * kNq;
+		int* tb = s_tb + wg * kNq;
 		TcQueue* qu = s_queue + wg;
 		uint4* rec = s_rec + wg * a.queue_slots;
 		const uint32_t slots = a.queue_slots;
@@ -762,7 +796,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		const unsigned char* ring_smem = s_rows;
 		// accumulator fragment of wgmma.m64nN: d[4j + {0,1}] = (row r0, query 8j + 2c + {0,1}), d[4j + {2,3}] = the same for row r0 + 8
 		const uint32_t r0 = (wtid >> 5) * 16 + (lane >> 2), c2 = 2 * (lane & 3);
-		const uint32_t my_q = wtid;  // the query whose threshold this thread refreshes from the global list
+		const uint32_t my_q = wtid;  // the query whose threshold this thread refreshes from the global list and turns into block thresholds
 		unsigned int tau_ahead = my_q < nq_valid ? a.tau[q0 + my_q] : 0u;
 		const bool l2 = a.metric == kL2;
 		const float ka = (1.f + 0x1p-7f) * s_ab[0], kb = (1.f + 0x1p-7f) * s_ab[1];  // 2^-8 of e, and 2^-8 for the rounding of M_v
@@ -796,12 +830,16 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 				const float tn = ord_float(tau_ahead);
 				if (tn < thr[my_q]) {
 					thr[my_q] = tn;
-					pr[my_q] = tc_make_pr(a.metric, tn, s_qc[my_q], l2eps);
 				}
 				tau_ahead = a.tau[q0 + my_q];
 			}
-			const uint32_t row0 = (2 * t + half) * 64 + r0, row1 = row0 + 8;
-			const float4 rc0 = a.rowc[row0], rc1 = a.rowc[row1];  // rows are padded to whole tiles; consumed after the MMAs
+			const uint32_t sb = 2 * t + half, slot0 = sb * 64 + r0, slot1 = slot0 + 8;
+			// the block's row factors (slots are padded to whole tiles), consumed after the MMAs by the threads that own a query
+			float4 bc0 = {}, bc1 = {};
+			if (my_q < nq_valid) {
+				bc0 = a.blockc[2 * sb];
+				bc1 = a.blockc[2 * sb + 1];
+			}
 			int acc[kNq / 2];
 #pragma unroll
 			for (int i = 0; i < kNq / 2; ++i) {
@@ -868,51 +906,35 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 			s1 = clk();
 			wgmma_wait<0>();
 			release(prev);
+			// this block's threshold of query my_q (header of tc_block_threshold), from the tightest tau this warpgroup knows now
+			if (my_q < nq_valid) {
+				const float4 qc = s_qc[my_q];
+				const float2 pr = tc_make_pr(a.metric, thr[my_q], qc, l2eps);
+				tb[my_q] = tc_block_threshold(pr.y, pr.x, l2 ? qc.w : 0.f, ka, kb, bc0, bc1);
+			}
 			s2 = clk();
-			asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // the refreshed (P, R) of all queries are visible
+			asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // the block thresholds of all queries are visible
 			s3 = clk();
-			// per-row factors of the block test (rows beyond n have all-zero constants and are masked anyway)
-			const float S0 = rc0.x * rc0.w, S1 = rc1.x * rc1.w;
-			const float M0 = rc0.w * fmaf(ka, rc0.y, kb * rc0.z), M1 = rc1.w * fmaf(ka, rc1.y, kb * rc1.z);
-			const float W0 = l2 ? 0.5f * (1.f - l2eps) * rc0.z * rc0.z : 0.f, W1 = l2 ? 0.5f * (1.f - l2eps) * rc1.z * rc1.z : 0.f;
 			// The block test: the predicate of every accumulator into the hit mask, bit i for acc[i] (quad j: bits 4j + {0, 1, 2, 3} =
-			// (row0, q), (row0, q + 1), (row1, q), (row1, q + 1)).  No call and no branch in the loop, so the quads' (P, R) loads and
-			// arithmetic overlap; the rows beyond n are masked out of every quad at once after it, and the hits, about one per block,
-			// are appended after that.
-			const uint32_t ok = (row0 < a.n ? 0x33333333u : 0u) | (row1 < a.n ? 0xCCCCCCCCu : 0u);
+			// (slot0, q), (slot0, q + 1), (slot1, q), (slot1, q + 1)): one integer compare per score against the (query, block)
+			// threshold.  No call and no branch in the loop; the slots beyond n are masked out of every quad at once after it, and the
+			// hits, about one per block, are appended after that.
+			const uint32_t ok = (slot0 < a.n ? 0x33333333u : 0u) | (slot1 < a.n ? 0xCCCCCCCCu : 0u);
 			constexpr int kMaskWords = (kNq / 2 + 31) / 32;
 			uint32_t hm[kMaskWords] = {};
-			auto test = [&](auto kL2Tag) {
-				constexpr bool kL2 = decltype(kL2Tag)::value;
-#pragma unroll
-				for (int j = 0; j < kNq / 8; ++j) {
-					const uint32_t q = 8 * j + c2;
-					const float4 p2 = *reinterpret_cast<const float4*>(&pr[q]);  // (P, R) of queries q and q + 1
-					float Ra = p2.y, Rb = p2.w, Rc = p2.y, Rd = p2.w;
-					if constexpr (kL2) {
-						const float za = s_qc[q].w, zb = s_qc[q + 1].w;
-						Ra = fmaf(-za, W0, Ra);
-						Rb = fmaf(-zb, W0, Rb);
-						Rc = fmaf(-za, W1, Rc);
-						Rd = fmaf(-zb, W1, Rd);
-					}
-					const float x0 = float(acc[4 * j]), x1 = float(acc[4 * j + 1]), x2 = float(acc[4 * j + 2]), x3 = float(acc[4 * j + 3]);
-					const bool h0 = !(fmaf(x0, S0, fmaf(p2.x, M0, Ra)) < 0.f);
-					const bool h1 = !(fmaf(x1, S0, fmaf(p2.z, M0, Rb)) < 0.f);
-					const bool h2 = !(fmaf(x2, S1, fmaf(p2.x, M1, Rc)) < 0.f);
-					const bool h3 = !(fmaf(x3, S1, fmaf(p2.z, M1, Rd)) < 0.f);
-					hm[4 * j / 32] |= (uint32_t(h0) | uint32_t(h1) << 1 | uint32_t(h2) << 2 | uint32_t(h3) << 3) << (4 * j % 32);
-				}
-			};
 			if constexpr (kDiag == kTcDiagNoTest) {
 #pragma unroll
 				for (int i = 0; i < kNq / 2; ++i) {
 					sink ^= uint32_t(acc[i]);
 				}
-			} else if (l2) {
-				test(std::true_type{});
 			} else {
-				test(std::false_type{});
+#pragma unroll
+				for (int j = 0; j < kNq / 8; ++j) {
+					const int2 t2 = *reinterpret_cast<const int2*>(&tb[8 * j + c2]);  // thresholds of queries q and q + 1
+					const bool h0 = acc[4 * j] >= t2.x, h1 = acc[4 * j + 1] >= t2.y;
+					const bool h2 = acc[4 * j + 2] >= t2.x, h3 = acc[4 * j + 3] >= t2.y;
+					hm[4 * j / 32] |= (uint32_t(h0) | uint32_t(h1) << 1 | uint32_t(h2) << 2 | uint32_t(h3) << 3) << (4 * j % 32);
+				}
 			}
 #pragma unroll
 			for (int w = 0; w < kMaskWords; ++w) {
@@ -935,7 +957,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 					for (int j = 0; j < kNq / 8; ++j) {
 						const uint32_t h = hm[4 * j / 32] >> (4 * j % 32) & 15u;
 						if (h) {
-							const bool waited = tc_enqueue_quad(qu, rec, slots, h, 8 * j + c2, row0, row1, float(acc[4 * j]), float(acc[4 * j + 1]),
+							const bool waited = tc_enqueue_quad(qu, rec, slots, h, 8 * j + c2, slot0, slot1, float(acc[4 * j]), float(acc[4 * j + 1]),
 																float(acc[4 * j + 2]), float(acc[4 * j + 3]));
 							if constexpr (kStamp) {
 								if (waited) {
@@ -948,7 +970,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 			}
 			__syncwarp();  // the rare path diverges (per-lane queue waits): reconverge before the .aligned wgmma of the next block
 			s5 = clk();
-			asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // nobody still reads (P, R) when the next refresh writes them
+			asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");  // nobody still reads tb when the next block's thresholds are written
 			if constexpr (kStamp) {
 				const long long s6 = clk();
 				dt[kTcDgMma] += s1 - s0;
@@ -1102,9 +1124,12 @@ __global__ void __launch_bounds__(kScanThreads) knn_rerank(const float* rows, ui
 
 // ---- staged exact thresholds (k1 > kTcMaxK1) ---------------------------------------------------------------------------------------
 // Any k1 rows give a valid threshold: their k1-th best exact distance is at least the k1-th best over all rows.  The seed is the exact
-// top-k1 over a short prefix of the rows; stage s then runs the filter with that fixed threshold over a prefix r times longer, re-ranks
-// the candidates with knn_rerank's range mode (radius = the next float above tau: it keeps exactly dist <= tau) and takes the k1-th
-// best survivor as the next threshold.  The last stage covers every row; its k1 best survivors are the exact answer.
+// top-k1 over a short prefix of the rows; stage s then runs the filter with that fixed threshold over a prefix of the shadow's SLOTS
+// r times longer than the last (slots are sorted, so a prefix holds other rows than the seed: it does not matter), re-ranks the
+// candidates with knn_rerank's range mode (radius = the next float above tau: it keeps exactly dist <= tau) and takes the k1-th best
+// survivor as the next threshold, or keeps the threshold when fewer than k1 survive.  Every threshold kept is thus its predecessor or
+// the k1-th best exact distance of some k1 distinct rows, so it stays valid.  The last stage covers every slot, so every row; its k1
+// best survivors are the exact answer.
 constexpr uint32_t kTcStagedMaxK1 = 1024;  // k + 1 <= 1024: the staged path's limit
 constexpr int kSelThreads = 512;
 constexpr uint32_t kSelSort = 4096;        // keys sorted in shared memory by knn_select_topk
@@ -1327,25 +1352,141 @@ __device__ __forceinline__ float3 tc_quantize(const float* p, uint32_t dim, uint
 	return make_float3(s, __double2float_ru(sqrt(rr) * (1.0 + 0x1p-40)), __double2float_ru(sqrt(ss) * (1.0 + 0x1p-40)));
 }
 
-// rows fp32 [n][pitch] -> int8 shadow + per-row constants (s_v, r_v, n_v, c_v), c_v = the Cosine norm coefficient (1 otherwise).
-// Shadow layout: [64-row block][K chunk of 128][64 rows x 128 bytes], and inside every 8 KB block the 16-byte units of row r are
-// XOR-permuted with (r % 8) -- the SWIZZLE_128B pattern wgmma expects in shared memory -- so that a plain contiguous cp.async.bulk
-// brings a ready-to-multiply operand tile.
-__global__ void tc_convert_rows(const float* rows, uint32_t pitch, uint32_t dim, uint32_t row_begin, uint32_t row_end, unsigned char* shadow,
-								uint32_t kchunks, const float* norm_coefs, float4* rowc) {
+// rows fp32 [n][pitch] -> int8 shadow + per-row constants (s_v, r_v, n_v, c_v), c_v = the Cosine norm coefficient (1 otherwise),
+// row v into slot row_slot[v].  Shadow layout: [64-slot block][K chunk of 128][64 slots x 128 bytes], and inside every 8 KB block the
+// 16-byte units of slot r are XOR-permuted with (r % 8) -- the SWIZZLE_128B pattern wgmma expects in shared memory -- so that a plain
+// contiguous cp.async.bulk brings a ready-to-multiply operand tile.
+__global__ void tc_convert_rows(const float* rows, uint32_t pitch, uint32_t dim, uint32_t row_begin, uint32_t row_end, const uint32_t* row_slot,
+								unsigned char* shadow, uint32_t kchunks, const float* norm_coefs, float4* rowc) {
 	const uint32_t row = row_begin + (blockIdx.x * blockDim.x + threadIdx.x) / 32;
 	const int lane = threadIdx.x & 31;
 	if (row >= row_end) {
 		return;
 	}
-	const uint32_t blk = row / 64u, r = row % 64u;
+	const uint32_t slot = row_slot[row], blk = slot / 64u, r = slot % 64u;
 	const float3 srn = tc_quantize(rows + size_t(row) * pitch, dim, kchunks * kTcChunkK, lane, [&](uint32_t c, uint32_t code4) {
 		const uint32_t kc = c / kTcChunkK, cc = c % kTcChunkK;
 		const uint32_t unit = (cc >> 4) ^ (r & 7u);  // 16-byte unit = 16 codes
 		*reinterpret_cast<uint32_t*>(shadow + (size_t(blk) * kchunks + kc) * kTcBlockBytes + r * 128u + unit * 16u + (cc & 15u)) = code4;
 	});
 	if (lane == 0) {
-		rowc[row] = make_float4(srn.x, srn.y, srn.z, norm_coefs ? norm_coefs[row] : 1.f);
+		rowc[slot] = make_float4(srn.x, srn.y, srn.z, norm_coefs ? norm_coefs[row] : 1.f);
+	}
+}
+
+// The sort key of the shadow's slot order (ensureShadow), one warp per row: S_v = s_v c_v descending (s_v as tc_quantize computes it),
+// for L2 after a coarse bucket of n_v^2 (its top 10 mantissa bits), so that the rows of a 64-slot block have nearly equal u_v and w_v
+// (tc_block_threshold).  The value is the row itself: a stable radix sort then breaks ties by the row.
+__global__ void tc_sort_keys(const float* rows, uint32_t pitch, uint32_t dim, uint32_t n, const float* norm_coefs, int metric, uint64_t* keys,
+							 uint32_t* vals) {
+	const uint32_t row = (blockIdx.x * blockDim.x + threadIdx.x) / 32;
+	const int lane = threadIdx.x & 31;
+	if (row >= n) {
+		return;
+	}
+	const float* p = rows + size_t(row) * pitch;
+	float mx = 0.f, ss = 0.f;
+	for (uint32_t c = lane; c < dim; c += 32) {
+		const float v = p[c];
+		mx = fmaxf(mx, fabsf(v));
+		ss = fmaf(v, v, ss);
+	}
+	for (int off = 16; off > 0; off >>= 1) {
+		mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+		ss += __shfl_xor_sync(0xffffffffu, ss, off);
+	}
+	if (lane == 0) {
+		const float S = (mx / 127.f) * (norm_coefs ? norm_coefs[row] : 1.f);
+		const uint64_t bucket = metric == kL2 ? float_ord(ss) >> 13 : 0u;
+		keys[row] = bucket << 32 | ~float_ord(S);
+		vals[row] = row;
+	}
+}
+
+// slot_row[0, n) holds the rows in slot order: the inverse map
+__global__ void tc_invert_slots(const uint32_t* slot_row, uint32_t n, uint32_t* row_slot) {
+	const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+	if (s < n) {
+		row_slot[slot_row[s]] = s;
+	}
+}
+
+// Incremental shadow updates: rows [row_begin, row_end) appended to slots slot_begin, slot_begin + 1, ... (assign), or gone (kill:
+// their slots become dead, all-zero constants)
+__global__ void tc_assign_slots(uint32_t row_begin, uint32_t row_end, uint32_t slot_begin, uint32_t* slot_row, uint32_t* row_slot) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (row_begin + i < row_end) {
+		slot_row[slot_begin + i] = row_begin + i;
+		row_slot[row_begin + i] = slot_begin + i;
+	}
+}
+__global__ void tc_kill_rows(uint32_t row_begin, uint32_t row_end, const uint32_t* row_slot, uint32_t* slot_row, float4* rowc) {
+	const uint32_t row = row_begin + blockIdx.x * blockDim.x + threadIdx.x;
+	if (row < row_end) {
+		const uint32_t slot = row_slot[row];
+		slot_row[slot] = kTcDeadSlot;
+		rowc[slot] = make_float4(0.f, 0.f, 0.f, 0.f);
+	}
+}
+
+// The block test's factors of every 64-slot block over its live slots (tc_block_threshold), one warp per block, two slots per lane:
+// fp64 quotients with directed rounding, so u_lo, w_lo are at or below and u_hi, rho_hi, nu_hi, w_hi at or above every live row's.
+// one_minus_eps = 1 - tc_l2eps(dim) for L2 (w = 0 otherwise), the same fp32 value the consumers' R uses.
+__global__ void tc_block_consts(const float4* rowc, const uint32_t* slot_row, uint32_t nslots, uint32_t nblocks, float one_minus_eps,
+								int metric, float4* blockc) {
+	const uint32_t blk = (blockIdx.x * blockDim.x + threadIdx.x) / 32;
+	const int lane = threadIdx.x & 31;
+	if (blk >= nblocks) {
+		return;
+	}
+	float u_lo = INFINITY, u_hi = 0.f, rho_hi = 0.f, nu_hi = 0.f, w_lo = INFINITY, w_hi = 0.f;
+	bool live = false, pass_all = false;
+	for (uint32_t i = 0; i < 2; ++i) {
+		const uint32_t slot = blk * 64 + 2 * lane + i;
+		if (slot >= nslots || slot_row[slot] == kTcDeadSlot) {
+			continue;
+		}
+		live = true;
+		const float4 rc = rowc[slot];  // (s, r, n, c)
+		const double S = double(rc.x) * double(rc.w);  // exact: 24 x 24 significant bits
+		if (!(S > 0.0) || !isfinite(S) || !isfinite(rc.y) || !isfinite(rc.z)) {  // NaN included
+			pass_all = true;
+			continue;
+		}
+		const float u0 = __double2float_rd(__ddiv_rd(1.0, S)), u1 = __double2float_ru(__ddiv_ru(1.0, S));
+		const float rho = __double2float_ru(__ddiv_ru(double(rc.y), double(rc.x)));
+		const float nu = __double2float_ru(__ddiv_ru(double(rc.z), double(rc.x)));
+		float w0 = 0.f, w1 = 0.f;
+		if (metric == kL2) {  // w = (1 - eps) n^2 / (2 S)
+			const double nn = double(rc.z) * double(rc.z);  // exact
+			w0 = __double2float_rd(__ddiv_rd(__dmul_rd(nn, double(one_minus_eps)), 2.0 * S));
+			w1 = __double2float_ru(__ddiv_ru(__dmul_ru(nn, double(one_minus_eps)), 2.0 * S));
+		}
+		if (!isfinite(u1) || !isfinite(rho) || !isfinite(nu) || !isfinite(w1) || u0 == 0.f) {
+			pass_all = true;
+			continue;
+		}
+		u_lo = fminf(u_lo, u0);
+		u_hi = fmaxf(u_hi, u1);
+		rho_hi = fmaxf(rho_hi, rho);
+		nu_hi = fmaxf(nu_hi, nu);
+		w_lo = fminf(w_lo, w0);
+		w_hi = fmaxf(w_hi, w1);
+	}
+	for (int off = 16; off > 0; off >>= 1) {
+		u_lo = fminf(u_lo, __shfl_xor_sync(0xffffffffu, u_lo, off));
+		u_hi = fmaxf(u_hi, __shfl_xor_sync(0xffffffffu, u_hi, off));
+		rho_hi = fmaxf(rho_hi, __shfl_xor_sync(0xffffffffu, rho_hi, off));
+		nu_hi = fmaxf(nu_hi, __shfl_xor_sync(0xffffffffu, nu_hi, off));
+		w_lo = fminf(w_lo, __shfl_xor_sync(0xffffffffu, w_lo, off));
+		w_hi = fmaxf(w_hi, __shfl_xor_sync(0xffffffffu, w_hi, off));
+	}
+	live = __any_sync(0xffffffffu, live);
+	pass_all = __any_sync(0xffffffffu, pass_all);
+	if (lane == 0) {
+		const float flag = pass_all ? 1.f : live ? 0.f : -1.f;
+		blockc[2 * blk] = flag == 0.f ? make_float4(u_lo, u_hi, rho_hi, nu_hi) : make_float4(0.f, 0.f, 0.f, 0.f);
+		blockc[2 * blk + 1] = flag == 0.f ? make_float4(w_lo, w_hi, flag, 0.f) : make_float4(0.f, 0.f, flag, 0.f);
 	}
 }
 
