@@ -1,4 +1,4 @@
-// Internal declarations shared by the translation units of librxgpu (index.cu, hnsw.cu, ft_bm25.cu).  Not part of the ABI.
+// Internal declarations shared by the translation units of librxgpu (index.cu, ivf.cu, hnsw.cu, ft_bm25.cu, ...).  Not part of the ABI.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -175,7 +175,7 @@ struct Workspace {
 }  // namespace rxgpu
 
 struct rxgpu_hnsw_device;  // hnsw.cu
-struct rxgpu_ivf_device;   // index.cu
+struct rxgpu_ivf_device;   // ivf.cu
 struct rxgpu_sq8_device;   // sq8.cu
 namespace rxgpu {
 void hnswRelease(rxgpu_hnsw_device*);
@@ -334,6 +334,25 @@ struct Hit;  // host/knn_select.h
 using RangeEmit = std::function<void(uint32_t q, const std::vector<Hit>& hits)>;
 int rangeBatch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, const float* radius,
 			   uint64_t max_out, const RangeEmit& emit);
+
+// index.cu -- the kernels of knn_scan.cuh, which are compiled there only; the IVF index (ivf.cu) launches them through these
+struct ScanArgs;
+struct MergeArgs;
+// the exact scan (knn_scan_warp) with a qt-query tile, its grid to *gridOut (dryRun: nothing launched); keysOut: the key mode of the
+// work-item scan (qt = 1)
+cudaError_t launchScan(const rxgpu_index* ix, int qt, const ScanArgs& a, unsigned* gridOut, cudaStream_t st, bool dryRun = false,
+					   bool keysOut = false);
+cudaError_t launchMergeLists(const MergeArgs& m, uint32_t nq, cudaStream_t st);  // knn_merge_lists, one CTA per query
+// 1/||row|| of the rows [row_begin, row_end) (norm_coef_kernel)
+cudaError_t launchNormCoefs(const float* rows, uint32_t pitch, uint32_t dim, uint32_t row_begin, uint32_t row_end, float* coefs, cudaStream_t st);
+// staged rows [n][dim] to rows[dst[i]] (zero padded to pitch) with their labels, and with `norms` their 1/||row|| too
+cudaError_t scatterRows(const float* staged, const uint32_t* dst, const uint64_t* staged_labels, uint32_t n, uint32_t dim, uint32_t pitch,
+						float* rows, uint64_t* labels, float* norms, cudaStream_t st);
+// The range-mode scan `a` until its key buffer held every match: zeroes the counter, scans, reads the count, and when the buffer
+// (a.range_cap keys) was too small grows it and scans again.  The matches with their labels (h_labels, by row), in the order of
+// hitLessByLabel; `scans` counts the launches.
+int scanRangeHits(const rxgpu_index* ix, cudaStream_t st, ScanArgs a, DevBuf<uint64_t>& d_keys, DevBuf<unsigned long long>& d_count,
+				  PinBuf<uint64_t>& h_keys, const uint64_t* h_labels, std::vector<Hit>& res, uint32_t& scans);
 
 // writes row `idx` (== size: appends) with a new vector and label, keeping the label dictionary consistent (index.cu)
 int setRowAt(rxgpu_index* ix, uint32_t idx, uint64_t label, const float* vec);
