@@ -331,7 +331,8 @@ int rxgpu_hnsw_search_knn_sq8(const rxgpu_index*, uint32_t nq, const float* quer
 /* ---------------------------------------------------------------- IVF index (faiss::IndexIVFFlat as reindexer::IvfIndex drives it)
  * Replaces the search side of IvfIndex: map_->search(1, key, k, dists, ids, &IVFSearchParameters{nprobe})
  *   core/index/float_vector/ivf_index.cc:150-204 (callers), vendor_subdirs/faiss/IndexIVF.cpp (search_preassigned), IndexIVFFlat.cpp
- *   (the flat list scanner).  Training (k-means) and list assignment stay with the reference's FAISS on the CPU; the adapter fills
+ *   (the flat list scanner).  Training (k-means) and list assignment run either on the device (rxgpu_ivf_train / _assign below) or in
+ * the reference's FAISS on the CPU; in the second case the adapter fills
  * the device index with the rows GROUPED BY LIST (list 0's vectors first, then list 1's, ...; label = the FAISS id) and hands
  * over the centroids and list sizes.  A search = coarse quantiser (distance to every centroid, nprobe nearest) + a scan of the
  * probed lists with the exact-scan kernel (fused top-k per list) + one merge.  Cosine: queries pre-normalised, rows and centroids
@@ -375,6 +376,51 @@ int rxgpu_ivf_add(rxgpu_index*, uint64_t n, const uint32_t* list_nos, const uint
 int rxgpu_ivf_remove(rxgpu_index*, uint64_t label); /* errNotFound when the id is in no list */
 uint64_t rxgpu_ivf_size(const rxgpu_index*);
 int rxgpu_ivf_list_stats(const rxgpu_index*, uint64_t* slab_rows, uint64_t* dead_rows, uint64_t* relocations, uint64_t* compactions);
+
+/* Training on the device -- what IvfIndex::trainIdx runs on the CPU (idx.train(n, x, norms): IndexIVFFlat::train -> Level1Quantizer::
+ * train_q1 -> faiss::Clustering::train, nredo 1, unweighted, spherical for IP and Cosine) and the list assignment of add_with_ids
+ * (quantizer->assign).  The sample and the initial centroids come from the same std::mt19937 draws as FAISS's (rxgpu_kmeans_plan); an
+ * iteration assigns every point to its nearest centroid under (distance, centroid id) with the coarse pass's exact arithmetic, sums
+ * each centroid's members in ascending point order in fp32 and scales by 1 / count, splits empty clusters as split_clusters does,
+ * then renormalises (spherical: fp64 norm, one rounding).  Given the same assignments the centroids are FAISS's bit for bit for L2
+ * (DESIGN.md §3.7).  Cosine input is normalised first: each vector times norm_coefs[i] when given, else as rxgpu_select_knn normalises
+ * a query. */
+typedef struct {
+	int32_t niter;                   /* Lloyd iterations, >= 0 (IndexIVF: 10) */
+	int32_t seed;                    /* >= 0 (1234); FAISS turns a negative seed into a clock-based one: errParams here */
+	int32_t max_points_per_centroid; /* >= 1 (256): more than nlist x this points are subsampled */
+} rxgpu_ivf_train_params;
+typedef struct { /* per iteration, as faiss::ClusteringIterationStats */
+	double obj;          /* fp64 sum of the points' exact distances in FAISS's convention (L2: squared distance, IP / Cosine: similarity) */
+	int32_t nsplit;      /* empty clusters split */
+	float assign_ms;     /* the assignment kernel (CUDA events) */
+	float update_ms;     /* the update's device work: key split, sort, sums, splits and renormalisation (CUDA events) */
+	float host_ms;       /* the update's host work between them: keys back, objective, histogram, split choices, offsets out */
+} rxgpu_ivf_train_stats;
+/* Trains nlist centroids on n host vectors and leaves the index as rxgpu_ivf_create(nlist, centroids) would: empty lists, centroids
+ * resident.  out_centroids: nlist x dim or NULL; stats: niter entries or NULL (n == nlist after sampling copies the points, as FAISS's
+ * corner case does, and reports zeros); params NULL: IndexIVF's defaults.  The index must be empty with no IVF attached (errLogic).
+ * errParams: NaN or Inf in the input, n < nlist, nlist outside [1, 131072], dim beyond the coarse pass's bound, bad params.  Device
+ * memory short for the training set: errSystem.  On any error the index is unchanged. */
+int rxgpu_ivf_train(rxgpu_index*, uint32_t nlist, uint64_t n, const float* vecs /* n x dim, host */,
+					const float* norm_coefs /* Cosine: n or NULL */, const rxgpu_ivf_train_params* params, float* out_centroids,
+					rxgpu_ivf_train_stats* stats);
+/* quantizer->assign as IndexIVF::add_with_ids calls it (same Cosine handling as rxgpu_ivf_train): the nearest centroid of every vector
+ * under (distance, centroid id), exactly the centroid rxgpu_ivf_search_* probes first at nprobe = 1.  out_dist: its distance in map
+ * space, or NULL.  Needs IVF lists (imported or created) and the index unchanged since, like the searches. */
+/* Concurrency: rxgpu_ivf_assign only reads the centroids, which no call changes while the lists exist, so it may run beside searches
+ * and adds; rxgpu_ivf_add_assign is a mutation like rxgpu_ivf_add (one at a time per index, as the reference's write lock keeps them). */
+int rxgpu_ivf_assign(const rxgpu_index*, uint64_t n, const float* vecs /* n x dim, host */, const float* norm_coefs, uint32_t* out_list_nos,
+					 float* out_dist);
+/* rxgpu_ivf_assign followed by rxgpu_ivf_add with those lists, all or nothing; out_list_nos (n or NULL) receives the lists, for
+ * IndexIVF::add_core on the CPU side. */
+int rxgpu_ivf_add_assign(rxgpu_index*, uint64_t n, const uint64_t* labels, const float* vecs /* n x dim, host */, const float* norm_coefs,
+						 uint32_t* out_list_nos);
+/* Host only: the sample rxgpu_ivf_train takes (subsample_training_set with rand_perm(n, seed): the first nlist x max_points_per_centroid
+ * entries when n exceeds that, else 0 .. n-1; out_sample holds min(n, nlist x max_points_per_centroid) rows or is NULL) and the input row
+ * each initial centroid copies (out_init, nlist entries: sample[perm[c]] with perm = rand_perm(sample size, seed + 1), or c when the
+ * sample size equals nlist). */
+int rxgpu_kmeans_plan(uint64_t n, uint32_t nlist, int32_t seed, int32_t max_points_per_centroid, int32_t* out_sample, int32_t* out_init);
 
 /* ---------------------------------------------------------------- ft_fast full-text merge (BM25 scoring over posting lists)
  * Replaces ft::Merger<IdCont, ft::MergeData, OffsetT>::Merge<Bm25Rx|Bm25Classic|TermCount>  core/ft/ft_fast/mergerimpl.h:466-566

@@ -90,6 +90,14 @@ class FtStats(C.Structure):
 FT_MERGE_INFO_DTYPE = np.dtype([("id", np.int32), ("proc", np.float32), ("field", np.uint8), ("normalized_proc", np.uint8)], align=True)
 
 
+class IvfTrainParams(C.Structure):
+    _fields_ = [("niter", C.c_int32), ("seed", C.c_int32), ("max_points_per_centroid", C.c_int32)]
+
+
+class IvfTrainStats(C.Structure):
+    _fields_ = [("obj", C.c_double), ("nsplit", C.c_int32), ("assign_ms", C.c_float), ("update_ms", C.c_float), ("host_ms", C.c_float)]
+
+
 class SearchStats(C.Structure):
     _fields_ = [("launches", C.c_uint32), ("passes", C.c_uint32), ("query_tile", C.c_uint32), ("tie_replays", C.c_uint32), ("tie_from_lists", C.c_uint32),
                 ("algorithmic_bytes", C.c_uint64), ("scan_launches", C.c_uint32), ("scan_kernel_ms", C.c_float),
@@ -167,6 +175,10 @@ _SIGNATURES = {
     "rxgpu_sq8_search_knn": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, _f32p, C.c_uint32, _f32p, _u64p, _u32p]),
     "rxgpu_hnsw_search_knn_sq8": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, _f32p, C.c_uint32, C.c_uint32, _f32p, _u64p, _u32p, _u32p]),
     "rxgpu_ivf_import": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, _u64p]),
+    "rxgpu_ivf_train": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint64, _f32p, _f32p, C.POINTER(IvfTrainParams), _f32p, C.POINTER(IvfTrainStats)]),
+    "rxgpu_ivf_assign": (C.c_int, [C.c_void_p, C.c_uint64, _f32p, _f32p, _u32p, _f32p]),
+    "rxgpu_ivf_add_assign": (C.c_int, [C.c_void_p, C.c_uint64, _u64p, _f32p, _f32p, _u32p]),
+    "rxgpu_kmeans_plan": (C.c_int, [C.c_uint64, C.c_uint32, C.c_int32, C.c_int32, _i32p, _i32p]),
     "rxgpu_ivf_search_knn": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, C.c_uint32, C.c_uint32, _f32p, _u64p, _u32p]),
     "rxgpu_ivf_search_knn_large_k": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, C.c_uint32, C.c_uint32, _f32p, _u64p, _u32p]),
     "rxgpu_ivf_search_range": (C.c_int, [C.c_void_p, _f32p, C.c_float, C.c_uint32, C.c_uint64, _f32p, _u64p, C.POINTER(C.c_uint64)]),
@@ -394,6 +406,39 @@ class GpuBruteforceSearch:
         v = np.ascontiguousarray(vecs, np.float32).reshape(-1, self.dim)
         assert len(ln) == len(lb) == len(v)
         _check(self._lib.rxgpu_ivf_add(self._h, len(ln), _p(ln, _u32p), _p(lb, _u64p), _p(v, _f32p)))
+
+    def ivf_train(self, nlist: int, vecs, norm_coefs=None, niter: int = 10, seed: int = 1234, max_points_per_centroid: int = 256):
+        """k-means on the device (rxgpu_ivf_train); leaves empty lists over the trained centroids, as ivf_create does.
+        Returns (centroids [nlist, dim], per-iteration stats: a list of dicts obj / nsplit / assign_ms / update_ms / host_ms)"""
+        v = np.ascontiguousarray(vecs, np.float32).reshape(-1, self.dim)
+        nc = None if norm_coefs is None else np.ascontiguousarray(norm_coefs, np.float32)
+        prm = IvfTrainParams(niter, seed, max_points_per_centroid)
+        cent = np.zeros((max(nlist, 1), self.dim), np.float32)
+        st = (IvfTrainStats * max(niter, 1))()
+        _check(self._lib.rxgpu_ivf_train(self._h, nlist, len(v), _p(v, _f32p), None if nc is None else _p(nc, _f32p), C.byref(prm),
+                                         _p(cent, _f32p), st))
+        stats = [{f: getattr(st[i], f) for f, _ in IvfTrainStats._fields_} for i in range(max(niter, 0))]
+        return cent[:nlist], stats
+
+    def ivf_assign(self, vecs, norm_coefs=None):
+        """quantizer->assign on the device (rxgpu_ivf_assign): (list numbers, distances in map space)"""
+        v = np.ascontiguousarray(vecs, np.float32).reshape(-1, self.dim)
+        nc = None if norm_coefs is None else np.ascontiguousarray(norm_coefs, np.float32)
+        ln = np.zeros(max(len(v), 1), np.uint32)
+        d = np.zeros(max(len(v), 1), np.float32)
+        _check(self._lib.rxgpu_ivf_assign(self._h, len(v), _p(v, _f32p), None if nc is None else _p(nc, _f32p), _p(ln, _u32p), _p(d, _f32p)))
+        return ln[:len(v)], d[:len(v)]
+
+    def ivf_add_assign(self, labels, vecs, norm_coefs=None):
+        """ivf_assign then ivf_add with those lists (rxgpu_ivf_add_assign), all or nothing; returns the list numbers"""
+        lb = np.ascontiguousarray(labels, np.uint64)
+        v = np.ascontiguousarray(vecs, np.float32).reshape(-1, self.dim)
+        assert len(lb) == len(v)
+        nc = None if norm_coefs is None else np.ascontiguousarray(norm_coefs, np.float32)
+        ln = np.zeros(max(len(v), 1), np.uint32)
+        _check(self._lib.rxgpu_ivf_add_assign(self._h, len(v), _p(lb, _u64p), _p(v, _f32p), None if nc is None else _p(nc, _f32p),
+                                              _p(ln, _u32p)))
+        return ln[:len(v)]
 
     def ivf_remove(self, label: int):
         _check(self._lib.rxgpu_ivf_remove(self._h, int(label)))
@@ -879,6 +924,15 @@ class GpuFtIndex:
         s = FtStats()
         self._lib.rxgpu_ft_last_stats(C.byref(s))
         return {f: getattr(s, f) for f, _ in FtStats._fields_}
+
+
+def kmeans_plan(n: int, nlist: int, seed: int = 1234, max_points_per_centroid: int = 256):
+    """host only: (sample, init) of rxgpu_ivf_train -- the input rows it trains on and the input row each initial centroid copies"""
+    ns = min(n, nlist * max_points_per_centroid)
+    sample = np.zeros(max(ns, 1), np.int32)
+    init = np.zeros(max(nlist, 1), np.int32)
+    _check(lib().rxgpu_kmeans_plan(n, nlist, seed, max_points_per_centroid, _p(sample, _i32p), _p(init, _i32p)))
+    return sample[:ns], init[:nlist]
 
 
 def ft_decode_packed(data, count: int):

@@ -354,6 +354,23 @@ cudaError_t scatterRows(const float* staged, const uint32_t* dst, const uint64_t
 int scanRangeHits(const rxgpu_index* ix, cudaStream_t st, ScanArgs a, DevBuf<uint64_t>& d_keys, DevBuf<unsigned long long>& d_count,
 				  PinBuf<uint64_t>& h_keys, const uint64_t* h_labels, std::vector<Hit>& res, uint32_t& scans);
 
+// ivf.cu -- the coarse quantiser of the attached IVF lists, for the k-means assignment (ivf_train.cu): errLogic as the searches report it
+// when no lists are attached or the index changed since
+struct IvfCentroids {
+	const float* centroids;  // [nlist][pitch]
+	const float* cnorm;      // Cosine: 1/||centroid||, else nullptr
+	uint32_t nlist;
+	bool own;                // lists made by rxgpu_ivf_create
+};
+int ivfCentroids(const rxgpu_index* ix, IvfCentroids& out);
+// errParams when the coarse pass cannot stage one query of `dim` floats in shared memory
+int ivfCheckCoarseDim(uint32_t dim);
+// keys[i] = make_key(distance, centroid) of the nearest of the nlist centroids [nlist][ix->pitch] to the device row x[i] ([n][ix->dim],
+// Cosine rows normalised) under (distance, centroid id): the coarse pass's distance kernel in argmin mode, same tile and grid
+cudaError_t ivfAssignRows(const rxgpu_index* ix, const float* centroids, const float* cnorm, uint32_t nlist, const float* x, uint32_t n,
+						  uint64_t* keys, cudaStream_t st);
+constexpr uint32_t kIvfMaxCentroids = 1u << 17;  // the reference's centroids_count bound (kIvfNCentroidsMax, indexopts.cc)
+
 // writes row `idx` (== size: appends) with a new vector and label, keeping the label dictionary consistent (index.cu)
 int setRowAt(rxgpu_index* ix, uint32_t idx, uint64_t label, const float* vec);
 

@@ -92,6 +92,23 @@ struct rxgpu_ivf_device {
 };
 namespace rxgpu {
 void ivfRelease(rxgpu_ivf_device* p) { delete p; }
+int ivfCentroids(const rxgpu_index* ix, IvfCentroids& out) {
+	const rxgpu_ivf_device* h = ix->ivf;
+	if (!h) {
+		return fail(RXGPU_ERR_LOGIC, "rxgpu: no IVF lists imported into this index");
+	}
+	if (h->index_version != ix->version) {
+		return fail(RXGPU_ERR_LOGIC, "rxgpu: the index changed after the IVF lists were imported");
+	}
+	out = IvfCentroids{h->centroids.p, ix->metric == RXGPU_COS ? h->cnorm.p : nullptr, h->nlist, h->own};
+	return 0;
+}
+int ivfCheckCoarseDim(uint32_t dim) {
+	if (coarse_smem_bytes(1, dim) > kCoarseSmemMax) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: dimension exceeds the coarse quantiser's shared memory");
+	}
+	return 0;
+}
 }  // namespace rxgpu
 
 namespace {
@@ -113,10 +130,7 @@ int ivfSearchChecks(const rxgpu_index* ix, uint32_t k, uint32_t kmax, uint32_t p
 	if (nprobe > probeMax) {
 		return fail(RXGPU_ERR_PARAMS, "rxgpu: nprobe exceeds the merge fan-in (1024)");
 	}
-	if (coarse_smem_bytes(1, ix->dim) > kCoarseSmemMax) {
-		return fail(RXGPU_ERR_PARAMS, "rxgpu: dimension exceeds the coarse quantiser's shared memory");
-	}
-	return 0;
+	return ivfCheckCoarseDim(ix->dim);
 }
 
 // where the lists' rows live: in the index (rxgpu_ivf_import) or in the lists' own slab (rxgpu_ivf_create)
@@ -150,15 +164,23 @@ ScanArgs ivfScanArgs(const rxgpu_index* ix, const rxgpu_ivf_device* h, const Ivf
 	return a;
 }
 
-template <bool kIsL2, int QT>
-cudaError_t launchCoarseDist(const rxgpu_index* ix, rxgpu_ivf_device* h, dim3 grid, size_t smem, const float* queries, uint32_t cq,
-							 const float* cnorm, cudaStream_t st) {
-	if (cudaError_t e = raiseSmemCeilingOnce(ivf_coarse_dist_kernel<kIsL2, QT>, ix->device, int(kCoarseSmemMax))) {
+template <bool kIsL2, int QT, bool kArgmin = false>
+cudaError_t launchCoarseDist(const rxgpu_index* ix, const float* centroids, uint32_t nlist, dim3 grid, size_t smem, const float* queries,
+							 uint32_t cq, const float* cnorm, uint64_t* keys, cudaStream_t st) {
+	if (cudaError_t e = raiseSmemCeilingOnce(ivf_coarse_dist_kernel<kIsL2, QT, kArgmin>, ix->device, int(kCoarseSmemMax))) {
 		return e;
 	}
-	ivf_coarse_dist_kernel<kIsL2, QT><<<grid, kScanThreads, smem, st>>>(h->centroids.p, ix->pitch, ix->dim, h->nlist, queries, cq, cnorm,
-																		 h->d_keys.p);
+	ivf_coarse_dist_kernel<kIsL2, QT, kArgmin><<<grid, kScanThreads, smem, st>>>(centroids, ix->pitch, ix->dim, nlist, queries, cq, cnorm, keys);
 	return cudaGetLastError();
+}
+// the coarse pass's query tile for a batch of nq, and its grid over tiles x centroid slices: query tiles fastest, so the CTAs in flight
+// share centroid slices through L2; about 4 CTAs per SM over the whole grid
+int coarseTile(const rxgpu_index* ix, uint32_t nq) { return nq > 1 && coarse_smem_bytes(kCoarseTile, ix->dim) <= kCoarseSmemMax ? kCoarseTile : 1; }
+dim3 coarseGrid(const rxgpu_index* ix, uint32_t nlist, uint32_t cq, int qt) {
+	const uint32_t groups = (nlist + kCoarseRows - 1) / kCoarseRows;
+	const uint32_t tiles = (cq + qt - 1) / qt;
+	const uint32_t slices = std::max(1u, std::min((groups + kScanWarps - 1) / kScanWarps, (uint32_t(ix->sm_count) * 4 + tiles - 1) / tiles));
+	return dim3(tiles, slices);
 }
 // the coarse quantiser (ivf_coarse.cuh) over nq host queries, staged in h->d_q: work items of the list scans in h->d_work, probe-major.
 // Per query chunk of at most kIvfKeyCap keys: distances, select, sort, emit (4 launches, counted in g_stats with the centroid bytes, read
@@ -169,7 +191,7 @@ int ivfLaunchCoarse(const rxgpu_index* ix, rxgpu_ivf_device* h, uint32_t nq, con
 	RX_CUDA(h->d_q.ensure(size_t(nq) * ix->dim));
 	RX_CUDA(h->d_work.ensure(size_t(nq) * nprobe));
 	RX_CUDA(cudaMemcpyAsync(h->d_q.p, queries, size_t(nq) * ix->dim * 4, cudaMemcpyHostToDevice, st));
-	const int qt = nq > 1 && coarse_smem_bytes(kCoarseTile, ix->dim) <= kCoarseSmemMax ? kCoarseTile : 1;
+	const int qt = coarseTile(ix, nq);
 	const size_t smem = coarse_smem_bytes(qt, ix->dim);
 	const uint32_t chunk = uint32_t(std::max<uint64_t>(1, kIvfKeyCap / nlist));
 	const uint32_t cqMax = std::min(nq, chunk);
@@ -178,20 +200,19 @@ int ivfLaunchCoarse(const rxgpu_index* ix, rxgpu_ivf_device* h, uint32_t nq, con
 	RX_CUDA(h->d_seg_begin.ensure(cqMax));
 	RX_CUDA(h->d_seg_end.ensure(cqMax));
 	const float* cnorm = ix->metric == RXGPU_COS ? h->cnorm.p : nullptr;
-	const uint32_t groups = (nlist + kCoarseRows - 1) / kCoarseRows;
 	for (uint32_t q0 = 0; q0 < nq; q0 += chunk) {
 		const uint32_t cq = std::min(chunk, nq - q0);
-		const uint32_t tiles = (cq + qt - 1) / qt;
-		// query tiles fastest: the CTAs in flight share centroid slices through L2; about 4 CTAs per SM over the whole grid
-		const uint32_t slices = std::max(1u, std::min((groups + kScanWarps - 1) / kScanWarps, (uint32_t(ix->sm_count) * 4 + tiles - 1) / tiles));
-		const dim3 grid(tiles, slices);
+		const dim3 grid = coarseGrid(ix, nlist, cq, qt);
+		const uint32_t tiles = grid.x;
 		const float* qs = h->d_q.p + size_t(q0) * ix->dim;
+		const float* cp = h->centroids.p;
+		uint64_t* keys = h->d_keys.p;
 		if (ix->metric == RXGPU_L2) {
-			RX_CUDA(qt == 1 ? (launchCoarseDist<true, 1>(ix, h, grid, smem, qs, cq, cnorm, st))
-							: (launchCoarseDist<true, kCoarseTile>(ix, h, grid, smem, qs, cq, cnorm, st)));
+			RX_CUDA(qt == 1 ? (launchCoarseDist<true, 1>(ix, cp, nlist, grid, smem, qs, cq, cnorm, keys, st))
+							: (launchCoarseDist<true, kCoarseTile>(ix, cp, nlist, grid, smem, qs, cq, cnorm, keys, st)));
 		} else {
-			RX_CUDA(qt == 1 ? (launchCoarseDist<false, 1>(ix, h, grid, smem, qs, cq, cnorm, st))
-							: (launchCoarseDist<false, kCoarseTile>(ix, h, grid, smem, qs, cq, cnorm, st)));
+			RX_CUDA(qt == 1 ? (launchCoarseDist<false, 1>(ix, cp, nlist, grid, smem, qs, cq, cnorm, keys, st))
+							: (launchCoarseDist<false, kCoarseTile>(ix, cp, nlist, grid, smem, qs, cq, cnorm, keys, st)));
 		}
 		ivf_coarse_select_kernel<<<cq, kIvfSelThreads, 0, st>>>(h->d_keys.p, nlist, nprobe, h->d_sel_label.p, h->d_seg_begin.p, h->d_seg_end.p);
 		RX_CUDA(cudaGetLastError());
@@ -279,6 +300,24 @@ int ivfSortSurvivors(rxgpu_ivf_device* h, int n, int nseg, int* begin, int* end,
 	return 0;
 }
 }  // namespace
+
+namespace rxgpu {
+cudaError_t ivfAssignRows(const rxgpu_index* ix, const float* centroids, const float* cnorm, uint32_t nlist, const float* x, uint32_t n,
+						  uint64_t* keys, cudaStream_t st) {
+	if (cudaError_t e = cudaMemsetAsync(keys, 0xFF, size_t(n) * 8, st)) {
+		return e;
+	}
+	const int qt = coarseTile(ix, n);
+	const size_t smem = coarse_smem_bytes(qt, ix->dim);
+	const dim3 grid = coarseGrid(ix, nlist, n, qt);
+	if (ix->metric == RXGPU_L2) {
+		return qt == 1 ? launchCoarseDist<true, 1, true>(ix, centroids, nlist, grid, smem, x, n, cnorm, keys, st)
+					   : launchCoarseDist<true, kCoarseTile, true>(ix, centroids, nlist, grid, smem, x, n, cnorm, keys, st);
+	}
+	return qt == 1 ? launchCoarseDist<false, 1, true>(ix, centroids, nlist, grid, smem, x, n, cnorm, keys, st)
+				   : launchCoarseDist<false, kCoarseTile, true>(ix, centroids, nlist, grid, smem, x, n, cnorm, keys, st);
+}
+}  // namespace rxgpu
 
 extern "C" {
 

@@ -21,12 +21,13 @@ namespace rxgpu {
 constexpr int kCoarseRows = 4;          // centroids per warp step: each staged query float4 feeds 4 rows
 constexpr int kCoarseTile = 16;         // queries per tile of a batch
 constexpr size_t kCoarseSmemMax = 200 * 1024;
-constexpr uint32_t kIvfMaxCentroids = 1u << 17;  // the reference's centroids_count bound (kIvfNCentroidsMax, indexopts.cc)
 
 // shared memory of a query tile of qt queries, zero padded to whole 128-float chunks
 __host__ __device__ inline size_t coarse_smem_bytes(int qt, uint32_t dim) { return size_t(qt) * ((dim + 127u) / 128u) * 512u; }
 
-template <bool kIsL2, int QT>
+// kArgmin (k-means assignment, rxgpu_ivf_train / rxgpu_ivf_assign): instead of every key, the query's smallest key goes to keys[query]
+// through a 64-bit atomicMin over the CTAs of its centroid slices (order-independent, so deterministic; keys preset to kKeyNone)
+template <bool kIsL2, int QT, bool kArgmin = false>
 __global__ void __launch_bounds__(kScanThreads, 2) ivf_coarse_dist_kernel(const float* centroids, uint32_t pitch, uint32_t dim, uint32_t nlist,
 																		   const float* queries, uint32_t cq, const float* centroid_norm_coefs,
 																		   uint64_t* keys) {
@@ -54,6 +55,7 @@ __global__ void __launch_bounds__(kScanThreads, 2) ivf_coarse_dist_kernel(const 
 	}
 	const float4* rows4 = reinterpret_cast<const float4*>(centroids);
 	const uint32_t ngroups = (nlist + kCoarseRows - 1) / kCoarseRows;
+	uint64_t best = kKeyNone;  // kArgmin: lane j < QT keeps the best key of query j over this warp's centroids
 	for (uint32_t g = blockIdx.y * kScanWarps + warp; g < ngroups; g += gridDim.y * kScanWarps) {
 		uint32_t row[kCoarseRows];
 #pragma unroll
@@ -63,16 +65,35 @@ __global__ void __launch_bounds__(kScanThreads, 2) ivf_coarse_dist_kernel(const 
 		float d[kCoarseRows][QT];
 		// IndexFlatCosine: knn_cosine = IP * norm coefficient of the centroid
 		row_dists_warp<kIsL2, kCoarseRows, QT>(rows4, pitch4, nch, row, q4, centroid_norm_coefs, lane, d);
-		// every lane holds every distance: lane l writes slots l, l + 32, ... of the (query, row) pairs, rows fastest
+		if constexpr (kArgmin) {
 #pragma unroll
-		for (int j = 0; j < QT; ++j) {
+			for (int j = 0; j < QT; ++j) {
 #pragma unroll
-			for (int r = 0; r < kCoarseRows; ++r) {
-				const uint32_t c = g * kCoarseRows + r;
-				if (((j * kCoarseRows + r) & 31) == lane && c < nlist && t0 + j < cq) {
-					keys[size_t(t0 + j) * nlist + c] = make_key(d[r][j], c);
+				for (int r = 0; r < kCoarseRows; ++r) {
+					const uint32_t c = g * kCoarseRows + r;
+					if (j == lane && c < nlist) {
+						best = min(best, make_key(d[r][j], c));
+					}
 				}
 			}
+		} else {
+			// every lane holds every distance: lane l writes slots l, l + 32, ... of the (query, row) pairs, rows fastest
+#pragma unroll
+			for (int j = 0; j < QT; ++j) {
+#pragma unroll
+				for (int r = 0; r < kCoarseRows; ++r) {
+					const uint32_t c = g * kCoarseRows + r;
+					if (((j * kCoarseRows + r) & 31) == lane && c < nlist && t0 + j < cq) {
+						keys[size_t(t0 + j) * nlist + c] = make_key(d[r][j], c);
+					}
+				}
+			}
+		}
+	}
+	if constexpr (kArgmin) {
+		static_assert(QT <= 32, "one lane per query of the tile");
+		if (lane < QT && t0 + lane < cq && best != kKeyNone) {
+			atomicMin(reinterpret_cast<unsigned long long*>(keys) + t0 + lane, static_cast<unsigned long long>(best));
 		}
 	}
 }

@@ -5,7 +5,9 @@
 //   search(1, key, k, dists, ids, &IVFSearchParameters{nprobe})      range_search(1, key, radius, &result, &params)
 //   add_with_ids(1, vec[, norm], &id)                                 remove_ids(IDSelectorArray{1, &id})
 // -- are served by librxgpu (include/rxgpu.h: rxgpu_ivf_create / _add / _remove / _search_knn_large_k / _search_range, and
-// _search_range_batch for range_search with n > 1).  The device lists are filled once, from the trained index, by the first search; after that every upsert / delete patches them in place (the list number
+// _search_range_batch for range_search with n > 1).  The device lists are filled once, from the trained index, by the first search, or
+// built on the device together with the CPU index by TrainAndFill (rxgpu_ivf_train / _add_assign); after that every upsert / delete
+// patches them in place (the list number
 // is read back from FAISS' direct map, so both sides agree on the assignment bit for bit).  Distances follow FAISS' conventions
 // (L2: squared distance ascending; inner product / cosine: +similarity descending, labels -1 past the end).
 // Meant to be dropped into cpp_src/core/index/float_vector/; compiled only where the reference tree is available
@@ -24,6 +26,7 @@
 #include "faiss/impl/IDSelector.h"
 #include "faiss/invlists/DirectMap.h"
 #include "rxgpu.h"
+#include "tools/normalize.h"
 
 namespace reindexer {
 
@@ -153,6 +156,52 @@ public:
 				result->distances[result->lims[q] + i] = similarity ? -d[q][i] : d[q][i];
 			}
 		}
+	}
+
+	// Building the index on the device -- replaces IvfIndex::trainIdx followed by add_with_ids of every row (the training upsert,
+	// ivf_index.cc:97-102, and RebuildCentroids, :671-679): `idx` is the new, untrained IndexIVFFlat over its empty quantizer.  The
+	// centroids are trained on the first `ntrain` rows (all n by default; RebuildCentroids trains on a part) by rxgpu_ivf_train with
+	// idx.cp's niter / seed / max_points_per_centroid, added to idx.quantizer, and both are marked trained; every row is then assigned
+	// on the device (rxgpu_ivf_add_assign) and its list handed to idx.add_core, so FAISS's lists and the device's are the same by
+	// construction.  This map then owns idx and keeps the device index it built: the next search needs no import.  Cosine: norms are
+	// the rows' norm coefficients as IvfIndex passes them, or NULL (computed here as add_with_ids does).  Throws on any error, leaving
+	// this map as it was.
+	void TrainAndFill(std::unique_ptr<faiss::IndexIVFFlat> idx, const float* x, const float* norms, size_t n, const faiss::idx_t* ids,
+					  size_t ntrain = 0) {
+		ntrain = ntrain ? ntrain : n;
+		const auto metric = idx->metric_type == faiss::METRIC_L2 ? RXGPU_L2 : idx->is_cosine ? RXGPU_COS : RXGPU_IP;
+		const size_t dim = size_t(idx->d), nlist = idx->nlist;
+		if (idx->direct_map.type != faiss::DirectMap::Type::Hashtable) {
+			idx->set_direct_map_type(faiss::DirectMap::Type::Hashtable);  // as IvfIndex::trainIdx sets it
+		}
+		rxgpu_index* ix = nullptr;
+		check(rxgpu_index_create(&ix, metric, uint32_t(dim), 16, deviceFromEnv(), 0));
+		std::unique_ptr<rxgpu_index, void (*)(rxgpu_index*)> guard(ix, rxgpu_index_destroy);
+		const rxgpu_ivf_train_params prm{int32_t(idx->cp.niter), int32_t(idx->cp.seed), int32_t(idx->cp.max_points_per_centroid)};
+		std::vector<float> centroids(nlist * dim);
+		check(rxgpu_ivf_train(ix, uint32_t(nlist), uint64_t(ntrain), x, norms, &prm, centroids.data(), nullptr));
+		idx->quantizer->reset();
+		idx->quantizer->add(faiss::idx_t(nlist), centroids.data());  // IndexFlatCosine computes the centroids' norm coefficients here
+		idx->quantizer->is_trained = true;
+		idx->is_trained = true;
+		std::vector<uint64_t> labels(ids, ids + n);
+		std::vector<uint32_t> lists(n);
+		check(rxgpu_ivf_add_assign(ix, uint64_t(n), labels.data(), x, norms, lists.data()));
+		std::vector<float> coefs;
+		if (metric == RXGPU_COS && !norms) {  // IndexIVF::add_with_ids without norms: the coefficients of NormalizeVector
+			coefs.resize(n);
+			std::vector<float> row(dim);
+			for (size_t i = 0; i < n; ++i) {
+				coefs[i] = reindexer::ann::NormalizeCopyVector(x + i * dim, int32_t(dim), row.data());
+			}
+			norms = coefs.data();
+		}
+		const std::vector<faiss::idx_t> listNos(lists.begin(), lists.end());
+		idx->add_core(faiss::idx_t(n), x, metric == RXGPU_COS ? norms : nullptr, ids, listNos.data());
+		std::lock_guard<std::mutex> lck(mtx_);
+		releaseDevice();
+		cpu_ = std::move(idx);
+		gpu_ = guard.release();
 	}
 
 	size_t DeviceImports() const noexcept { return imports_; }
