@@ -606,6 +606,20 @@ int rxgpu_set_profile(int on);
  * blocks of 128 are served, in the cluster shape the index's rxgpu_set_tensor_core_filter mode picks.  A mode other than 0 is refused (RXGPU_ERR_LOGIC) unless the environment has
  * RXGPU_TC_DIAG=1, and a search a diagnostic instantiation answered reports tc_kernel = 1 + mode in its statistics. */
 int rxgpu_tc_diag(int mode, void* d_counters);
+/* tests only: the int8 filter's certificate, read back.  Brings the index's int8 shadow up to date (as a large-batch search would;
+ * nothing else changes) and writes, for nq queries with thresholds tau[nq] (map space, as a range radius) tested in query blocks of
+ * query_block (32, 64, 96 or 128) queries, what the filter's consumers and bookkeepers compute (knn_tc.cuh):
+ *   out_shape[2]                 the shadow's slots S and its 64-slot blocks B (whole 128-slot tiles)
+ *   slot_row[S]                  the row of every slot (0xFFFFFFFF: dead)        rowc[S][4]  (s_v, r_v, n_v, c_v)
+ *   blockc[B][8]                 tc_block_consts' record of every block
+ *   row_codes[S][dim]            the int8 codes of every slot, un-swizzled       query_codes[nq][dim], qc[nq][4]: tc_prepare_queries
+ *   kab[nq / query_block][2]     (ka, kb) of every query block
+ *   block_thr[nq][B]             tc_block_threshold of every (query, block)
+ *   row_bound[nq][S][2]          (d~, err) of tc_row_bound with x = float(I), I = the int32 dot product of the codes
+ * Call it once with every array null to learn S and B.  Any output but out_shape may be null. */
+int rxgpu_tc_audit(const rxgpu_index*, uint32_t nq, const float* queries, const float* tau, uint32_t query_block, uint32_t* out_shape,
+                   uint32_t* slot_row, float* rowc, float* blockc, signed char* row_codes, signed char* query_codes, float* qc, float* kab,
+                   int32_t* block_thr, float* row_bound);
 
 #ifdef __cplusplus
 }

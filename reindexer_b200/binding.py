@@ -209,6 +209,8 @@ _SIGNATURES = {
     "rxgpu_last_search_stats": (None, [C.POINTER(SearchStats)]),
     "rxgpu_set_profile": (C.c_int, [C.c_int]),
     "rxgpu_tc_diag": (C.c_int, [C.c_int, C.c_void_p]),
+    "rxgpu_tc_audit": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, _f32p, C.c_uint32, _u32p, _u32p, _f32p, _f32p, C.c_void_p, C.c_void_p, _f32p,
+                                 _f32p, _i32p, _f32p]),
     "rxgpu_set_tensor_core_filter": (C.c_int, [C.c_void_p, C.c_int]),
 }
 
@@ -642,6 +644,32 @@ class GpuBruteforceSearch:
         """0 = auto, 1 = whenever possible, 2 = never (exact fp32 scan only); 3 / 4 / 5 = as 1 in single CTAs / clusters of up to
         two / clusters of up to four CTAs that share every row tile (0 and 1: clusters of up to two on >= 2^23 rows)"""
         _check(self._lib.rxgpu_set_tensor_core_filter(self._h, mode))
+
+    def tc_audit(self, queries, tau, query_block: int = 128, row_bound: bool = True) -> dict:
+        """rxgpu_tc_audit: the int8 filter's certificate for these queries at thresholds tau (map space, a scalar or [nq]), as
+        host arrays: slot_row [S], rowc [S, 4], blockc [B, 8], row_codes [S, dim], query_codes [nq, dim], qc [nq, 4],
+        kab [query blocks, 2], block_thr [nq, B] and, with row_bound, row_bound [nq, S, 2] = (d~, err)."""
+        q = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, self.dim)
+        nq = q.shape[0]
+        t = np.ascontiguousarray(np.broadcast_to(np.asarray(tau, dtype=np.float32), (nq,)))
+        shape = np.zeros(2, np.uint32)
+        _check(self._lib.rxgpu_tc_audit(self._h, 0, None, None, query_block, _p(shape, _u32p), *([None] * 9)))
+        S, B = int(shape[0]), int(shape[1])
+        o = {"slot_row": np.zeros(max(S, 1), np.uint32), "rowc": np.zeros((max(S, 1), 4), np.float32),
+             "blockc": np.zeros((max(B, 1), 8), np.float32), "row_codes": np.zeros((max(S, 1), self.dim), np.int8),
+             "query_codes": np.zeros((max(nq, 1), self.dim), np.int8), "qc": np.zeros((max(nq, 1), 4), np.float32),
+             "kab": np.zeros((max((nq + query_block - 1) // query_block, 1), 2), np.float32),
+             "block_thr": np.zeros((max(nq, 1), max(B, 1)), np.int32),
+             "row_bound": np.zeros((max(nq, 1), max(S, 1), 2), np.float32) if row_bound and S else None}
+        _check(self._lib.rxgpu_tc_audit(self._h, nq, _p(q, _f32p), _p(t, _f32p), query_block, _p(shape, _u32p), _p(o["slot_row"], _u32p),
+                                        _p(o["rowc"], _f32p), _p(o["blockc"], _f32p), o["row_codes"].ctypes.data,
+                                        o["query_codes"].ctypes.data, _p(o["qc"], _f32p), _p(o["kab"], _f32p), _p(o["block_thr"], _i32p),
+                                        None if o["row_bound"] is None else _p(o["row_bound"], _f32p)))
+        nqb = (nq + query_block - 1) // query_block
+        out = {"slot_row": o["slot_row"][:S], "rowc": o["rowc"][:S], "blockc": o["blockc"][:B], "row_codes": o["row_codes"][:S],
+               "query_codes": o["query_codes"][:nq], "qc": o["qc"][:nq], "kab": o["kab"][:nqb], "block_thr": o["block_thr"][:nq, :B],
+               "row_bound": None if o["row_bound"] is None else o["row_bound"][:nq, :S]}
+        return out
 
 
 COMM_ID_BYTES = 128

@@ -1547,6 +1547,90 @@ int rxgpu_tc_diag(int mode, void* d_counters) {
 	g_tc_diag.store(mode);
 	return 0;
 }
+int rxgpu_tc_audit(const rxgpu_index* ix, uint32_t nq, const float* queries, const float* tau, uint32_t query_block, uint32_t* out_shape,
+				   uint32_t* slot_row, float* rowc, float* blockc, signed char* row_codes, signed char* query_codes, float* qc, float* kab,
+				   int32_t* block_thr, float* row_bound) {
+	if (int rc = checkIndex(ix)) {
+		return rc;
+	}
+	if (!out_shape || (nq && (!queries || !tau)) || query_block == 0 || query_block > kTcMaxNq || query_block % 32) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: audit needs the shape output, queries with their thresholds and a query block of 32..128");
+	}
+	RX_CUDA(cudaSetDevice(ix->device));
+	cudaStream_t st = ix->stream;
+	if (int rc = ensureShadow(ix, st)) {
+		return rc;
+	}
+	const uint32_t pitch = ix->pitch_q, kchunks = pitch / kTcChunkK, dim = ix->dim, slots = ix->shadow_slots;
+	const uint32_t nblocks = uint32_t((uint64_t(slots) + kTcTileRows - 1) / kTcTileRows * kTcTileRows / 64);  // as the filter walks them
+	const uint32_t nqblocks = (nq + query_block - 1) / query_block;
+	out_shape[0] = slots;
+	out_shape[1] = nblocks;
+	auto fetch = [&](void* dst, const void* src, size_t bytes) -> cudaError_t {
+		return dst && bytes ? cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost) : cudaSuccess;
+	};
+	RX_CUDA(fetch(slot_row, ix->d_slot_row, size_t(slots) * 4));
+	RX_CUDA(fetch(rowc, ix->d_rowc, size_t(slots) * sizeof(float4)));
+	RX_CUDA(fetch(blockc, ix->d_blockc, size_t(nblocks) * 2 * sizeof(float4)));
+	// the row codes by slot, un-swizzled (tc_convert_rows' layout): [64-slot block][K chunk][64 slots x 128 B]
+	std::vector<signed char> sh(size_t(nblocks) * 64 * pitch), codes(size_t(nblocks) * 64 * pitch);
+	RX_CUDA(fetch(sh.data(), ix->d_shadow, sh.size()));
+	for (uint32_t s = 0; s < nblocks * 64; ++s) {
+		const uint32_t blk = s / 64, r = s % 64;
+		for (uint32_t c = 0; c < pitch; c += 16) {
+			const uint32_t kc = c / kTcChunkK, unit = ((c % kTcChunkK) >> 4) ^ (r & 7u);
+			std::memcpy(&codes[size_t(s) * pitch + c], &sh[(size_t(blk) * kchunks + kc) * kTcBlockBytes + r * 128u + unit * 16u], 16);
+		}
+	}
+	if (row_codes) {
+		for (uint32_t s = 0; s < slots; ++s) {
+			std::memcpy(row_codes + size_t(s) * dim, &codes[size_t(s) * pitch], dim);
+		}
+	}
+	if (nq == 0) {
+		return 0;
+	}
+	DevBuf<float> d_q, d_qf, d_tau;
+	DevBuf<unsigned char> d_qcodes;
+	DevBuf<signed char> d_rcodes;
+	DevBuf<float4> d_qc;
+	DevBuf<float2> d_kab, d_bound;
+	DevBuf<int> d_thr;
+	RX_CUDA(d_q.ensure(size_t(nq) * dim));
+	RX_CUDA(d_qf.ensure(size_t(nq) * pitch));
+	RX_CUDA(d_tau.ensure(nq));
+	RX_CUDA(d_qcodes.ensure(size_t(nq) * pitch));
+	RX_CUDA(d_qc.ensure(nq));
+	RX_CUDA(d_kab.ensure(nqblocks));
+	RX_CUDA(d_thr.ensure(std::max<size_t>(size_t(nq) * nblocks, 1)));
+	RX_CUDA(cudaMemcpyAsync(d_q.p, queries, size_t(nq) * dim * 4, cudaMemcpyHostToDevice, st));
+	RX_CUDA(cudaMemcpyAsync(d_tau.p, tau, size_t(nq) * 4, cudaMemcpyHostToDevice, st));
+	tc_prepare_queries<<<(nq * 32 + 255) / 256, 256, 0, st>>>(d_q.p, nq, nq, dim, pitch, d_qcodes.p, d_qc.p, d_qf.p);
+	tc_audit_thresholds<<<nqblocks, 256, 0, st>>>(d_qc.p, d_tau.p, nq, query_block, dim, ix->metric, ix->d_blockc, nblocks, d_kab.p, d_thr.p);
+	if (row_bound && slots) {
+		RX_CUDA(d_rcodes.ensure(size_t(slots) * pitch));
+		RX_CUDA(d_bound.ensure(size_t(nq) * slots));
+		RX_CUDA(cudaMemcpyAsync(d_rcodes.p, codes.data(), size_t(slots) * pitch, cudaMemcpyHostToDevice, st));
+		tc_audit_bounds<<<dim3((slots + 255) / 256, nq), 256, 0, st>>>(reinterpret_cast<const signed char*>(d_qcodes.p), d_qc.p, d_rcodes.p,
+																		ix->d_rowc, pitch, slots, dim, ix->metric, d_bound.p);
+	}
+	RX_CUDA(cudaGetLastError());
+	RX_CUDA(cudaStreamSynchronize(st));
+	if (query_codes) {
+		std::vector<signed char> qcodes(size_t(nq) * pitch);
+		RX_CUDA(fetch(qcodes.data(), d_qcodes.p, qcodes.size()));
+		for (uint32_t q = 0; q < nq; ++q) {
+			std::memcpy(query_codes + size_t(q) * dim, &qcodes[size_t(q) * pitch], dim);
+		}
+	}
+	RX_CUDA(fetch(qc, d_qc.p, size_t(nq) * sizeof(float4)));
+	RX_CUDA(fetch(kab, d_kab.p, size_t(nqblocks) * sizeof(float2)));
+	RX_CUDA(fetch(block_thr, d_thr.p, size_t(nq) * nblocks * 4));
+	if (row_bound && slots) {
+		RX_CUDA(fetch(row_bound, d_bound.p, size_t(nq) * slots * sizeof(float2)));
+	}
+	return 0;
+}
 int rxgpu_set_profile(int on) {
 	g_profile.store(on ? 1 : 0);
 	return 0;

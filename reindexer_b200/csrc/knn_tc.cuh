@@ -19,6 +19,11 @@
 //   L2      d~ = n_q^2 + n_v^2 - 2p,  lb/ub = d~ -+ (2e + eps (n_q^2 + n_v^2)),  eps = kTcL2Eps + (D + 1) 2^-23 (the exact scan's sum
 //                                                                                  of squares and the rounding of d~ itself)
 // For sigma = 0.25 rows at 768 dims r_v / n_v is about 0.7 %, so e is about 0.015 n_q n_v.
+// These relative bounds assume no fp32 underflow.  Below FLT_MIN every rounding of the exact scan's sum and of s_q s_v is absolute,
+// up to D 2^-149 in all, which the relative terms cover only while n_q n_v (L2: n_q^2 + n_v^2) stays above about D 2^-142.  A pair
+// below kTcTinyNorm2 = 2^-96 therefore gets err = +inf (tc_row_bound: never rejected by its own bound), and the block test passes
+// every pair of a query or a row with 0 < n < kTcTinyNorm = 2^-48 (tc_prepare_queries: 1 / k_q = +inf; tc_block_consts: flag 1), so
+// that every such pair reaches the exact re-rank.  Rows and queries that small only arise from subnormal-scale data.
 //   threshold     tau_q = the largest entry of the query's BOUND LIST: k1 EXACT distances (the exact scan's own arithmetic,
 //                 row_dists_warp) of k1 distinct rows (one small list per query in HBM, updated under a per-query lock -- only
 //                 O(k log n) successful inserts per query over a whole pass); a row is a candidate iff lb <= tau_q.  tc_init_tau
@@ -369,6 +374,17 @@ __device__ __forceinline__ int tc_block_threshold(float R, float P, float Z, flo
 	}
 	return f > 0x1p30f ? kTcPassNone : int(floorf(f));
 }
+// (a*, b*) of a query block: every thread folds the queries it holds into s_ab[2] (zeroed first) with tc_block_ab_add, and after a
+// barrier tc_block_ab_k turns the maxima into the (ka, kb) tc_block_threshold takes.  The filter and rxgpu_tc_audit both call these.
+__device__ __forceinline__ void tc_block_ab_add(float* s_ab, float4 qc, float delta) {  // qc = (s_q, r_q, n_q, 1 / k_q)
+	if (qc.z > 0.f) {  // non-negative floats order like their bit patterns
+		atomicMax(reinterpret_cast<unsigned int*>(&s_ab[0]), __float_as_uint((qc.z + qc.y) / qc.z));
+		atomicMax(reinterpret_cast<unsigned int*>(&s_ab[1]), __float_as_uint(qc.y / qc.z + delta));
+	}
+}
+__device__ __forceinline__ float2 tc_block_ab_k(const float* s_ab) {  // 2^-8 of e, and 2^-8 for the rounding of M_v
+	return make_float2((1.f + 0x1p-7f) * s_ab[0], (1.f + 0x1p-7f) * s_ab[1]);
+}
 __device__ __forceinline__ float2 tc_make_pr(int metric, float tau, float4 qc, float l2eps) {  // qc = (s_q, r_q, n_q, 1 / k_q)
 	const float p = qc.z * qc.w;
 	if (metric != kL2) {
@@ -453,17 +469,21 @@ __device__ __noinline__ bool tc_enqueue_quad(TcQueue* qu, uint4* rec, uint32_t s
 	return waited;
 }
 
-// The row's own bound: d~ and its certified error (header comment), from x = float(I) and the query's and the row's constants.
+// The row's own bound: d~ and its certified error (header comment), from x = float(I) and the query's and the row's constants.  A
+// pair below kTcTinyNorm2 (header comment) gets an infinite error: its own bound never rejects it.
+constexpr float kTcTinyNorm = 0x1p-48f, kTcTinyNorm2 = 0x1p-96f;
 __device__ __forceinline__ float2 tc_row_bound(const TcArgs& a, float x, float4 qc, float4 rc) {
 	const float p = qc.x * rc.x * x;
 	const float e = (1.f + 0x1p-8f) * fmaf(qc.z + qc.y, rc.y, (qc.y + float(a.dim + 16) * 0x1p-23f * qc.z) * rc.z);
 	if (a.metric == kL2) {
-		return make_float2(fmaf(-2.f, p, fmaf(qc.z, qc.z, rc.z * rc.z)), 2.f * e + tc_l2eps(a.dim) * (qc.z * qc.z + rc.z * rc.z));
+		const float nn = qc.z * qc.z + rc.z * rc.z;
+		return make_float2(fmaf(-2.f, p, fmaf(qc.z, qc.z, rc.z * rc.z)), nn < kTcTinyNorm2 ? INFINITY : 2.f * e + tc_l2eps(a.dim) * nn);
 	}
+	const float err = qc.z * rc.z < kTcTinyNorm2 ? INFINITY : e;
 	if (a.metric == kCos) {
-		return make_float2(-p * rc.w, e * rc.w);
+		return make_float2(-p * rc.w, err * rc.w);
 	}
-	return make_float2(-p, e);
+	return make_float2(-p, err);
 }
 
 // Exact distance d of a row below the query's threshold: insert it into the query's global bound list (under the per-query lock;
@@ -709,10 +729,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		const bool valid = i < nq_valid;
 		const float thr = valid ? ord_float(a.tau[q0 + i]) : -INFINITY;
 		const float4 qc = valid ? a.qc[q0 + i] : make_float4(0.f, 0.f, 0.f, 0.f);
-		if (qc.z > 0.f) {  // non-negative floats order like their bit patterns
-			atomicMax(reinterpret_cast<unsigned int*>(&s_ab[0]), __float_as_uint((qc.z + qc.y) / qc.z));
-			atomicMax(reinterpret_cast<unsigned int*>(&s_ab[1]), __float_as_uint(qc.y / qc.z + delta));
-		}
+		tc_block_ab_add(s_ab, qc, delta);
 		s_qc[i] = qc;
 		for (int w = 0; w < kTcConsumers; ++w) {
 			s_thr[w * kNq + i] = thr;
@@ -799,7 +816,8 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 		const uint32_t my_q = wtid;  // the query whose threshold this thread refreshes from the global list and turns into block thresholds
 		unsigned int tau_ahead = my_q < nq_valid ? a.tau[q0 + my_q] : 0u;
 		const bool l2 = a.metric == kL2;
-		const float ka = (1.f + 0x1p-7f) * s_ab[0], kb = (1.f + 0x1p-7f) * s_ab[1];  // 2^-8 of e, and 2^-8 for the rounding of M_v
+		const float2 kab = tc_block_ab_k(s_ab);
+		const float ka = kab.x, kb = kab.y;
 		auto release = [&](uint32_t st) {  // this warp is done with stage st in every CTA that reads it: lane c signals CTA c
 			if constexpr (kCluster == 1) {
 				if (lane == 0) {
@@ -1449,7 +1467,7 @@ __global__ void tc_block_consts(const float4* rowc, const uint32_t* slot_row, ui
 		live = true;
 		const float4 rc = rowc[slot];  // (s, r, n, c)
 		const double S = double(rc.x) * double(rc.w);  // exact: 24 x 24 significant bits
-		if (!(S > 0.0) || !isfinite(S) || !isfinite(rc.y) || !isfinite(rc.z)) {  // NaN included
+		if (!(S > 0.0) || !isfinite(S) || !isfinite(rc.y) || !isfinite(rc.z) || rc.z < kTcTinyNorm) {  // NaN included
 			pass_all = true;
 			continue;
 		}
@@ -1598,8 +1616,59 @@ __global__ void tc_prepare_queries(const float* queries, uint32_t nq, uint32_t n
 	const float3 srn = tc_quantize(queries + size_t(q) * dim, q < nq ? dim : 0u, pitch, lane,
 								   [&](uint32_t c, uint32_t code4) { *reinterpret_cast<uint32_t*>(out + c) = code4; });
 	if (lane == 0 && q < nq) {
-		qc[q] = make_float4(srn.x, srn.y, srn.z, srn.x > 0.f ? 1.f / srn.x : 1.f);
+		// 1 / k_q = +inf for a tiny but non-zero query: its block thresholds all pass (header comment: fp32 underflow)
+		qc[q] = make_float4(srn.x, srn.y, srn.z, srn.z > 0.f && srn.z < kTcTinyNorm ? INFINITY : srn.x > 0.f ? 1.f / srn.x : 1.f);
 	}
+}
+
+// ---- the certificate's audit (rxgpu_tc_audit) ------------------------------------------------------------------------------------
+// One CTA per query block of nqb queries: its (ka, kb) as the filter's consumers compute them, then thr[q][b] = the integer threshold of
+// query q against shadow block b, from the query's threshold tau[q] (map space) exactly as a consumer turns it into its block test.
+__global__ void tc_audit_thresholds(const float4* qc, const float* tau, uint32_t nq, uint32_t nqb, uint32_t dim, int metric,
+									const float4* blockc, uint32_t nblocks, float2* kab, int* thr) {
+	__shared__ float s_ab[2];
+	const uint32_t q0 = blockIdx.x * nqb, nv = min(nqb, nq - q0);
+	if (threadIdx.x == 0) {
+		s_ab[0] = s_ab[1] = 0.f;
+	}
+	__syncthreads();
+	const float delta = float(dim + 16) * 0x1p-23f;
+	for (uint32_t i = threadIdx.x; i < nv; i += blockDim.x) {
+		tc_block_ab_add(s_ab, qc[q0 + i], delta);
+	}
+	__syncthreads();
+	const float2 k = tc_block_ab_k(s_ab);
+	if (threadIdx.x == 0) {
+		kab[blockIdx.x] = k;
+	}
+	const float l2eps = tc_l2eps(dim);
+	for (uint32_t i = threadIdx.x; i < nv * nblocks; i += blockDim.x) {
+		const uint32_t q = q0 + i / nblocks, b = i % nblocks;
+		const float4 c = qc[q];
+		const float2 pr = tc_make_pr(metric, tau[q], c, l2eps);
+		thr[size_t(q) * nblocks + b] = tc_block_threshold(pr.y, pr.x, metric == kL2 ? c.w : 0.f, k.x, k.y, blockc[2 * b], blockc[2 * b + 1]);
+	}
+}
+
+// bound[q][slot] = (d~, err) of tc_row_bound with x = float(I), I = the plain int32 dot product of the query's and the slot's codes
+// (row codes un-swizzled to [slots][pitch], query codes [nq][pitch], both zero beyond dim)
+__global__ void tc_audit_bounds(const signed char* qcodes, const float4* qc, const signed char* rcodes, const float4* rowc, uint32_t pitch,
+								uint32_t nslots, uint32_t dim, int metric, float2* bound) {
+	const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x, q = blockIdx.y;
+	if (slot >= nslots) {
+		return;
+	}
+	const char4* a = reinterpret_cast<const char4*>(qcodes + size_t(q) * pitch);
+	const char4* b = reinterpret_cast<const char4*>(rcodes + size_t(slot) * pitch);
+	int I = 0;
+	for (uint32_t i = 0; i < pitch / 4; ++i) {
+		const char4 x = a[i], y = b[i];
+		I += int(x.x) * int(y.x) + int(x.y) * int(y.y) + int(x.z) * int(y.z) + int(x.w) * int(y.w);
+	}
+	TcArgs args{};
+	args.dim = dim;
+	args.metric = metric;
+	bound[size_t(q) * nslots + slot] = tc_row_bound(args, float(I), qc[q], rowc[slot]);
 }
 
 }  // namespace rxgpu
