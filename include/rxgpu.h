@@ -271,6 +271,43 @@ uint64_t rxgpu_hnsw_update_count(const rxgpu_index*); /* nodes patched in place 
  * A search that meets more than 4096 deleted nodes waiting for expansion at once fails with errLogic (rebuild the graph). */
 int rxgpu_hnsw_mark_deleted(rxgpu_index*, uint64_t label);
 uint64_t rxgpu_hnsw_deleted_count(const rxgpu_index*); /* DeletedCountUnsafe */
+/* ---------------------------------------------------------------- HNSW graph construction on the device
+ * Replaces HierarchicalNSWImpl::addPoint (hnswalg.h:1695-1852) as the transaction path reaches it through AddPointConcurrent: rows
+ * [first, n) of the index (n = rxgpu_index_size) are inserted into the graph over rows [0, first) -- none when first == 0, else the graph
+ * of rxgpu_hnsw_import, rxgpu_hnsw_load_index_cache or an earlier build -- by a deterministic batched insertion (DESIGN.md §3.8):
+ * the batches of rxgpu_hnsw_build_plan; every row of a batch does the greedy descent, searchBaseLayer with ef = efConstruction and
+ * getNeighborsByHeuristic2 with M against the graph as the batch began; then the selected neighbours receive their reverse links, a
+ * list that overflows Mcurmax being pruned once per batch with the heuristic.  Equal distances are ordered by row id.
+ * levels: n - first levels, or NULL to draw them as getRandomLevel does (hnswalg.h:625-635): std::default_random_engine seeded with
+ * `seed` (the adapter's 100), one draw per row in row order -- with first == 0 these are the reference's element_levels_.
+ * M in [2, 32], efConstruction in [4, 1024] and a dimension the search kernel serves at that ef (errParams otherwise, and for first
+ * other than the graph's node count, a graph of another M or negative levels); errLogic when the graph has tombstones, or when a
+ * row it covers was rewritten or moved (an upsert of an existing label, a remove) since it was imported, built or patched; errSystem
+ * when the workspace does not fit.  On any error the index and its graph are unchanged.  The graph left behind is searched by every
+ * rxgpu_hnsw_* call without an import. */
+typedef struct {
+	uint64_t batches, rows;
+	uint64_t distances;      /* distance evaluations (the reference's metric_distance_computations, summed over the inserts) */
+	uint64_t reverse_links;  /* links written to the lists of the selected neighbours */
+	uint64_t lists_pruned;   /* neighbour lists pruned with the heuristic (one per overflowing list and batch) */
+	float search_select_ms;  /* CUDA-event times: the descent, searches and neighbour selection of every row */
+	float sort_ms;           /* the sort of the reverse links */
+	float link_ms;           /* appending and pruning the lists that receive them */
+} rxgpu_hnsw_build_stats;
+int rxgpu_hnsw_build(rxgpu_index*, uint32_t M, uint32_t ef_construction, uint64_t first, const int32_t* levels /* n - first or NULL */,
+					 uint64_t seed, rxgpu_hnsw_build_stats* stats /* or NULL */);
+/* The batches of rxgpu_hnsw_build, on the host: rows [first, n) onto a graph whose top level is maxlevel (-1 exactly when first == 0).
+ * out_ends[b] = the end of batch b (at most n - first of them), *out_nbatches = their number; out_levels (n - first, or NULL) = the
+ * levels used (drawn when levels is NULL, as rxgpu_hnsw_build draws them). */
+int rxgpu_hnsw_build_plan(uint32_t M, uint64_t first, uint64_t n, int32_t maxlevel, const int32_t* levels, uint64_t seed,
+						  int32_t* out_levels, uint64_t* out_ends, uint64_t* out_nbatches);
+/* Reads the device graph back in the layout of rxgpu_hnsw_graph for nodes[0, nnodes) (NULL: nodes 0 .. nnodes-1).  level0:
+ * nnodes x (1 + maxM0); levels: nnodes; upper_offsets: nnodes + 1 slots into `upper`, which receives the nodes' upper-level lists in
+ * order (upper_offsets[nnodes] x (1 + M)).  Every output may be NULL (ask for upper_offsets first to size `upper`); info (or NULL)
+ * receives n, M, maxM0, maxlevel, enterpoint and upper_slots with NULL arrays.  With nodes == NULL and nnodes == n the arrays are
+ * what rxgpu_hnsw_import takes. */
+int rxgpu_hnsw_export(const rxgpu_index*, uint64_t nnodes, const uint32_t* nodes, uint32_t* level0, int32_t* levels, int64_t* upper_offsets,
+					  uint32_t* upper, rxgpu_hnsw_graph* info);
 /* labels of n shard-local internal indices (device pointers; enqueued on `stream`): the HNSW device search returns indices, the
  * multi-GPU merge needs labels */
 int rxgpu_gather_labels_device(const rxgpu_index*, uint64_t n, const uint32_t* d_idx, uint64_t* d_out_label, void* stream);

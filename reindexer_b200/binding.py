@@ -98,6 +98,11 @@ class IvfTrainStats(C.Structure):
     _fields_ = [("obj", C.c_double), ("nsplit", C.c_int32), ("assign_ms", C.c_float), ("update_ms", C.c_float), ("host_ms", C.c_float)]
 
 
+class HnswBuildStats(C.Structure):
+    _fields_ = [("batches", C.c_uint64), ("rows", C.c_uint64), ("distances", C.c_uint64), ("reverse_links", C.c_uint64),
+                ("lists_pruned", C.c_uint64), ("search_select_ms", C.c_float), ("sort_ms", C.c_float), ("link_ms", C.c_float)]
+
+
 class SearchStats(C.Structure):
     _fields_ = [("launches", C.c_uint32), ("passes", C.c_uint32), ("query_tile", C.c_uint32), ("tie_replays", C.c_uint32), ("tie_from_lists", C.c_uint32),
                 ("algorithmic_bytes", C.c_uint64), ("scan_launches", C.c_uint32), ("scan_kernel_ms", C.c_float),
@@ -156,6 +161,9 @@ _SIGNATURES = {
     "rxgpu_gather_labels_device": (C.c_int, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rxgpu_hnsw_search_range": (C.c_int, [C.c_void_p, _f32p, C.c_float, C.c_uint32, C.c_uint64, _f32p, _u64p, C.POINTER(C.c_uint64)]),
     "rxgpu_hnsw_search_range_batch": (C.c_int, [C.c_void_p, C.c_uint32, _f32p, _f32p, C.c_uint32, C.c_uint64, _f32p, _u64p, _u64p]),
+    "rxgpu_hnsw_build": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint64, _i32p, C.c_uint64, C.POINTER(HnswBuildStats)]),
+    "rxgpu_hnsw_build_plan": (C.c_int, [C.c_uint32, C.c_uint64, C.c_uint64, C.c_int32, _i32p, C.c_uint64, _i32p, _u64p, C.POINTER(C.c_uint64)]),
+    "rxgpu_hnsw_export": (C.c_int, [C.c_void_p, C.c_uint64, _u32p, _u32p, _i32p, C.POINTER(C.c_int64), _u32p, C.POINTER(HnswGraph)]),
     "rxgpu_hnsw_search_knn_device": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.c_void_p]),
     "rxgpu_ivf_create": (C.c_int, [C.c_void_p, C.c_uint32, _f32p]),
@@ -397,6 +405,32 @@ class GpuBruteforceSearch:
         _check(self._lib.rxgpu_hnsw_search_knn(self._h, nq, _p(q, _f32p), k, ef, _p(d, _f32p), _p(l, _u64p), _p(c, _u32p),
                                                _p(st, _u32p)))
         return (d, l, c, st) if with_stats else (d, l, c)
+
+    def hnsw_build(self, M: int, ef_construction: int, first: int = 0, levels=None, seed: int = 100) -> dict:
+        """Insert rows [first, size) into the device graph (rxgpu_hnsw_build); `first` = the graph's node count (0: no graph yet).
+        levels: one per inserted row, or None to draw them like the reference's getRandomLevel.  Returns the build's stats."""
+        lv = None if levels is None else np.ascontiguousarray(levels, np.int32)
+        st = HnswBuildStats()
+        _check(self._lib.rxgpu_hnsw_build(self._h, M, ef_construction, first, None if lv is None else _p(lv, _i32p), seed, C.byref(st)))
+        return {f: getattr(st, f) for f, _ in HnswBuildStats._fields_}
+
+    def hnsw_export(self, nodes=None) -> dict:
+        """The device graph (rxgpu_hnsw_export) as a dict in the layout of hnsw_import: every node, or the nodes listed (their
+        upper-level lists then follow one another, upper_offsets indexing them)."""
+        info = HnswGraph()
+        _check(self._lib.rxgpu_hnsw_export(self._h, 0, None, None, None, None, None, C.byref(info)))
+        nd = None if nodes is None else np.ascontiguousarray(nodes, np.uint32)
+        cnt = info.n if nd is None else len(nd)
+        ndp = None if nd is None else _p(nd, _u32p)
+        offs = np.zeros(cnt + 1, np.int64)
+        levels = np.zeros(max(cnt, 1), np.int32)
+        level0 = np.zeros((max(cnt, 1), 1 + info.maxM0), np.uint32)
+        _check(self._lib.rxgpu_hnsw_export(self._h, cnt, ndp, _p(level0, _u32p), _p(levels, _i32p), offs.ctypes.data_as(C.POINTER(C.c_int64)),
+                                           None, None))
+        upper = np.zeros((max(int(offs[cnt]), 1), 1 + info.M), np.uint32)
+        _check(self._lib.rxgpu_hnsw_export(self._h, cnt, ndp, None, None, None, _p(upper, _u32p), None))
+        return dict(n=info.n, maxlevel=info.maxlevel, enterpoint=info.enterpoint, M=info.M, maxM0=info.maxM0, level0=level0[:cnt],
+                    levels=levels[:cnt], upper_offsets=offs, upper=upper[:int(offs[cnt])])
 
     def ivf_create(self, centroids):
         c = np.ascontiguousarray(centroids, np.float32).reshape(-1, self.dim)
@@ -961,6 +995,17 @@ def kmeans_plan(n: int, nlist: int, seed: int = 1234, max_points_per_centroid: i
     init = np.zeros(max(nlist, 1), np.int32)
     _check(lib().rxgpu_kmeans_plan(n, nlist, seed, max_points_per_centroid, _p(sample, _i32p), _p(init, _i32p)))
     return sample[:ns], init[:nlist]
+
+
+def hnsw_build_plan(M: int, n: int, first: int = 0, maxlevel: int = -1, levels=None, seed: int = 100):
+    """host only: (levels, batch ends) of rxgpu_hnsw_build for rows [first, n) onto a graph whose top level is maxlevel"""
+    lv = None if levels is None else np.ascontiguousarray(levels, np.int32)
+    out = np.zeros(max(n - first, 1), np.int32)
+    ends = np.zeros(max(n - first, 1), np.uint64)
+    nb = C.c_uint64(0)
+    _check(lib().rxgpu_hnsw_build_plan(M, first, n, maxlevel, None if lv is None else _p(lv, _i32p), seed, _p(out, _i32p), _p(ends, _u64p),
+                                       C.byref(nb)))
+    return out[:n - first], ends[:nb.value]
 
 
 def ft_decode_packed(data, count: int):

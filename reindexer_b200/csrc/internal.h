@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
 #include <functional>
 #include <memory>
@@ -234,8 +235,14 @@ struct rxgpu_index {
 	static constexpr size_t kShadowLogMax = 4096;
 	mutable std::vector<std::pair<uint32_t, uint32_t>> shadow_dirty;
 	mutable bool shadow_dirty_all = true;
+	// lowest row written since the attached HNSW graph was imported, built or patched (~0: none): an append onto the graph needs
+	// its rows unchanged
+	uint64_t rows_touched_from = ~0ull;
 	void touchRows(uint64_t begin, uint64_t end) {
 		std::lock_guard<std::mutex> lck(tc_mtx);
+		if (begin < end) {
+			rows_touched_from = std::min(rows_touched_from, begin);
+		}
 		if (!d_shadow || shadow_dirty_all || begin >= end) {
 			return;
 		}

@@ -5,7 +5,11 @@
 // _search_range / _mark_deleted / _update).  The device copy (rows in internal-id order + level-0 slab + upper levels) is imported by
 // the first search; after that single-writer inserts patch it in place (rxgpu_hnsw_update: the inserted row and the lists of the nodes
 // the reference's inserter rewrote), MarkDelete sets a tombstone bit (like hnswalg.h:1303-1335).  Concurrent bulk inserts, resizes and
-// cache loads re-import.
+// cache loads re-import -- unless device building is switched on (constructor flag, RX_GPU_HNSW_BUILD at the patch site): then
+// AddPointConcurrent only stages (label, vector), and the first other member call sorts the staged rows by label, appends them to the
+// device copy and inserts them there with rxgpu_hnsw_build, then writes the new nodes and every list they changed back into the host
+// graph with addPoint's bookkeeping.  The host graph then equals the device graph list for list and no import follows.  That graph
+// differs from the one the reference's inserter would build (DESIGN.md §3.8), so the switch is off by default.
 // Meant to be dropped into cpp_src/core/index/float_vector/hnswlib/ next to hnsw.h; it includes the reference's own headers and is
 // therefore compiled only where that tree is available (tests/cpp/dropin_hnsw_check.cc does so in the authoring container).
 // INTEGRATION.md section 5 shows the patch of hnsw_index.cc.
@@ -21,7 +25,9 @@
 #include <mutex>
 #include <optional>
 #include <stdexcept>
+#include <numeric>
 #include <string>
+#include <unordered_map>
 #include <utility>
 #include <vector>
 
@@ -37,12 +43,17 @@ class [[nodiscard]] GpuHnsw {
 	using Cpu = HierarchicalNSWImpl<float, synchronization>;
 
 public:
-	GpuHnsw(reindexer::IsArray, reindexer::VectorMetric metric, size_t dim, size_t maxElements, size_t M, size_t efConstruction)
+	GpuHnsw(reindexer::IsArray, reindexer::VectorMetric metric, size_t dim, size_t maxElements, size_t M, size_t efConstruction,
+			bool deviceBuild = false)
 		: metric_(metric),
 		  dim_(dim),
-		  cpu_(std::make_unique<Cpu>(metric, dim, maxElements, M, efConstruction, kHnswRandomSeed, reindexer::ReplaceDeleted_True)) {}
+		  cpu_(std::make_unique<Cpu>(metric, dim, maxElements, M, efConstruction, kHnswRandomSeed, reindexer::ReplaceDeleted_True)),
+		  deviceBuild_(deviceBuild) {}
 	GpuHnsw(const GpuHnsw& other, size_t newCapacity)
-		: metric_(other.metric_), dim_(other.dim_), cpu_(std::make_unique<Cpu>(*other.cpu_, newCapacity)) {}  // device copy: lazily
+		: metric_(other.metric_),
+		  dim_(other.dim_),
+		  cpu_((other.materialise(), std::make_unique<Cpu>(*other.cpu_, newCapacity))),
+		  deviceBuild_(other.deviceBuild_) {}  // device copy: lazily
 	GpuHnsw& operator=(GpuHnsw&& o) noexcept {
 		releaseDevice();
 		metric_ = o.metric_;
@@ -54,22 +65,50 @@ public:
 		pendingRows_ = std::move(o.pendingRows_);
 		pendingLists_ = std::move(o.pendingLists_);
 		deviceCapacity_ = o.deviceCapacity_;
+		deviceBuild_ = o.deviceBuild_;
+		stagedLabels_ = std::move(o.stagedLabels_);
+		stagedRows_ = std::move(o.stagedRows_);
+		stagedIndex_ = std::move(o.stagedIndex_);
+		stagedCount_.store(o.stagedCount_.load());
 		return *this;
 	}
 	~GpuHnsw() { releaseDevice(); }
 
+	// staged rows count: upsertConcurrent's capacity check (hnsw_index.cc:106) sees them
 	size_t MaxElements() const noexcept { return cpu_->MaxElements(); }
-	size_t CurrentElementCount() const noexcept { return cpu_->CurrentElementCount(); }
-	size_t DeletedCountUnsafe() const noexcept { return cpu_->DeletedCountUnsafe(); }
-	size_t AllocatedMemSize() const noexcept { return cpu_->AllocatedMemSize(); }
+	size_t CurrentElementCount() const noexcept { return cpu_->CurrentElementCount() + stagedCount_.load(std::memory_order_acquire); }
+	size_t DeletedCountUnsafe() const {
+		materialise();
+		return cpu_->DeletedCountUnsafe();
+	}
+	size_t AllocatedMemSize() const {
+		materialise();
+		return cpu_->AllocatedMemSize();
+	}
 	size_t ElementSize() const noexcept { return cpu_->ElementSize(); }
-	size_t DeviceMemSize() const noexcept { return gpu_ ? rxgpu_index_device_bytes(gpu_) : 0; }
-	labeltype ExternalLabel(tableint internalId) const { return cpu_->ExternalLabel(internalId); }
-	bool IsMarkedDeleted(tableint internalId) const noexcept { return cpu_->IsMarkedDeleted(internalId); }
-	const float* FloatPtrByExternalLabel(labeltype label) const { return cpu_->FloatPtrByExternalLabel(label); }
-	size_t GetHash(reindexer::FloatVectorId id) const { return cpu_->GetHash(id.AsNumber()); }
+	size_t DeviceMemSize() const {
+		materialise();
+		return gpu_ ? rxgpu_index_device_bytes(gpu_) : 0;
+	}
+	labeltype ExternalLabel(tableint internalId) const {
+		materialise();
+		return cpu_->ExternalLabel(internalId);
+	}
+	bool IsMarkedDeleted(tableint internalId) const {
+		materialise();
+		return cpu_->IsMarkedDeleted(internalId);
+	}
+	const float* FloatPtrByExternalLabel(labeltype label) const {
+		materialise();
+		return cpu_->FloatPtrByExternalLabel(label);
+	}
+	size_t GetHash(reindexer::FloatVectorId id) const {
+		materialise();
+		return cpu_->GetHash(id.AsNumber());
+	}
 
 	void MarkDelete(reindexer::FloatVectorId id) {
+		materialise();
 		const labeltype label = id.AsNumber();
 		if (gpu_ && !dirty_.load(std::memory_order_acquire) && hasPending_.load(std::memory_order_acquire)) {
 			try {
@@ -90,6 +129,7 @@ public:
 	// Single-writer insert (the namespace's exclusive lock): the device copy is patched in place by the next search -- the nodes whose
 	// lists addPoint / updatePoint rewrote are known exactly (one-hop neighbours before and after the call), so an upsert costs O(M) small copies, not a re-import.
 	void AddPointNoLock(reindexer::ConstFloatVectorView vect, reindexer::FloatVectorId id) {
+		materialise();
 		const labeltype label = id.AsNumber();
 		if (!gpu_ || dirty_.load(std::memory_order_acquire)) {
 			cpu_->AddPointNoLock(vect.Data(), label);
@@ -122,20 +162,47 @@ public:
 		}
 		hasPending_.store(true, std::memory_order_release);
 	}
-	// concurrent inserts interleave their list rewrites, so the set of touched nodes is not known per call: full re-import
+	// The transaction's inserter threads (TransactionConcurrentInserter).  Device building: a new label on a map without tombstones is
+	// only staged, never touching the device; an existing label, or a map whose tombstones replace_deleted would reuse, takes the
+	// reference's path.  Without device building, concurrent inserts interleave their list rewrites, so the set of touched nodes is not
+	// known per call: full re-import.
 	void AddPointConcurrent(reindexer::ConstFloatVectorView vect, reindexer::FloatVectorId id) {
-		cpu_->AddPointConcurrent(vect.Data(), id.AsNumber());
+		const labeltype label = id.AsNumber();
+		if (deviceBuild_) {
+			std::lock_guard<std::mutex> lck(stageMtx_);  // also orders the reference's path below after the label_lookup_ read
+			if (cpu_->DeletedCountUnsafe() == 0 && cpu_->label_lookup_.find(label) == cpu_->label_lookup_.end()) {
+				if (const auto it = stagedIndex_.find(label); it != stagedIndex_.end()) {  // staged twice: the later vector wins
+					std::copy(vect.Data(), vect.Data() + dim_, stagedRows_.begin() + it->second * dim_);
+					return;
+				}
+				if (cpu_->CurrentElementCount() + stagedLabels_.size() >= cpu_->MaxElements()) {
+					throw std::runtime_error("The number of elements exceeds the specified limit");  // hnswalg.h:1730
+				}
+				stagedIndex_.emplace(label, stagedLabels_.size());
+				stagedLabels_.push_back(label);
+				stagedRows_.insert(stagedRows_.end(), vect.Data(), vect.Data() + dim_);
+				stagedCount_.store(stagedLabels_.size(), std::memory_order_release);
+				return;
+			}
+			cpu_->AddPointConcurrent(vect.Data(), label);
+			dirty_.store(true, std::memory_order_release);
+			return;
+		}
+		cpu_->AddPointConcurrent(vect.Data(), label);
 		dirty_.store(true, std::memory_order_release);
 	}
 	void ResizeIndex(size_t newMaxElements) {
+		materialise();
 		cpu_->ResizeIndex(newMaxElements);
 		dirty_.store(true, std::memory_order_release);  // the device copy is re-imported at the new capacity
 	}
 	void SaveIndex(IWriter& writer, const std::atomic_int32_t& cancel) const {
+		materialise();
 		writer.PutVarUInt(uint32_t(0));  // not quantised (HierarchicalNSW::serializeQuantizingParams, hnsw.cc:52-58)
 		cpu_->SaveIndex(writer, cancel);
 	}
 	void LoadIndex(IReader& reader) {
+		materialise();
 		if (reader.GetVarUInt() != 0) {
 			throw std::runtime_error("GpuHnsw: quantised HNSW caches are not supported on the device path");
 		}
@@ -143,6 +210,10 @@ public:
 		dirty_.store(true, std::memory_order_release);
 	}
 	void Reset() noexcept {
+		stagedLabels_.clear();
+		stagedRows_.clear();
+		stagedIndex_.clear();
+		stagedCount_.store(0);
 		releaseDevice();
 		cpu_.reset();
 	}
@@ -150,6 +221,7 @@ public:
 	// returns the reference's max-heap (worst on top) so that HnswIndexBase::select drains it unchanged
 	SearchResultQueue SearchKnn(const float* queryData, std::optional<float> /*queryDataNorm*/, size_t k, size_t ef = 0) const {
 		using pair_t = std::pair<float, labeltype>;
+		materialise();
 		if (cpu_->CurrentElementCount() == 0) {
 			return SearchResultQueue();  // hnswalg.h:1989-1991
 		}
@@ -168,6 +240,7 @@ public:
 	}
 	SearchResultQueue SearchRange(const float* queryData, std::optional<float> /*queryDataNorm*/, float radius, size_t ef) const {
 		using pair_t = std::pair<float, labeltype>;
+		materialise();
 		if (cpu_->CurrentElementCount() == 0) {
 			return SearchResultQueue();  // hnswalg.h:2017-2019
 		}
@@ -190,6 +263,7 @@ public:
 	}
 	// streaming search: the reference's own routine on the host graph (hnswalg.h:1865-1975)
 	StreamingSearchSession BeginStreamingSearch(const float* queryData, std::optional<float> queryDataNorm, StreamingSearchOptions opts) const {
+		materialise();
 		return cpu_->BeginStreamingSearch(queryData, queryDataNorm, opts);
 	}
 	StreamingBatch ContinueStreamingSearch(StreamingSearchSession& session, size_t batchSize) const {
@@ -206,6 +280,16 @@ public:
 	// nodes patched in place since the last import
 	const std::string& LastPatchError() const noexcept { return lastPatchError_; }  // why the copy was last scheduled for a re-import
 	size_t DevicePatchedNodes() const noexcept { return gpu_ ? size_t(rxgpu_hnsw_update_count(gpu_)) : 0; }
+	// rows inserted by rxgpu_hnsw_build, and the graphs themselves -- exposed for tests
+	size_t DeviceBuiltRows() const noexcept { return builtRows_.load(); }
+	const Cpu& HostGraph() const {
+		materialise();
+		return *cpu_;
+	}
+	const rxgpu_index* DeviceIndex() const {
+		materialise();
+		return gpu_;
+	}
 
 private:
 	constexpr static int kHnswRandomSeed = 100;  // hnsw.h:73
@@ -230,7 +314,7 @@ private:
 			throw std::runtime_error(rxgpu_last_error());
 		}
 	}
-	void releaseDevice() noexcept {
+	void releaseDevice() const noexcept {
 		if (gpu_) {
 			rxgpu_index_destroy(gpu_);
 			gpu_ = nullptr;
@@ -310,6 +394,151 @@ private:
 		pendingRows_.clear();
 		pendingLists_.clear();
 		hasPending_.store(false, std::memory_order_release);
+	}
+
+	// Inserts the staged rows: sorted by label (so the graph depends on the set of rows, not on thread timing), appended to the device
+	// copy brought up to date first, levels drawn from the host graph's own generator as addPoint would draw them, rxgpu_hnsw_build,
+	// then the new nodes and every old node their lists name are read back and written into the host graph.  When the device step
+	// fails the rows go through the reference's inserter instead and the device copy is rebuilt by the next search.
+	void materialise() const {
+		if (stagedCount_.load(std::memory_order_acquire) == 0) {
+			return;
+		}
+		std::lock_guard<std::mutex> lck(stageMtx_);
+		const size_t cnt = stagedLabels_.size();
+		if (cnt == 0) {
+			return;
+		}
+		std::vector<size_t> order(cnt);
+		std::iota(order.begin(), order.end(), size_t(0));
+		std::sort(order.begin(), order.end(), [&](size_t a, size_t b) { return stagedLabels_[a] < stagedLabels_[b]; });
+		std::vector<uint64_t> labels(cnt);
+		std::vector<float> rows(cnt * dim_);
+		for (size_t i = 0; i < cnt; ++i) {
+			labels[i] = stagedLabels_[order[i]];
+			std::copy_n(stagedRows_.begin() + order[i] * dim_, dim_, rows.begin() + i * dim_);
+		}
+		stagedLabels_.clear();
+		stagedRows_.clear();
+		stagedIndex_.clear();
+		Cpu& g = *cpu_;
+		const size_t first = g.cur_element_count.load();
+		std::vector<int32_t> levels(cnt);
+		for (auto& l : levels) {
+			l = g.template getRandomLevel<DummyLocker>(g.mult_);
+		}
+		try {
+			buildOnDevice(first, labels, rows, levels);
+		} catch (const std::exception& e) {
+			lastPatchError_ = e.what();
+			for (size_t i = 0; i < cnt; ++i) {
+				if (g.label_lookup_.find(labels[i]) == g.label_lookup_.end()) {
+					g.AddPointNoLock(rows.data() + i * dim_, labels[i]);
+				}
+			}
+			dirty_.store(true, std::memory_order_release);
+		}
+		stagedCount_.store(0, std::memory_order_release);
+	}
+	void buildOnDevice(size_t first, const std::vector<uint64_t>& labels, const std::vector<float>& rows, const std::vector<int32_t>& levels) const {
+		Cpu& g = *cpu_;
+		const size_t cnt = labels.size(), m0 = g.maxM0_, m = g.M_;
+		if (first == 0) {  // nothing to import: a fresh device index
+			std::lock_guard<std::mutex> lk(mtx_);
+			releaseDevice();
+			pendingRows_.clear();
+			pendingLists_.clear();
+			hasPending_.store(false, std::memory_order_release);
+			rxgpu_index* ix = nullptr;
+			check(rxgpu_index_create(&ix, toMetric(metric_), uint32_t(dim_), g.MaxElements(), deviceFromEnv(), 0));
+			gpu_ = ix;
+			deviceCapacity_ = g.MaxElements();
+			dirty_.store(false, std::memory_order_release);
+		} else {
+			if (first + cnt > deviceCapacity_) {
+				dirty_.store(true, std::memory_order_release);  // re-imported at the map's capacity
+			}
+			ensureDevice();
+		}
+		check(rxgpu_index_upsert_batch(gpu_, cnt, labels.data(), rows.data()));
+		rxgpu_hnsw_build_stats st{};
+		check(rxgpu_hnsw_build(gpu_, uint32_t(m), uint32_t(g.ef_construction_), first, levels.data(), 0, &st));
+		// the new nodes, then every old node one of their lists names: only those lists changed
+		std::vector<uint32_t> nodes(cnt);
+		std::iota(nodes.begin(), nodes.end(), uint32_t(first));
+		rxgpu_hnsw_graph info{};
+		std::vector<uint32_t> l0, up;
+		std::vector<int32_t> lv;
+		std::vector<int64_t> off;
+		auto read = [&](const std::vector<uint32_t>& which) {
+			l0.assign(which.size() * (1 + m0), 0u);
+			lv.assign(which.size(), 0);
+			off.assign(which.size() + 1, 0);
+			check(rxgpu_hnsw_export(gpu_, which.size(), which.data(), l0.data(), lv.data(), off.data(), nullptr, &info));
+			up.assign(std::max<int64_t>(off[which.size()], 1) * (1 + m), 0u);
+			check(rxgpu_hnsw_export(gpu_, which.size(), which.data(), nullptr, nullptr, nullptr, up.data(), nullptr));
+		};
+		read(nodes);
+		std::vector<uint32_t> oldNodes;
+		for (size_t i = 0; i < cnt; ++i) {
+			for (uint32_t j = 1; j <= l0[i * (1 + m0)]; ++j) {
+				oldNodes.push_back(l0[i * (1 + m0) + j]);
+			}
+			for (int64_t s = off[i]; s < off[i + 1]; ++s) {
+				for (uint32_t j = 1; j <= up[s * (1 + m)]; ++j) {
+					oldNodes.push_back(up[s * (1 + m) + j]);
+				}
+			}
+		}
+		oldNodes.erase(std::remove_if(oldNodes.begin(), oldNodes.end(), [&](uint32_t v) { return v >= first; }), oldNodes.end());
+		std::sort(oldNodes.begin(), oldNodes.end());
+		oldNodes.erase(std::unique(oldNodes.begin(), oldNodes.end()), oldNodes.end());
+		const std::vector<uint32_t> newL0 = l0, newUp = up;
+		const std::vector<int64_t> newOff = off;
+		// addPoint's bookkeeping for every new node (hnswalg.h:1727-1775)
+		for (size_t i = 0; i < cnt; ++i) {
+			const tableint id = tableint(first + i);
+			const float* data = rows.data() + i * dim_;
+			g.label_lookup_[labels[i]] = id;
+			g.cur_element_count++;
+			g.fstdistfunc_.AddNorm(data, id);
+			g.element_levels_[id] = levels[i];
+			std::memset(g.data_level0_memory_ + size_t(id) * g.size_data_per_element_, 0, g.size_data_per_element_);
+			g.setExternalLabel(id, labels[i]);
+			g.setHashByInternalId(id, g.CalcHash(data));
+			std::memcpy(g.getDataByInternalId(id), data, g.data_size_);
+			if (levels[i]) {
+				g.linkLists_[id] = static_cast<char*>(malloc(g.size_links_per_element_ * levels[i] + 1));
+				if (g.linkLists_[id] == nullptr) {
+					throw std::runtime_error("Not enough memory: addPoint failed to allocate linklist");
+				}
+				std::memset(g.linkLists_[id], 0, g.size_links_per_element_ * levels[i] + 1);
+			}
+		}
+		auto write = [&](tableint v, const uint32_t* list0, const uint32_t* upper, int level) {
+			auto put = [&](linklistsizeint* ll, const uint32_t* src) {
+				g.setListCount(ll, (unsigned short)src[0]);
+				for (uint32_t j = 0; j < src[0]; ++j) {
+					writeLinkListNeighbor(ll, j, src[1 + j]);
+				}
+			};
+			put(g.get_linklist0(v), list0);
+			for (int l = 1; l <= level; ++l) {
+				put(g.get_linklist(v, l), upper + size_t(l - 1) * (1 + m));
+			}
+		};
+		for (size_t i = 0; i < cnt; ++i) {
+			write(tableint(first + i), newL0.data() + i * (1 + m0), newUp.data() + newOff[i] * (1 + m), levels[i]);
+		}
+		if (!oldNodes.empty()) {
+			read(oldNodes);
+			for (size_t i = 0; i < oldNodes.size(); ++i) {
+				write(tableint(oldNodes[i]), l0.data() + i * (1 + m0), up.data() + off[i] * (1 + m), lv[i]);
+			}
+		}
+		g.maxlevel_ = info.maxlevel;
+		g.enterpoint_node_ = tableint(info.enterpoint);
+		builtRows_.fetch_add(cnt);
 	}
 
 	void ensureDevice() const {
@@ -421,6 +650,13 @@ private:
 	mutable std::string lastPatchError_;
 	mutable std::atomic<size_t> imports_{0};
 	mutable std::mutex mtx_;
+	bool deviceBuild_ = false;
+	mutable std::mutex stageMtx_;  // the staged rows (AddPointConcurrent) and their materialisation
+	mutable std::vector<labeltype> stagedLabels_;
+	mutable std::vector<float> stagedRows_;
+	mutable std::unordered_map<labeltype, size_t> stagedIndex_;
+	mutable std::atomic<size_t> stagedCount_{0};
+	mutable std::atomic<size_t> builtRows_{0};
 };
 
 }  // namespace hnswlib
