@@ -57,9 +57,6 @@ struct BuildArgs {
 	unsigned long long* npruned;
 };
 
-__device__ __forceinline__ const uint32_t* list_of(const HnswArgs& a, uint32_t node, int level) {
-	return level ? a.upper + (size_t(a.upper_off[node]) + size_t(level - 1)) * a.up_stride : a.level0 + size_t(node) * a.l0_stride;
-}
 __device__ __forceinline__ uint32_t* list_of_mut(const HnswArgs& a, uint32_t node, int level) {
 	return const_cast<uint32_t*>(list_of(a, node, level));
 }
@@ -100,14 +97,7 @@ __device__ uint32_t search_layer(const BuildArgs& b, const float4* sq4, uint32_t
 	__syncwarp();
 	uint32_t size = 1, vcount = 1;
 	for (;;) {
-		int pos = -1;
-		for (uint32_t c = 0; c < size && pos < 0; c += 32) {
-			const uint32_t i = c + lane;
-			const unsigned m = __ballot_sync(0xffffffffu, i < size && !(l_id[i] & kExpanded));
-			if (m) {
-				pos = int(c) + __ffs(m) - 1;
-			}
-		}
+		const int pos = first_unexpanded(l_id, size, lane);
 		if (pos < 0) {
 			break;  // every candidate at or below lowerBound is expanded (:681)
 		}
@@ -117,29 +107,7 @@ __device__ uint32_t search_layer(const BuildArgs& b, const float4* sq4, uint32_t
 			l_id[pos] = node | kExpanded;
 		}
 		const uint32_t* ll = list_of(a, node, level);
-		const uint32_t cnt = min(ll[0], uint32_t(kMaxNeighbours));
-		uint32_t ucnt = 0;
-		for (uint32_t c = 0; c < cnt; c += 32) {
-			const uint32_t j = c + lane;
-			uint32_t nid = 0;
-			bool fresh = false;
-			if (j < cnt) {
-				nid = ll[1 + j];
-				const uint32_t bit = 1u << (nid & 31);
-				fresh = !(atomicOr(&visited[nid >> 5], bit) & bit);
-			}
-			const unsigned fm = __ballot_sync(0xffffffffu, fresh);
-			if (fresh) {
-				const uint32_t o = ucnt + __popc(fm & ((1u << lane) - 1u));
-				s_ids[o] = nid;
-				if (vcount + o - ucnt < kVlogCap) {
-					vlog[vcount + o - ucnt] = nid;
-				}
-			}
-			ucnt += __popc(fm);
-			vcount += __popc(fm);
-		}
-		__syncwarp();
+		const uint32_t ucnt = gather_fresh(ll, min(ll[0], uint32_t(kMaxNeighbours)), visited, vlog, vcount, s_ids, lane);
 		if (ucnt == 0) {
 			continue;
 		}
@@ -151,36 +119,14 @@ __device__ uint32_t search_layer(const BuildArgs& b, const float4* sq4, uint32_t
 			if (size >= a.ef && !key_less(d, nid, l_dist[size - 1], l_id[size - 1] & ~kExpanded)) {
 				continue;
 			}
-			uint32_t p = 0;  // entries before (d, nid)
-			for (uint32_t c = 0; c < size; c += 32) {
-				const uint32_t i = c + lane;
-				p += __popc(__ballot_sync(0xffffffffu, i < size && key_less(l_dist[i], l_id[i] & ~kExpanded, d, nid)));
-			}
+			const uint32_t p = warp_count(size, lane, [&](uint32_t i) { return key_less(l_dist[i], l_id[i] & ~kExpanded, d, nid); });
 			const uint32_t newsize = min(size + 1, a.ef);
-			for (int c = int((newsize - 1) / 32) * 32; c >= 0; c -= 32) {  // shift right, highest chunk first
-				const uint32_t i = uint32_t(c) + lane;
-				const bool mv = i > p && i < newsize;
-				float td = 0.f;
-				uint32_t ti = 0;
-				if (mv) {
-					td = l_dist[i - 1];
-					ti = l_id[i - 1];
-				}
-				__syncwarp();
-				if (mv) {
-					l_dist[i] = td;
-					l_id[i] = ti;
-				}
-				__syncwarp();
-			}
-			if (lane == 0) {
-				l_dist[p] = d;
-				l_id[p] = nid;
-			}
-			__syncwarp();
+			list_insert(l_dist, l_id, p, newsize, d, nid, lane);
 			size = newsize;
 		}
 	}
+	// the visited bitmap cleared from its log, as the search kernel does: as a helper shared with that kernel, ptxas allocated
+	// hnsw_build_insert<true> differently and its insert phase ran 5 % slower
 	if (vcount <= kVlogCap) {
 		for (uint32_t j = lane; j < vcount; j += 32) {
 			visited[vlog[j] >> 5] = 0;
@@ -223,7 +169,7 @@ __global__ void __launch_bounds__(kHnswThreads) hnsw_build_insert(const BuildArg
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const HnswArgs& a = b.g;
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-	const uint32_t dp4 = ((a.dim + 127u) / 128u) * 32u;
+	const uint32_t dp4 = hnsw_query_words(a.dim);
 	// per warp: query | list dist[ef] | list id[ef] | gather ids[64] | gather dists[64] | selected[32]
 	const uint32_t efp = (a.ef + 3u) & ~3u;
 	const size_t per_warp = size_t(dp4) * 16 + size_t(efp) * 8 + kMaxNeighbours * 8 + kBuildSelMax * 4;
@@ -250,7 +196,8 @@ __global__ void __launch_bounds__(kHnswThreads) hnsw_build_insert(const BuildArg
 		const uint32_t u = b.b0 + qi;
 		stage_row(b, sq4, u, dp4, lane);
 		const int lvl = a.levels[u];
-		// greedy descent through maxlevel .. lvl + 1 (:1781-1811): strict <, the first minimum wins
+		// greedy descent through maxlevel .. lvl + 1 (:1781-1811), the entry point's distance counted: greedy_descent's rule, written
+		// out with list_of because through the helper ptxas gives the Cosine instantiation 64 registers instead of 56
 		uint32_t cur = a.enterpoint;
 		if (lvl < a.maxlevel) {
 			if (lane == 0) {
@@ -356,7 +303,7 @@ __global__ void __launch_bounds__(kHnswThreads) hnsw_build_link(const BuildArgs 
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const HnswArgs& a = b.g;
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-	const uint32_t dp4 = ((a.dim + 127u) / 128u) * 32u;
+	const uint32_t dp4 = hnsw_query_words(a.dim);
 	// per warp: query | gather ids[64] | gather dists[64] | old list keys[64] | old list sorted[64] | selected[64]
 	const size_t per_warp = size_t(dp4) * 16 + kMaxNeighbours * (4 + 4 + 8 + 8 + 4);
 	unsigned char* base = smem_raw + per_warp * warp;
@@ -509,13 +456,9 @@ __global__ void hnsw_gather_lists(const uint32_t* src, uint32_t width, const uin
 }
 
 size_t insertSmem(uint32_t dim, uint32_t ef) {
-	const uint32_t dp4 = ((dim + 127u) / 128u) * 32u;
-	return (size_t(dp4) * 16 + size_t((ef + 3u) & ~3u) * 8 + kMaxNeighbours * 8 + kBuildSelMax * 4) * kHnswWarps;
+	return (size_t(hnsw_query_words(dim)) * 16 + size_t((ef + 3u) & ~3u) * 8 + kMaxNeighbours * 8 + kBuildSelMax * 4) * kHnswWarps;
 }
-size_t linkSmem(uint32_t dim) {
-	const uint32_t dp4 = ((dim + 127u) / 128u) * 32u;
-	return (size_t(dp4) * 16 + kMaxNeighbours * (4 + 4 + 8 + 8 + 4)) * kHnswWarps;
-}
+size_t linkSmem(uint32_t dim) { return (size_t(hnsw_query_words(dim)) * 16 + kMaxNeighbours * (4 + 4 + 8 + 8 + 4)) * kHnswWarps; }
 constexpr size_t kBuildSmemBudget = 200 * 1024;
 
 // getRandomLevel (hnswalg.h:625-635) for `count` rows: std::default_random_engine seeded like level_generator_ (:293), one draw each
@@ -599,7 +542,6 @@ int buildGraph(rxgpu_index* ix, const rxgpu_hnsw_device* old, uint32_t M, uint32
 	}
 	h->h_upper_off.push_back((long long)slots);
 	h->upper_slots = slots;
-	const size_t up = std::max<size_t>(1, slots) * s1;
 	// keys of a batch: at most M per selected level of each row
 	uint64_t keyCap = 1;
 	{
@@ -616,17 +558,9 @@ int buildGraph(rxgpu_index* ix, const rxgpu_hnsw_device* old, uint32_t M, uint32
 		}
 	}
 	cudaStream_t s = ix->stream;
-	RX_CUDA(h->level0.ensure(capNodes * s0));
-	RX_CUDA(h->levels.ensure(capNodes));
-	RX_CUDA(h->upper_off.ensure(capNodes + 1));
-	RX_CUDA(h->upper.ensure(up + (capNodes - n) / 8 * s1 + 64 * s1));
-	h->cap_nodes = capNodes;
-	h->slots = hnswSlots(ix);
-	h->words = uint32_t((capNodes + 31) / 32);
-	RX_CUDA(h->visited.ensure(size_t(h->slots) * h->words));
-	RX_CUDA(h->vlog.ensure(size_t(h->slots) * kVlogCap));
-	RX_CUDA(h->counter.ensure(1));
-	RX_CUDA(h->deleted.ensure(h->words));
+	if (int rc = allocGraph(ix, h, capNodes, std::max<size_t>(1, slots) * s1)) {
+		return rc;
+	}
 	DevBuf<uint64_t> keys, sorted, alt;
 	DevBuf<uint32_t> seg;
 	DevBuf<unsigned int> cnt32;         // next row, keys, segments, next segment
@@ -659,8 +593,6 @@ int buildGraph(rxgpu_index* ix, const rxgpu_hnsw_device* old, uint32_t M, uint32
 	}
 	RX_CUDA(cudaMemcpyAsync(h->levels.p, h->h_levels.data(), size_t(n) * 4, cudaMemcpyHostToDevice, s));
 	RX_CUDA(cudaMemcpyAsync(h->upper_off.p, h->h_upper_off.data(), (size_t(n) + 1) * 8, cudaMemcpyHostToDevice, s));
-	RX_CUDA(cudaMemsetAsync(h->visited.p, 0, size_t(h->slots) * h->words * 4, s));
-	RX_CUDA(cudaMemsetAsync(h->deleted.p, 0, size_t(h->words) * 4, s));
 	RX_CUDA(cudaMemsetAsync(cnt64.p, 0, 16, s));
 	if (ix->metric == RXGPU_COS) {
 		hnsw_build_query_coefs<<<unsigned((n + 255) / 256), 256, 0, s>>>(ix->d_rows, ix->pitch, ix->dim, uint32_t(n), qk.p);
@@ -686,21 +618,11 @@ int buildGraph(rxgpu_index* ix, const rxgpu_hnsw_device* old, uint32_t M, uint32
 		}
 	} evGuard{ev};
 	BuildArgs b{};
-	b.g.rows = ix->d_rows;
-	b.g.norm_coefs = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
-	b.g.level0 = h->level0.p;
-	b.g.levels = h->levels.p;
-	b.g.upper_off = h->upper_off.p;
-	b.g.upper = h->upper.p;
+	b.g = graphArgs(ix, h);
 	b.g.visited = h->visited.p;
 	b.g.vlog = h->vlog.p;
 	b.g.next_query = cnt32.p;
-	b.g.pitch = ix->pitch;
-	b.g.dim = ix->dim;
-	b.g.l0_stride = s0;
-	b.g.up_stride = s1;
 	b.g.ef = ef_construction;
-	b.g.words = h->words;
 	b.qk = ix->metric == RXGPU_COS ? qk.p : nullptr;
 	b.M = M;
 	b.keys = keys.p;
@@ -771,7 +693,6 @@ int buildGraph(rxgpu_index* ix, const rxgpu_hnsw_device* old, uint32_t M, uint32
 	h->maxlevel = ml;
 	h->enterpoint = ep;
 	h->index_version = ix->version;
-	h->h_deleted.assign(h->words, 0u);
 	if (old) {
 		h->updates = old->updates;
 	}
@@ -882,13 +803,10 @@ int rxgpu_hnsw_export(const rxgpu_index* ix, uint64_t nnodes, const uint32_t* no
 	if (int rc = checkIndex(ix)) {
 		return rc;
 	}
+	if (int rc = checkGraph(ix)) {
+		return rc;
+	}
 	const rxgpu_hnsw_device* h = ix->hnsw;
-	if (!h) {
-		return fail(RXGPU_ERR_LOGIC, "rxgpu: no HNSW graph imported into this index");
-	}
-	if (h->n != ix->size || h->index_version != ix->version) {
-		return fail(RXGPU_ERR_LOGIC, "rxgpu: the index changed after the HNSW graph was imported");
-	}
 	if (info) {
 		*info = rxgpu_hnsw_graph{h->n, h->M, h->maxM0, h->maxlevel, h->enterpoint, h->upper_slots, nullptr, nullptr, nullptr, nullptr};
 	}

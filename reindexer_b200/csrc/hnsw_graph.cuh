@@ -1,4 +1,5 @@
-// The device HNSW graph and the distance gather shared by the search kernels (hnsw.cu) and the graph builder (hnsw_build.cu).
+// The device HNSW graph, the distance gather and the warp-level traversal steps shared by the search kernels (hnsw.cu) and the graph
+// builder (hnsw_build.cu), and the host set-up of a graph both entry points use.
 #pragma once
 #include <algorithm>
 #include <cstdlib>
@@ -179,6 +180,137 @@ __device__ __forceinline__ void warp_dists(const HnswArgs& a, const float4* sq4,
 	__syncwarp();
 }
 
+// float4 slots of a query staged in shared memory: the dimension rounded up to whole 128-float chunks of warp_dists
+__host__ __device__ __forceinline__ uint32_t hnsw_query_words(uint32_t dim) { return ((dim + 127u) / 128u) * 32u; }
+
+// the neighbour list of `node` at `level`: [count, ids...]; upper_list_of for level >= 1
+__device__ __forceinline__ const uint32_t* upper_list_of(const HnswArgs& a, uint32_t node, int level) {
+	return a.upper + (size_t(a.upper_off[node]) + size_t(level - 1)) * a.up_stride;
+}
+__device__ __forceinline__ const uint32_t* list_of(const HnswArgs& a, uint32_t node, int level) {
+	return level ? upper_list_of(a, node, level) : a.level0 + size_t(node) * a.l0_stride;
+}
+
+// the query q[0, dim) zero padded to dp4 float4 slots, thread t of nt
+__device__ __forceinline__ void stage_query(float4* sq4, const float* q, uint32_t dim, uint32_t dp4, uint32_t t, uint32_t nt) {
+	float* sq = reinterpret_cast<float*>(sq4);
+	for (uint32_t c = t; c < dp4 * 4; c += nt) {
+		sq[c] = c < dim ? q[c] : 0.f;
+	}
+}
+
+// greedy descent through levels top .. stop + 1 (stop >= 0) from cur at distance curdist (hnswalg.h:799-827, :1781-1811): strict <,
+// the first minimum wins
+template <bool kIsL2>
+__device__ __forceinline__ void greedy_descent(const HnswArgs& a, const float4* sq4, uint32_t& cur, float& curdist, int top, int stop, uint32_t* s_ids,
+											   float* s_d, int lane, uint32_t& n_dist, uint32_t& n_hops, float qcorr = 0.f, float qcoef = 1.f) {
+	for (int level = top; level > stop; --level) {
+		bool changed = true;
+		while (changed) {
+			changed = false;
+			const uint32_t* ll = upper_list_of(a, cur, level);
+			const uint32_t cnt = min(ll[0], uint32_t(kMaxNeighbours));
+			for (uint32_t j = lane; j < cnt; j += 32) {
+				s_ids[j] = ll[1 + j];
+			}
+			__syncwarp();
+			n_hops++;
+			n_dist += cnt;
+			if (cnt) {
+				warp_dists<kIsL2>(a, sq4, s_ids, cnt, s_d, lane, qcorr, qcoef);
+			}
+			for (uint32_t j = 0; j < cnt; ++j) {
+				const float d = s_d[j];
+				if (d < curdist) {
+					curdist = d;
+					cur = s_ids[j];
+					changed = true;
+				}
+			}
+			__syncwarp();
+		}
+	}
+}
+
+// the batched visited test of list ll's first cnt neighbours: atomicOr on the warp's bitmap, the fresh ones to s_ids in neighbour order
+// and to the visited log (entries past kVlogCap are counted, not kept).  Returns the number of fresh neighbours.
+__device__ __forceinline__ uint32_t gather_fresh(const uint32_t* ll, uint32_t cnt, uint32_t* visited, uint32_t* vlog, uint32_t& vcount,
+												 uint32_t* s_ids, int lane) {
+	uint32_t ucnt = 0;
+	for (uint32_t b = 0; b < cnt; b += 32) {
+		const uint32_t j = b + lane;
+		uint32_t nid = 0;
+		bool fresh = false;
+		if (j < cnt) {
+			nid = ll[1 + j];
+			const uint32_t bit = 1u << (nid & 31);
+			fresh = !(atomicOr(&visited[nid >> 5], bit) & bit);
+		}
+		const unsigned fm = __ballot_sync(0xffffffffu, fresh);
+		if (fresh) {
+			const uint32_t o = ucnt + __popc(fm & ((1u << lane) - 1u));
+			s_ids[o] = nid;
+			if (vcount + o - ucnt < kVlogCap) {
+				vlog[vcount + o - ucnt] = nid;
+			}
+		}
+		ucnt += __popc(fm);
+		vcount += __popc(fm);
+	}
+	__syncwarp();
+	return ucnt;
+}
+
+// position of the first entry of l_id[0, size) without kExpanded, -1 when every entry is expanded
+__device__ __forceinline__ int first_unexpanded(const uint32_t* l_id, uint32_t size, int lane) {
+	int pos = -1;
+	for (uint32_t b = 0; b < size && pos < 0; b += 32) {
+		const uint32_t i = b + lane;
+		const unsigned m = __ballot_sync(0xffffffffu, i < size && !(l_id[i] & kExpanded));
+		if (m) {
+			pos = int(b) + __ffs(m) - 1;
+		}
+	}
+	return pos;
+}
+
+// how many i in [0, n) satisfy pred(i), warp-wide
+template <class Pred>
+__device__ __forceinline__ uint32_t warp_count(uint32_t n, int lane, Pred pred) {
+	uint32_t c = 0;
+	for (uint32_t b = 0; b < n; b += 32) {
+		const uint32_t i = b + lane;
+		c += __popc(__ballot_sync(0xffffffffu, i < n && pred(i)));
+	}
+	return c;
+}
+
+// (d, nid) into the sorted list dist / id at p < newsize, the entries from p on shifted right (highest chunk first) within
+// [0, newsize): the last entry falls out when the list does not grow
+__device__ __forceinline__ void list_insert(float* dist, uint32_t* id, uint32_t p, uint32_t newsize, float d, uint32_t nid, int lane) {
+	for (int b = int((newsize - 1) / 32) * 32; b >= 0; b -= 32) {
+		const uint32_t i = uint32_t(b) + lane;
+		const bool mv = i > p && i < newsize;
+		float td = 0.f;
+		uint32_t ti = 0;
+		if (mv) {
+			td = dist[i - 1];
+			ti = id[i - 1];
+		}
+		__syncwarp();
+		if (mv) {
+			dist[i] = td;
+			id[i] = ti;
+		}
+		__syncwarp();
+	}
+	if (lane == 0) {
+		dist[p] = d;
+		id[p] = nid;
+	}
+	__syncwarp();
+}
+
 }  // namespace
 
 // per-query state of a batched range search (hnsw.cu)
@@ -232,3 +364,34 @@ inline uint32_t hnswSlots(const rxgpu_index* ix) {
 	const uint32_t perSm = e ? std::max(1, std::min(16, std::atoi(e))) : 8u;
 	return uint32_t(ix->sm_count) * perSm * kHnswWarps;
 }
+
+namespace rxgpu {
+// errLogic unless ix holds a graph made at its current version (hnsw.cu)
+int checkGraph(const rxgpu_index* ix);
+// sizes h's graph arrays for capNodes nodes, the upper slab for upperEntries words plus room for appended nodes, and sizes and zeroes
+// the search scratch (hnsw.cu); h->M and h->maxM0 are set
+int allocGraph(const rxgpu_index* ix, rxgpu_hnsw_device* h, size_t capNodes, size_t upperEntries);
+}  // namespace rxgpu
+
+namespace {
+// the rows and graph h of ix, as the search, streaming and build kernels read them
+inline HnswArgs graphArgs(const rxgpu_index* ix, const rxgpu_hnsw_device* h) {
+	HnswArgs a{};
+	a.rows = ix->d_rows;
+	a.norm_coefs = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
+	a.level0 = h->level0.p;
+	a.levels = h->levels.p;
+	a.upper_off = h->upper_off.p;
+	a.upper = h->upper.p;
+	a.deleted = h->num_deleted ? h->deleted.p : nullptr;  // num_deleted_ == 0 -> the bare-bone search (hnswalg.h:1982)
+	a.pitch = ix->pitch;
+	a.dim = ix->dim;
+	a.n = h->n;
+	a.l0_stride = 1 + h->maxM0;
+	a.up_stride = 1 + h->M;
+	a.maxlevel = h->maxlevel;
+	a.enterpoint = h->enterpoint;
+	a.words = h->words;
+	return a;
+}
+}  // namespace
