@@ -150,7 +150,8 @@ int rxgpu_comm_create(rxgpu_comm** out, int nranks, int rank, const void* id /* 
 /* the ranks of ONE process (a reindexer process that drives several GPUs: one host thread per rank; the devices may repeat, which is
  * how a one-GPU box exercises the cross-shard paths): out[0..nranks) receive the communicators, rank r on devices[r] (NULL = all on
  * device 0).  Their exchanges go through host memory behind a rendezvous; every rank must make the same collective calls, each from its
- * own thread.  Serves rxgpu_sharded_search_knn, rxgpu_sharded_search_range_batch and rxgpu_sharded_ft_select. */
+ * own thread.  Serves rxgpu_sharded_search_knn, rxgpu_sharded_search_range_batch, rxgpu_sharded_ft_select, rxgpu_sharded_ivf_train,
+ * rxgpu_sharded_ivf_search_knn and rxgpu_sharded_ivf_search_range_batch. */
 int rxgpu_comm_create_local(rxgpu_comm** out, int nranks, const int* devices);
 void rxgpu_comm_destroy(rxgpu_comm*);
 int rxgpu_comm_rank(const rxgpu_comm*);
@@ -458,6 +459,54 @@ int rxgpu_ivf_add_assign(rxgpu_index*, uint64_t n, const uint64_t* labels, const
  * each initial centroid copies (out_init, nlist entries: sample[perm[c]] with perm = rand_perm(sample size, seed + 1), or c when the
  * sample size equals nlist). */
 int rxgpu_kmeans_plan(uint64_t n, uint32_t nlist, int32_t seed, int32_t max_points_per_centroid, int32_t* out_sample, int32_t* out_init);
+
+/* ---------------------------------------------------------------- multi-GPU IVF: one shard per GPU / rank over the same centroids
+ * Shard r holds a row range of the namespace in its own index, with IVF lists over the SAME centroids on every rank: the ranks train once
+ * (rxgpu_sharded_ivf_train), each fills its lists with rxgpu_ivf_add_assign (a row's list is a function of the centroids alone, so it is
+ * the list a single index would give it), and the searches below answer from all shards.  All three are collectives over an
+ * rxgpu_comm (NCCL, or rxgpu_comm_create_local's threads): every rank calls them with the same arguments except its own rows / shard.
+ * The exchanges and their sizes are in DESIGN.md §7.
+ *
+ * rxgpu_sharded_ivf_train: every rank leaves its index exactly as rxgpu_ivf_train leaves an index trained on the concatenation of all
+ * ranks' rows in rank order -- the same centroids and per-iteration obj / nsplit, bit for bit, on every rank.  The ranks all-gather their
+ * row counts and parameters; each prepares the sample entries it owns (rxgpu_kmeans_plan over the global rows, Cosine normalised as
+ * rxgpu_ivf_train does), one all-gather assembles the whole sample in plan order on every rank (each rank keeps it all, as one GPU
+ * does), each iteration assigns an even slice of the sample per rank and all-gathers the keys, and every rank runs the same update.
+ * stats[i].assign_ms is this rank's slice; obj and nsplit are global.  When the sample is exactly nlist rows, the centroids are the first
+ * nlist rows of the concatenation, as rxgpu_ivf_train (and FAISS) take them.  Errors are agreed: ranks that disagree on nlist, dim,
+ * metric or the parameters all return errParams; an error of one rank's own (its index not empty, a shard on another device than its
+ * communicator, NaN or Inf in its rows, device memory short for the training -- counted for every rank that shares its device) reaches
+ * every rank before the sample moves, and all return that code.  The other errors are rxgpu_ivf_train's, on the whole input.  On any
+ * of these every index is unchanged.  Not agreed, as in any collective: a null communicator or index, and a failure inside an exchange
+ * or of an allocation after the agreement (memory taken by something else meanwhile) -- that rank returns errSystem and its peers wait. */
+int rxgpu_sharded_ivf_train(rxgpu_comm*, rxgpu_index* shard, uint32_t nlist, uint64_t n_local, const float* vecs_local /* n_local x dim, host */,
+							const float* norm_coefs_local /* Cosine: n_local or NULL */, const rxgpu_ivf_train_params* params,
+							float* out_centroids /* nlist x dim or NULL */, rxgpu_ivf_train_stats* stats /* niter or NULL */);
+/* The sharded rxgpu_ivf_search_knn_large_k: any k in [1, 65535], any nprobe.  Each rank runs the coarse pass and its own best k under
+ * (distance, local row), one all-gather ships the lists, a device merge keeps the k best under (distance, global row) with the shards'
+ * rows laid end to end in rank order, and the survivors are ordered by (distance, label).  On every rank the answer has the labels,
+ * order and distance bits of rxgpu_ivf_search_knn_large_k on one index holding all rows in the same lists whenever the k-th place is
+ * not tied; when it is, the tied rows of the lower rank (then the lower local row) are kept.  With one rank it is that call's answer,
+ * bit for bit.  queries: nq x dim, host (queries_on_device == 0) or device pointer on the shard's GPU.  out_*: host, nq x k;
+ * out_count[q] = min(k, probed rows over all shards).  Every rank's payload carries a fingerprint of its centroids, nlist, nprobe, k,
+ * dim and metric: if they differ, every rank returns errLogic; an error in one rank's local IVF search (no lists, lists stale, device
+ * memory short for it) reaches every rank the same way.  Not agreed, as in any collective -- that rank returns alone and its peers wait
+ * in the all-gather: an argument error (null pointer, a shard on another device than its communicator, k outside [1, 65535]; every
+ * rank passes the same k, so that one is all ranks' error) and a failure to allocate the exchange buffers, 16·nq·k bytes to send and
+ * R times that to receive per rank (1.07 GB and 8.6 GB at nq = 1024, k = 65535, 8 ranks). */
+int rxgpu_sharded_ivf_search_knn(rxgpu_comm*, const rxgpu_index* shard, uint32_t nq, const float* queries, int queries_on_device, uint32_t k,
+								 uint32_t nprobe, float* out_dist, uint64_t* out_label, uint32_t* out_count);
+/* The sharded rxgpu_ivf_search_range_batch: per query q the result on every rank is that call's on one index holding all rows in the
+ * same lists, bit for bit -- out_n[q] = total matches, the best min(out_n[q], max_out) in the order of hitLessByLabel in row q of
+ * out_dist / out_label (host, nq x max_out; the rest of a row may be overwritten), NaN / -inf radii match nothing, +inf every probed
+ * row.  Labels must be unique across the shards.  Each rank runs the local range batch; the ranks then all-reduce the status, the
+ * width and the words every rank must agree on (the same check as the KNN call's), all-reduce the totals, all-gather the best
+ * min(matches, max_out) per query and shard, and merge them on the device -- the exchange of rxgpu_sharded_search_range_batch.  An
+ * error in one rank's local range batch reaches every rank through the first all-reduce; argument errors and a failure inside an
+ * exchange return on that rank alone, as in rxgpu_sharded_ivf_search_knn. */
+int rxgpu_sharded_ivf_search_range_batch(rxgpu_comm*, const rxgpu_index* shard, uint32_t nq, const float* queries, int queries_on_device,
+										 const float* radius /* nq, map space */, uint32_t nprobe, uint64_t max_out, float* out_dist,
+										 uint64_t* out_label, uint64_t* out_n);
 
 /* ---------------------------------------------------------------- ft_fast full-text merge (BM25 scoring over posting lists)
  * Replaces ft::Merger<IdCont, ft::MergeData, OffsetT>::Merge<Bm25Rx|Bm25Classic|TermCount>  core/ft/ft_fast/mergerimpl.h:466-566

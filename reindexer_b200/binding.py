@@ -208,6 +208,12 @@ _SIGNATURES = {
     "rxgpu_sharded_ft_select": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.POINTER(FtConfig), C.c_uint32, C.POINTER(FtTerm), _u8p, _u8p,
                                            C.c_int, C.c_uint64, _i32p, _f32p, C.POINTER(C.c_uint64)]),
     "rxgpu_comm_create_local": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.POINTER(C.c_int)]),
+    "rxgpu_sharded_ivf_train": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, _f32p, _f32p, C.POINTER(IvfTrainParams), _f32p,
+                                          C.POINTER(IvfTrainStats)]),
+    "rxgpu_sharded_ivf_search_knn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_int, C.c_uint32, C.c_uint32, _f32p, _u64p,
+                                               _u32p]),
+    "rxgpu_sharded_ivf_search_range_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_int, _f32p, C.c_uint32, C.c_uint64,
+                                                       _f32p, _u64p, _u64p]),
     "rxgpu_ft_select": (C.c_int, [C.c_void_p, C.POINTER(FtConfig), C.c_uint32, C.POINTER(FtTerm), _u8p, _u8p, C.c_int, C.c_uint64, _i32p, _f32p,
                                   C.POINTER(C.c_uint64)]),
     "rxgpu_ft_last_stats": (None, [C.POINTER(FtStats)]),
@@ -776,6 +782,51 @@ class ShardComm:
         oc = np.zeros(nq, np.uint64)
         _check(self._lib.rxgpu_sharded_search_range_batch(self._h, shard._h, nq, qp, on_dev, _p(r, _f32p), max_out, _p(od, _f32p),
                                                           _p(ol, _u64p), _p(oc, _u64p)))
+        return od[:, :max_out], ol[:, :max_out], oc
+
+    def ivf_train(self, shard: "GpuBruteforceSearch", nlist: int, vecs, norm_coefs=None, niter: int = 10, seed: int = 1234,
+                  max_points_per_centroid: int = 256):
+        """rxgpu_sharded_ivf_train: this rank's rows [n_local, dim] (a rank may have none); every rank gets what
+        GpuBruteforceSearch.ivf_train returns for the concatenation of all ranks' rows.  Collective: every rank calls it."""
+        v = np.ascontiguousarray(vecs, np.float32).reshape(-1, shard.dim)
+        nc = None if norm_coefs is None else np.ascontiguousarray(norm_coefs, np.float32)
+        prm = IvfTrainParams(niter, seed, max_points_per_centroid)
+        cent = np.zeros((max(nlist, 1), shard.dim), np.float32)
+        st = (IvfTrainStats * max(niter, 1))()
+        _check(self._lib.rxgpu_sharded_ivf_train(self._h, shard._h, nlist, len(v), _p(v, _f32p), None if nc is None else _p(nc, _f32p),
+                                                 C.byref(prm), _p(cent, _f32p), st))
+        stats = [{f: getattr(st[i], f) for f, _ in IvfTrainStats._fields_} for i in range(max(niter, 0))]
+        return cent[:nlist], stats
+
+    def ivf_search_knn(self, shard: "GpuBruteforceSearch", queries, k: int, nprobe: int, nq: int | None = None):
+        """rxgpu_sharded_ivf_search_knn.  queries: host ndarray [nq, dim] or a device pointer (int) with nq given.  Returns
+        (dists [nq, k], labels [nq, k], counts [nq]).  Collective: every rank calls it."""
+        if isinstance(queries, np.ndarray):
+            q = np.ascontiguousarray(queries, np.float32).reshape(-1, shard.dim)
+            nq, qp, on_dev = q.shape[0], q.ctypes.data_as(C.c_void_p), 0
+        else:
+            qp, on_dev = C.c_void_p(int(queries)), 1
+        od = np.zeros((nq, max(k, 1)), np.float32)
+        ol = np.zeros((nq, max(k, 1)), np.uint64)
+        oc = np.zeros(nq, np.uint32)
+        _check(self._lib.rxgpu_sharded_ivf_search_knn(self._h, shard._h, nq, qp, on_dev, k, nprobe, _p(od, _f32p), _p(ol, _u64p), _p(oc, _u32p)))
+        return od, ol, oc
+
+    def ivf_search_range_batch(self, shard: "GpuBruteforceSearch", queries, radius, nprobe: int, max_out: int, nq: int | None = None):
+        """rxgpu_sharded_ivf_search_range_batch.  queries: host ndarray [nq, dim] or a device pointer (int) with nq given; radius: a
+        scalar or [nq] (map space).  Returns (dists [nq, max_out], labels [nq, max_out], counts [nq]) as
+        GpuBruteforceSearch.ivf_search_range_batch returns them for one index holding every shard's rows.  Collective."""
+        if isinstance(queries, np.ndarray):
+            q = np.ascontiguousarray(queries, np.float32).reshape(-1, shard.dim)
+            nq, qp, on_dev = q.shape[0], q.ctypes.data_as(C.c_void_p), 0
+        else:
+            qp, on_dev = C.c_void_p(int(queries)), 1
+        r = np.ascontiguousarray(np.broadcast_to(np.asarray(radius, dtype=np.float32), (nq,)))
+        od = np.zeros((nq, max(max_out, 1)), np.float32)
+        ol = np.zeros((nq, max(max_out, 1)), np.uint64)
+        oc = np.zeros(nq, np.uint64)
+        _check(self._lib.rxgpu_sharded_ivf_search_range_batch(self._h, shard._h, nq, qp, on_dev, _p(r, _f32p), nprobe, max_out, _p(od, _f32p),
+                                                              _p(ol, _u64p), _p(oc, _u64p)))
         return od[:, :max_out], ol[:, :max_out], oc
 
 

@@ -377,6 +377,23 @@ int ivfCheckCoarseDim(uint32_t dim);
 cudaError_t ivfAssignRows(const rxgpu_index* ix, const float* centroids, const float* cnorm, uint32_t nlist, const float* x, uint32_t n,
 						  uint64_t* keys, cudaStream_t st);
 constexpr uint32_t kIvfMaxCentroids = 1u << 17;  // the reference's centroids_count bound (kIvfNCentroidsMax, indexopts.cc)
+// the local parts of the sharded IVF searches (shard.cu), each after rxgpu_ivf_search_*'s own checks.  `view` receives what the ranks
+// must agree on: a fingerprint of the centroids, nlist, nprobe as clamped, and the rows the lists address (the shard's size in the merge)
+struct IvfShardView {
+	uint64_t fingerprint;
+	uint32_t nlist, nprobe;
+	uint64_t rows;
+};
+// the best min(k, probed rows) rows of every query under (distance, local internal row), in that order, into the device rows
+// d_*[q * stride, + d_count[q]): the coarse pass, then the fused top-k or the key pass and exact select, as
+// rxgpu_ivf_search_knn_large_k chooses.  Done (synchronised) on return.
+int ivfShardKnn(const rxgpu_index* ix, uint32_t nq, const float* queries, uint32_t k, uint32_t nprobe, uint32_t stride, float* d_dist,
+				uint32_t* d_idx, uint64_t* d_label, uint32_t* d_count, IvfShardView& view);
+// rxgpu_ivf_search_range_batch without its output step: emit(q, n, dist, label, m) once per query with its n matches and the best
+// m = min(n, max_out) of them, in the order of hitLessByLabel (host arrays, valid during the call)
+using IvfRangeEmit = std::function<void(uint32_t q, uint64_t n, const float* dist, const uint64_t* label, uint64_t m)>;
+int ivfShardRange(const rxgpu_index* ix, uint32_t nq, const float* queries, const float* radius, uint32_t nprobe, uint64_t max_out,
+				  const IvfRangeEmit& emit, IvfShardView& view);
 
 // writes row `idx` (== size: appends) with a new vector and label, keeping the label dictionary consistent (index.cu)
 int setRowAt(rxgpu_index* ix, uint32_t idx, uint64_t label, const float* vec);

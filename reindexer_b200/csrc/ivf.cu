@@ -9,6 +9,7 @@
 #include <cub/device/device_segmented_sort.cuh>
 
 #include <algorithm>
+#include <functional>
 #include <limits>
 #include <memory>
 #include <mutex>
@@ -89,6 +90,7 @@ struct rxgpu_ivf_device {
 	DevBuf<uint32_t> st_dst;
 	DevBuf<uint64_t> st_labels;
 	uint64_t relocations = 0, compactions = 0;
+	uint64_t fingerprint = 0;  // of the centroids, made by the first sharded search (ivfShardView); 0: not yet
 };
 namespace rxgpu {
 void ivfRelease(rxgpu_ivf_device* p) { delete p; }
@@ -182,7 +184,7 @@ dim3 coarseGrid(const rxgpu_index* ix, uint32_t nlist, uint32_t cq, int qt) {
 	const uint32_t slices = std::max(1u, std::min((groups + kScanWarps - 1) / kScanWarps, (uint32_t(ix->sm_count) * 4 + tiles - 1) / tiles));
 	return dim3(tiles, slices);
 }
-// the coarse quantiser (ivf_coarse.cuh) over nq host queries, staged in h->d_q: work items of the list scans in h->d_work, probe-major.
+// the coarse quantiser (ivf_coarse.cuh) over nq queries (host, or device on the index's GPU), staged in h->d_q: work items of the list scans in h->d_work, probe-major.
 // Per query chunk of at most kIvfKeyCap keys: distances, select, sort, emit (4 launches, counted in g_stats with the centroid bytes, read
 // once per query tile).  The chunk's keys go to h->d_keys, its survivors to h->d_sel_label: the key pass and the selects that follow
 // reuse them.  A batch stages kCoarseTile queries per tile (dim <= 3 200), one query stages itself alone.
@@ -190,7 +192,7 @@ int ivfLaunchCoarse(const rxgpu_index* ix, rxgpu_ivf_device* h, uint32_t nq, con
 	const uint32_t nlist = h->nlist;
 	RX_CUDA(h->d_q.ensure(size_t(nq) * ix->dim));
 	RX_CUDA(h->d_work.ensure(size_t(nq) * nprobe));
-	RX_CUDA(cudaMemcpyAsync(h->d_q.p, queries, size_t(nq) * ix->dim * 4, cudaMemcpyHostToDevice, st));
+	RX_CUDA(cudaMemcpyAsync(h->d_q.p, queries, size_t(nq) * ix->dim * 4, cudaMemcpyDefault, st));  // host or device queries
 	const int qt = coarseTile(ix, nq);
 	const size_t smem = coarse_smem_bytes(qt, ix->dim);
 	const uint32_t chunk = uint32_t(std::max<uint64_t>(1, kIvfKeyCap / nlist));
@@ -299,6 +301,241 @@ int ivfSortSurvivors(rxgpu_ivf_device* h, int n, int nseg, int* begin, int* end,
 													 h->d_sel_label.p, n, nseg, begin, end, 0, 32, st));
 	return 0;
 }
+
+// The fused path of rxgpu_ivf_search_knn (k <= kMaxFusedK1, nprobe <= 256 * kMergeOwn), under h->mtx: the coarse pass, the list scans
+// with a fused top-k per (query, probed list), and one merge into out_* (rows of `stride` entries) under (distance, internal row),
+// bit-equal distances not yet ordered by label.  Device outputs, enqueued on st.
+int ivfFusedKnn(const rxgpu_index* ix, rxgpu_ivf_device* h, const IvfRows& r, uint32_t nq, const float* queries, uint32_t k, uint32_t nprobe,
+				uint32_t stride, float* out_dist, uint32_t* out_idx, uint64_t* out_label, uint32_t* out_count, cudaStream_t st) {
+	const size_t nwork = size_t(nq) * nprobe;
+	RX_CUDA(h->d_lists.ensure(nwork * k));
+	if (int rc = ivfLaunchCoarse(ix, h, nq, queries, nprobe, st)) {
+		return rc;
+	}
+	// list scans: the exact scan kernel in work-item mode, one CTA per (query, probed list), fused top-k per CTA
+	ScanArgs a = ivfScanArgs(ix, h, r, h->d_work.p, uint32_t(nwork), k, kModeTopK);
+	a.lists = h->d_lists.p;
+	if (scan_smem_bytes(1, ix->dim, k) > 100 * 1024) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: dimension/k combination exceeds the fused top-k shared-memory budget");
+	}
+	unsigned grid = 0;
+	RX_CUDA(launchScan(ix, 1, a, &grid, st));
+	MergeArgs m{};
+	m.lists = h->d_lists.p;
+	m.labels = r.labels;
+	m.out_dist = out_dist;
+	m.out_idx = out_idx;
+	m.out_label = out_label;
+	m.out_count = out_count;
+	m.nlists = nprobe;
+	m.qt = nq;  // lists are probe-major: list of (probe p, query q) = p * nq + q
+	m.k1 = k;
+	m.q_offset = 0;
+	m.out_stride = stride;
+	m.out_offset = 0;
+	m.mode = kModeTopK;
+	RX_CUDA(launchMergeLists(m, nq, st));
+	g_stats.launches += 2;  // list scans, merge (the coarse pass counts its own)
+	g_stats.passes = 1;
+	return 0;
+}
+
+// called once per query chunk [q0, q0 + cq) with its nkeys probed rows: the chunk's survivors are in h->d_sel_ord / d_sel_label
+// ([cq][k]), h->d_sel_count holds how many each query kept
+using IvfChunkDone = std::function<int(uint32_t q0, uint32_t cq, uint64_t nkeys)>;
+
+// The any-k select of rxgpu_ivf_search_knn_large_k, under h->mtx: the coarse pass over the nq queries, then per query chunk the key pass
+// and the exact select of the k smallest keys ((distance, internal row)), their survivors ordered by (distance word, selLabels' word)
+// -- selLabels = the rows' labels, or nullptr for the rows themselves -- and handed to `done`.  Adds launches and bytes to g_stats.
+int ivfSelectChunks(const rxgpu_index* ix, rxgpu_ivf_device* h, const IvfRows& r, uint32_t nq, const float* queries, uint32_t k, uint32_t nprobe,
+					const uint64_t* selLabels, const IvfChunkDone& done, cudaStream_t st) {
+	uint32_t launches = 2;  // probed rows, their scan (one CUB call); the coarse pass counts its own
+	std::vector<uint64_t> rows, off;
+	if (int rc = ivfProbedRows(ix, h, nq, queries, nprobe, st, rows, off)) {
+		return rc;
+	}
+	// query chunks: at most kIvfKeyCap keys and kIvfSlotCap survivor slots each; a query above the key cap is a chunk of its own
+	for (uint32_t q0 = 0, q1 = 0; q0 < nq; q0 = q1) {
+		q1 = ivfChunkEnd(off, q0, k);
+		const uint32_t cq = q1 - q0;
+		const uint64_t nkeys = off[q1] - off[q0];
+		const size_t slots = size_t(cq) * k;
+		RX_CUDA(h->d_sel_ord.ensure(slots));
+		RX_CUDA(h->d_sel_ord2.ensure(slots));
+		RX_CUDA(h->d_sel_label.ensure(slots));
+		RX_CUDA(h->d_sel_label2.ensure(slots));
+		RX_CUDA(h->d_sel_count.ensure(cq));
+		RX_CUDA(h->d_seg_begin.ensure(cq));
+		RX_CUDA(h->d_seg_end.ensure(cq));
+		RX_CUDA(cudaMemsetAsync(h->d_sel_count.p, 0, size_t(cq) * 4, st));
+		if (nkeys) {
+			if (int rc = ivfKeyPass(ix, h, r, nq, nprobe, q0, cq, nkeys, st)) {
+				return rc;
+			}
+			ivf_select_cta_kernel<<<cq, kIvfSelThreads, 0, st>>>(h->d_keys.p, h->d_qoff.p + q0, h->d_qrows.p + q0, off[q0], k, selLabels,
+															  h->d_sel_ord.p, h->d_sel_label.p, h->d_sel_count.p);
+			RX_CUDA(cudaGetLastError());
+			launches += 3;
+			for (uint32_t qi = 0; qi < cq; ++qi) {  // queries with many keys: the same select over many CTAs
+				const uint64_t n = rows[q0 + qi];
+				if (n <= kIvfSelCtaKeys) {
+					continue;
+				}
+				RX_CUDA(h->d_sel_state.ensure(1));
+				RX_CUDA(h->d_sel_hist.ensure(kIvfSelBins));
+				const SelState init{0ull, kKeyNone, k, 0u};
+				RX_CUDA(cudaMemcpyAsync(h->d_sel_state.p, &init, sizeof(init), cudaMemcpyHostToDevice, st));
+				RX_CUDA(cudaMemsetAsync(h->d_sel_hist.p, 0, kIvfSelBins * 4, st));
+				const uint64_t* kq = h->d_keys.p + (off[q0 + qi] - off[q0]);
+				const unsigned g = unsigned(std::min<uint64_t>((n + 16 * kIvfSelThreads - 1) / (16 * kIvfSelThreads), uint64_t(ix->sm_count) * 2));
+				for (int pass = 0; pass < kIvfSelPasses; ++pass) {
+					ivf_select_hist_kernel<<<g, kIvfSelThreads, 0, st>>>(kq, n, h->d_sel_state.p, pass, h->d_sel_hist.p);
+					ivf_select_pick_kernel<<<1, kIvfSelThreads, 0, st>>>(h->d_sel_state.p, pass, h->d_sel_hist.p);
+				}
+				ivf_select_compact_kernel<<<g, kIvfSelThreads, 0, st>>>(kq, n, h->d_sel_state.p, selLabels, h->d_sel_ord.p + size_t(qi) * k,
+																	 h->d_sel_label.p + size_t(qi) * k, h->d_sel_count.p + qi);
+				RX_CUDA(cudaGetLastError());
+				launches += 2 * kIvfSelPasses + 1;
+			}
+			// order the survivors by (distance, label): stable radix sorts by label, then by the ordered distance word
+			ivf_sort_bounds_kernel<<<(cq + 255u) / 256u, 256, 0, st>>>(h->d_sel_count.p, k, cq, h->d_seg_begin.p, h->d_seg_end.p);
+			RX_CUDA(cudaGetLastError());
+			if (int rc = ivfSortSurvivors(h, int(slots), int(cq), h->d_seg_begin.p, h->d_seg_end.p, st)) {
+				return rc;
+			}
+			launches += 3;
+		}
+		if (int rc = done(q0, cq, nkeys)) {
+			return rc;
+		}
+	}
+	const uint64_t probed = off[nq];
+	g_stats.launches += launches;
+	g_stats.passes = 1;
+	// rows read once; each key written once and read once by the select
+	g_stats.algorithmic_bytes += probed * ix->dim * 4 + (ix->metric == RXGPU_COS ? probed * 4 : 0) + probed * 16;
+	return 0;
+}
+
+// The range batch of rxgpu_ivf_search_range_batch, under h->mtx (arguments checked): one coarse pass and one key pass per key chunk; each
+// query's matches counted, kept, sorted by (distance, label) and gathered on the device.  emit(q, n, dist, label, m) once per query with
+// its n matches in total and the best m = min(n, max_out) of them, best first (host arrays, valid during the call).
+int ivfRangeBatch(const rxgpu_index* ix, rxgpu_ivf_device* h, uint32_t nq, const float* queries, const float* radius, uint32_t nprobe,
+				  uint64_t max_out, const IvfRangeEmit& emit) {
+	cudaStream_t st = ix->stream;
+	const IvfRows r = ivfRows(ix, h);
+	uint32_t launches = 2;  // probed rows, their scan; the coarse pass counts its own
+	std::vector<uint64_t> rows, off;
+	if (int rc = ivfProbedRows(ix, h, nq, queries, nprobe, st, rows, off)) {
+		return rc;
+	}
+	RX_CUDA(h->d_radius.ensure(nq));
+	RX_CUDA(cudaMemcpyAsync(h->d_radius.p, radius, size_t(nq) * 4, cudaMemcpyHostToDevice, st));
+	std::vector<uint2> tiles;
+	std::vector<size_t> tileAt;
+	std::vector<uint32_t> cnt;
+	std::vector<int> plan;
+	std::vector<float> dist;
+	std::vector<uint64_t> lab;
+	// the key chunks of the any-k select (no survivor slots to bound yet: a query's matches are counted before they are kept)
+	for (uint32_t q0 = 0, q1 = 0; q0 < nq; q0 = q1) {
+		q1 = ivfChunkEnd(off, q0, 0);
+		const uint32_t cq = q1 - q0;
+		const uint64_t nkeys = off[q1] - off[q0];
+		if (nkeys == 0) {
+			for (uint32_t q = q0; q < q1; ++q) {
+				emit(q, 0, nullptr, nullptr, 0);
+			}
+			continue;
+		}
+		if (int rc = ivfKeyPass(ix, h, r, nq, nprobe, q0, cq, nkeys, st)) {
+			return rc;
+		}
+		tiles.clear();
+		tileAt.assign(size_t(cq) + 1, 0);
+		for (uint32_t qi = 0; qi < cq; ++qi) {
+			for (uint64_t j = 0; j * kIvfRangeTile < rows[q0 + qi]; ++j) {
+				tiles.push_back(make_uint2(qi, uint32_t(j)));
+			}
+			tileAt[qi + 1] = tiles.size();
+		}
+		RX_CUDA(h->d_tiles.ensure(tiles.size()));
+		RX_CUDA(h->d_range_n.ensure(cq));
+		RX_CUDA(h->d_sel_count.ensure(cq));
+		RX_CUDA(cudaMemcpyAsync(h->d_tiles.p, tiles.data(), tiles.size() * sizeof(uint2), cudaMemcpyHostToDevice, st));
+		RX_CUDA(cudaMemsetAsync(h->d_range_n.p, 0, size_t(cq) * 4, st));
+		RX_CUDA(cudaMemsetAsync(h->d_sel_count.p, 0, size_t(cq) * 4, st));
+		ivf_range_count_kernel<<<unsigned(tiles.size()), kIvfRangeThreads, 0, st>>>(
+			h->d_keys.p, h->d_qoff.p + q0, h->d_qrows.p + q0, off[q0], h->d_radius.p + q0, h->d_tiles.p, h->d_range_n.p);
+		RX_CUDA(cudaGetLastError());
+		launches += 3;  // key plan, key scan, count
+		cnt.resize(cq);
+		RX_CUDA(cudaMemcpyAsync(cnt.data(), h->d_range_n.p, size_t(cq) * 4, cudaMemcpyDeviceToHost, st));
+		RX_CUDA(cudaStreamSynchronize(st));
+		// survivor sub-chunks of at most kIvfSlotCap matches; a query with more is a sub-chunk of its own.  Without max_out nothing is kept.
+		for (uint32_t s0 = 0, s1 = 0; s0 < cq; s0 = s1) {
+			uint64_t total = cnt[s0];
+			for (s1 = s0 + 1; s1 < cq && total + cnt[s1] <= kIvfSlotCap; ++s1) {
+				total += cnt[s1];
+			}
+			if (total == 0 || max_out == 0) {
+				for (uint32_t i = s0; i < s1; ++i) {
+					emit(q0 + i, cnt[i], nullptr, nullptr, 0);
+				}
+				continue;
+			}
+			if (total > uint64_t(std::numeric_limits<int>::max())) {  // the segmented sorts count items in an int
+				return fail(RXGPU_ERR_PARAMS, "rxgpu: more than 2^31 - 1 range matches for one IVF query");
+			}
+			const uint32_t ns = s1 - s0;
+			plan.assign(2 * (size_t(ns) + 1), 0);
+			int* seg = plan.data();     // survivors of query s0 + i: [seg[i], seg[i + 1])
+			int* pack = seg + ns + 1;   // its best min(matches, max_out) in the packed output: [pack[i], pack[i + 1])
+			int longest = 0;
+			for (uint32_t i = 0; i < ns; ++i) {
+				const int m = int(std::min<uint64_t>(cnt[s0 + i], max_out));
+				seg[i + 1] = seg[i] + int(cnt[s0 + i]);
+				pack[i + 1] = pack[i] + m;
+				longest = std::max(longest, m);
+			}
+			RX_CUDA(h->d_range_seg.ensure(plan.size()));
+			RX_CUDA(h->d_sel_ord.ensure(total));
+			RX_CUDA(h->d_sel_ord2.ensure(total));
+			RX_CUDA(h->d_sel_label.ensure(total));
+			RX_CUDA(h->d_sel_label2.ensure(total));
+			RX_CUDA(cudaMemcpyAsync(h->d_range_seg.p, plan.data(), plan.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+			int* dseg = h->d_range_seg.p;
+			const int* dpack = dseg + ns + 1;
+			ivf_range_emit_kernel<<<unsigned(tileAt[s1] - tileAt[s0]), kIvfRangeThreads, 0, st>>>(
+				h->d_keys.p, h->d_qoff.p + q0, h->d_qrows.p + q0, off[q0], h->d_radius.p + q0, h->d_tiles.p + tileAt[s0], s0, dseg, r.labels,
+				h->d_sel_count.p, h->d_sel_ord.p, h->d_sel_label.p);
+			RX_CUDA(cudaGetLastError());
+			if (int rc = ivfSortSurvivors(h, int(total), int(ns), dseg, dseg + 1, st)) {
+				return rc;
+			}
+			// the packed output goes to the sorts' second buffers, free again once the sorts are done
+			float* pdist = reinterpret_cast<float*>(h->d_sel_ord2.p);
+			const dim3 gg(ns, unsigned(std::min(1024, (longest + 255) / 256)));
+			ivf_range_gather_kernel<<<gg, 256, 0, st>>>(h->d_sel_ord.p, h->d_sel_label.p, dseg, dpack, pdist, h->d_sel_label2.p);
+			RX_CUDA(cudaGetLastError());
+			launches += 4;  // emit, two sorts, gather
+			dist.resize(size_t(pack[ns]));
+			lab.resize(size_t(pack[ns]));
+			RX_CUDA(cudaMemcpyAsync(dist.data(), pdist, dist.size() * 4, cudaMemcpyDeviceToHost, st));
+			RX_CUDA(cudaMemcpyAsync(lab.data(), h->d_sel_label2.p, lab.size() * 8, cudaMemcpyDeviceToHost, st));
+			RX_CUDA(cudaStreamSynchronize(st));
+			for (uint32_t i = 0; i < ns; ++i) {
+				emit(q0 + s0 + i, cnt[s0 + i], dist.data() + pack[i], lab.data() + pack[i], uint64_t(pack[i + 1] - pack[i]));
+			}
+		}
+	}
+	const uint64_t probed = off[nq];
+	g_stats.launches += launches;
+	g_stats.passes = 1;
+	// as rxgpu_ivf_search_knn_large_k: rows read once; each key written once and read once
+	g_stats.algorithmic_bytes += probed * ix->dim * 4 + (ix->metric == RXGPU_COS ? probed * 4 : 0) + probed * 16;
+	return 0;
+}
 }  // namespace
 
 namespace rxgpu {
@@ -316,6 +553,77 @@ cudaError_t ivfAssignRows(const rxgpu_index* ix, const float* centroids, const f
 	}
 	return qt == 1 ? launchCoarseDist<false, 1, true>(ix, centroids, nlist, grid, smem, x, n, cnorm, keys, st)
 				   : launchCoarseDist<false, kCoarseTile, true>(ix, centroids, nlist, grid, smem, x, n, cnorm, keys, st);
+}
+}  // namespace rxgpu
+
+namespace {
+// the view a sharded search compares across ranks, after ivfSearchChecks: a 64-bit FNV-1a of the centroids' bits (made once: the
+// centroids never change while the lists exist), nlist, the clamped nprobe, and the rows the lists address (the shard's size in the
+// (rank, local row) order the merge cuts ties by)
+int ivfShardView(const rxgpu_index* ix, rxgpu_ivf_device* h, uint32_t nprobe, IvfShardView& v) {
+	if (!h->fingerprint) {
+		std::vector<uint32_t> hc(size_t(h->nlist) * ix->dim);
+		RX_CUDA(cudaMemcpy2DAsync(hc.data(), size_t(ix->dim) * 4, h->centroids.p, size_t(ix->pitch) * 4, size_t(ix->dim) * 4, h->nlist,
+								  cudaMemcpyDeviceToHost, ix->stream));
+		RX_CUDA(cudaStreamSynchronize(ix->stream));
+		uint64_t f = 0xcbf29ce484222325ull;
+		for (const uint32_t w : hc) {
+			f = (f ^ w) * 0x100000001b3ull;
+		}
+		h->fingerprint = f ? f : 1;
+	}
+	v = IvfShardView{h->fingerprint, h->nlist, nprobe, h->own ? h->high_water : ix->size};
+	return 0;
+}
+}  // namespace
+
+namespace rxgpu {
+int ivfShardKnn(const rxgpu_index* ix, uint32_t nq, const float* queries, uint32_t k, uint32_t nprobe, uint32_t stride, float* d_dist,
+				uint32_t* d_idx, uint64_t* d_label, uint32_t* d_count, IvfShardView& view) {
+	if (int rc = ivfSearchChecks(ix, k, kMaxLargeK, UINT32_MAX, nprobe)) {
+		return rc;
+	}
+	rxgpu_ivf_device* h = ix->ivf;
+	std::lock_guard<std::mutex> lck(h->mtx);
+	cudaStream_t st = ix->stream;
+	const IvfRows r = ivfRows(ix, h);
+	if (int rc = ivfShardView(ix, h, nprobe, view)) {
+		return rc;
+	}
+	if (k <= kMaxFusedK1 && nprobe <= 256u * kMergeOwn) {  // the path rxgpu_ivf_search_knn_large_k takes here
+		if (int rc = ivfFusedKnn(ix, h, r, nq, queries, k, nprobe, stride, d_dist, d_idx, d_label, d_count, st)) {
+			return rc;
+		}
+	} else {
+		// the survivors by (distance word, row): the select keeps rows instead of labels, the emit looks the labels up
+		const IvfChunkDone done = [&](uint32_t q0, uint32_t cq, uint64_t) -> int {
+			const uint64_t slots = uint64_t(cq) * k;
+			ivf_shard_emit_kernel<<<unsigned((slots + 255) / 256), 256, 0, st>>>(h->d_sel_ord.p, h->d_sel_label.p, h->d_sel_count.p, k, cq, r.labels,
+																			   stride, d_dist + size_t(q0) * stride, d_idx + size_t(q0) * stride,
+																			   d_label + size_t(q0) * stride, d_count + q0);
+			RX_CUDA(cudaGetLastError());
+			g_stats.launches += 1;
+			return 0;
+		};
+		if (int rc = ivfSelectChunks(ix, h, r, nq, queries, k, nprobe, nullptr, done, st)) {
+			return rc;
+		}
+	}
+	RX_CUDA(cudaStreamSynchronize(st));
+	return 0;
+}
+
+int ivfShardRange(const rxgpu_index* ix, uint32_t nq, const float* queries, const float* radius, uint32_t nprobe, uint64_t max_out,
+				  const IvfRangeEmit& emit, IvfShardView& view) {
+	if (int rc = ivfSearchChecks(ix, 0, 0, UINT32_MAX, nprobe)) {
+		return rc;
+	}
+	rxgpu_ivf_device* h = ix->ivf;
+	std::lock_guard<std::mutex> lck(h->mtx);
+	if (int rc = ivfShardView(ix, h, nprobe, view)) {
+		return rc;
+	}
+	return ivfRangeBatch(ix, h, nq, queries, radius, nprobe, max_out, emit);
 }
 }  // namespace rxgpu
 
@@ -389,40 +697,13 @@ int rxgpu_ivf_search_knn(const rxgpu_index* ix, uint32_t nq, const float* querie
 	std::lock_guard<std::mutex> lck(h->mtx);
 	cudaStream_t st = ix->stream;
 	const IvfRows r = ivfRows(ix, h);
-	const size_t nwork = size_t(nq) * nprobe;
-	RX_CUDA(h->d_lists.ensure(nwork * k));
 	RX_CUDA(h->d_dist.ensure(size_t(nq) * k));
 	RX_CUDA(h->d_idx.ensure(size_t(nq) * k));
 	RX_CUDA(h->d_label.ensure(size_t(nq) * k));
 	RX_CUDA(h->d_count.ensure(nq));
-	if (int rc = ivfLaunchCoarse(ix, h, nq, queries, nprobe, st)) {
+	if (int rc = ivfFusedKnn(ix, h, r, nq, queries, k, nprobe, k, h->d_dist.p, h->d_idx.p, h->d_label.p, h->d_count.p, st)) {
 		return rc;
 	}
-	// list scans: the exact scan kernel in work-item mode, one CTA per (query, probed list), fused top-k per CTA
-	ScanArgs a = ivfScanArgs(ix, h, r, h->d_work.p, uint32_t(nwork), k, kModeTopK);
-	a.lists = h->d_lists.p;
-	if (scan_smem_bytes(1, ix->dim, k) > 100 * 1024) {
-		return fail(RXGPU_ERR_PARAMS, "rxgpu: dimension/k combination exceeds the fused top-k shared-memory budget");
-	}
-	unsigned grid = 0;
-	RX_CUDA(launchScan(ix, 1, a, &grid, st));
-	MergeArgs m{};
-	m.lists = h->d_lists.p;
-	m.labels = r.labels;
-	m.out_dist = h->d_dist.p;
-	m.out_idx = h->d_idx.p;
-	m.out_label = h->d_label.p;
-	m.out_count = h->d_count.p;
-	m.nlists = nprobe;
-	m.qt = nq;  // lists are probe-major: list of (probe p, query q) = p * nq + q
-	m.k1 = k;
-	m.q_offset = 0;
-	m.out_stride = k;
-	m.out_offset = 0;
-	m.mode = kModeTopK;
-	RX_CUDA(launchMergeLists(m, nq, st));
-	g_stats.launches += 2;  // list scans, merge (the coarse pass counts its own)
-	g_stats.passes = 1;
 	try {
 		std::vector<float> hd(size_t(nq) * k);
 		std::vector<uint64_t> hl(size_t(nq) * k);
@@ -473,65 +754,11 @@ int rxgpu_ivf_search_knn_large_k(const rxgpu_index* ix, uint32_t nq, const float
 	std::lock_guard<std::mutex> lck(h->mtx);
 	cudaStream_t st = ix->stream;
 	const IvfRows r = ivfRows(ix, h);
-	uint32_t launches = 2;  // probed rows, their scan (one CUB call); the coarse pass counts its own
 	try {
-		std::vector<uint64_t> rows, off;
-		if (int rc = ivfProbedRows(ix, h, nq, queries, nprobe, st, rows, off)) {
-			return rc;
-		}
 		std::vector<uint32_t> ord, cnt;
 		std::vector<uint64_t> lab;
-		// query chunks: at most kIvfKeyCap keys and kIvfSlotCap survivor slots each; a query above the key cap is a chunk of its own
-		for (uint32_t q0 = 0, q1 = 0; q0 < nq; q0 = q1) {
-			q1 = ivfChunkEnd(off, q0, k);
-			const uint32_t cq = q1 - q0;
-			const uint64_t nkeys = off[q1] - off[q0];
+		const IvfChunkDone done = [&](uint32_t q0, uint32_t cq, uint64_t nkeys) -> int {
 			const size_t slots = size_t(cq) * k;
-			RX_CUDA(h->d_sel_ord.ensure(slots));
-			RX_CUDA(h->d_sel_ord2.ensure(slots));
-			RX_CUDA(h->d_sel_label.ensure(slots));
-			RX_CUDA(h->d_sel_label2.ensure(slots));
-			RX_CUDA(h->d_sel_count.ensure(cq));
-			RX_CUDA(h->d_seg_begin.ensure(cq));
-			RX_CUDA(h->d_seg_end.ensure(cq));
-			RX_CUDA(cudaMemsetAsync(h->d_sel_count.p, 0, size_t(cq) * 4, st));
-			if (nkeys) {
-				if (int rc = ivfKeyPass(ix, h, r, nq, nprobe, q0, cq, nkeys, st)) {
-					return rc;
-				}
-				ivf_select_cta_kernel<<<cq, kIvfSelThreads, 0, st>>>(h->d_keys.p, h->d_qoff.p + q0, h->d_qrows.p + q0, off[q0], k, r.labels,
-																  h->d_sel_ord.p, h->d_sel_label.p, h->d_sel_count.p);
-				RX_CUDA(cudaGetLastError());
-				launches += 3;
-				for (uint32_t qi = 0; qi < cq; ++qi) {  // queries with many keys: the same select over many CTAs
-					const uint64_t n = rows[q0 + qi];
-					if (n <= kIvfSelCtaKeys) {
-						continue;
-					}
-					RX_CUDA(h->d_sel_state.ensure(1));
-					RX_CUDA(h->d_sel_hist.ensure(kIvfSelBins));
-					const SelState init{0ull, kKeyNone, k, 0u};
-					RX_CUDA(cudaMemcpyAsync(h->d_sel_state.p, &init, sizeof(init), cudaMemcpyHostToDevice, st));
-					RX_CUDA(cudaMemsetAsync(h->d_sel_hist.p, 0, kIvfSelBins * 4, st));
-					const uint64_t* kq = h->d_keys.p + (off[q0 + qi] - off[q0]);
-					const unsigned g = unsigned(std::min<uint64_t>((n + 16 * kIvfSelThreads - 1) / (16 * kIvfSelThreads), uint64_t(ix->sm_count) * 2));
-					for (int pass = 0; pass < kIvfSelPasses; ++pass) {
-						ivf_select_hist_kernel<<<g, kIvfSelThreads, 0, st>>>(kq, n, h->d_sel_state.p, pass, h->d_sel_hist.p);
-						ivf_select_pick_kernel<<<1, kIvfSelThreads, 0, st>>>(h->d_sel_state.p, pass, h->d_sel_hist.p);
-					}
-					ivf_select_compact_kernel<<<g, kIvfSelThreads, 0, st>>>(kq, n, h->d_sel_state.p, r.labels, h->d_sel_ord.p + size_t(qi) * k,
-																		 h->d_sel_label.p + size_t(qi) * k, h->d_sel_count.p + qi);
-					RX_CUDA(cudaGetLastError());
-					launches += 2 * kIvfSelPasses + 1;
-				}
-				// order the survivors by (distance, label): stable radix sorts by label, then by the ordered distance word
-				ivf_sort_bounds_kernel<<<(cq + 255u) / 256u, 256, 0, st>>>(h->d_sel_count.p, k, cq, h->d_seg_begin.p, h->d_seg_end.p);
-				RX_CUDA(cudaGetLastError());
-				if (int rc = ivfSortSurvivors(h, int(slots), int(cq), h->d_seg_begin.p, h->d_seg_end.p, st)) {
-					return rc;
-				}
-				launches += 3;
-			}
 			ord.resize(slots);
 			lab.resize(slots);
 			cnt.resize(cq);
@@ -549,16 +776,12 @@ int rxgpu_ivf_search_knn_large_k(const rxgpu_index* ix, uint32_t nq, const float
 				}
 				out_count[q0 + qi] = cnt[qi];
 			}
-		}
-		const uint64_t probed = off[nq];
-		g_stats.launches += launches;
-		g_stats.passes = 1;
-		// rows read once; each key written once and read once by the select
-		g_stats.algorithmic_bytes += probed * ix->dim * 4 + (ix->metric == RXGPU_COS ? probed * 4 : 0) + probed * 16;
+			return 0;
+		};
+		return ivfSelectChunks(ix, h, r, nq, queries, k, nprobe, r.labels, done, st);
 	} catch (const std::bad_alloc&) {
 		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
 	}
-	return 0;
 }
 
 int rxgpu_ivf_search_range(const rxgpu_index* ix, const float* query, float radius, uint32_t nprobe, uint64_t max_out, float* out_dist,
@@ -622,126 +845,16 @@ int rxgpu_ivf_search_range_batch(const rxgpu_index* ix, uint32_t nq, const float
 	}
 	rxgpu_ivf_device* h = ix->ivf;
 	std::lock_guard<std::mutex> lck(h->mtx);
-	cudaStream_t st = ix->stream;
-	const IvfRows r = ivfRows(ix, h);
-	uint32_t launches = 2;  // probed rows, their scan; the coarse pass counts its own
 	try {
-		std::vector<uint64_t> rows, off;
-		if (int rc = ivfProbedRows(ix, h, nq, queries, nprobe, st, rows, off)) {
-			return rc;
-		}
-		RX_CUDA(h->d_radius.ensure(nq));
-		RX_CUDA(cudaMemcpyAsync(h->d_radius.p, radius, size_t(nq) * 4, cudaMemcpyHostToDevice, st));
-		std::vector<uint2> tiles;
-		std::vector<size_t> tileAt;
-		std::vector<uint32_t> cnt;
-		std::vector<int> plan;
-		std::vector<float> dist;
-		std::vector<uint64_t> lab;
-		// the key chunks of the any-k select (no survivor slots to bound yet: a query's matches are counted before they are kept)
-		for (uint32_t q0 = 0, q1 = 0; q0 < nq; q0 = q1) {
-			q1 = ivfChunkEnd(off, q0, 0);
-			const uint32_t cq = q1 - q0;
-			const uint64_t nkeys = off[q1] - off[q0];
-			if (nkeys == 0) {
-				std::fill(out_n + q0, out_n + q1, uint64_t(0));
-				continue;
-			}
-			if (int rc = ivfKeyPass(ix, h, r, nq, nprobe, q0, cq, nkeys, st)) {
-				return rc;
-			}
-			tiles.clear();
-			tileAt.assign(size_t(cq) + 1, 0);
-			for (uint32_t qi = 0; qi < cq; ++qi) {
-				for (uint64_t j = 0; j * kIvfRangeTile < rows[q0 + qi]; ++j) {
-					tiles.push_back(make_uint2(qi, uint32_t(j)));
-				}
-				tileAt[qi + 1] = tiles.size();
-			}
-			RX_CUDA(h->d_tiles.ensure(tiles.size()));
-			RX_CUDA(h->d_range_n.ensure(cq));
-			RX_CUDA(h->d_sel_count.ensure(cq));
-			RX_CUDA(cudaMemcpyAsync(h->d_tiles.p, tiles.data(), tiles.size() * sizeof(uint2), cudaMemcpyHostToDevice, st));
-			RX_CUDA(cudaMemsetAsync(h->d_range_n.p, 0, size_t(cq) * 4, st));
-			RX_CUDA(cudaMemsetAsync(h->d_sel_count.p, 0, size_t(cq) * 4, st));
-			ivf_range_count_kernel<<<unsigned(tiles.size()), kIvfRangeThreads, 0, st>>>(
-				h->d_keys.p, h->d_qoff.p + q0, h->d_qrows.p + q0, off[q0], h->d_radius.p + q0, h->d_tiles.p, h->d_range_n.p);
-			RX_CUDA(cudaGetLastError());
-			launches += 3;  // key plan, key scan, count
-			cnt.resize(cq);
-			RX_CUDA(cudaMemcpyAsync(cnt.data(), h->d_range_n.p, size_t(cq) * 4, cudaMemcpyDeviceToHost, st));
-			RX_CUDA(cudaStreamSynchronize(st));
-			for (uint32_t qi = 0; qi < cq; ++qi) {
-				out_n[q0 + qi] = cnt[qi];
-			}
-			if (max_out == 0) {
-				continue;
-			}
-			// survivor sub-chunks of at most kIvfSlotCap matches; a query with more is a sub-chunk of its own
-			for (uint32_t s0 = 0, s1 = 0; s0 < cq; s0 = s1) {
-				uint64_t total = cnt[s0];
-				for (s1 = s0 + 1; s1 < cq && total + cnt[s1] <= kIvfSlotCap; ++s1) {
-					total += cnt[s1];
-				}
-				if (total == 0) {
-					continue;
-				}
-				if (total > uint64_t(std::numeric_limits<int>::max())) {  // the segmented sorts count items in an int
-					return fail(RXGPU_ERR_PARAMS, "rxgpu: more than 2^31 - 1 range matches for one IVF query");
-				}
-				const uint32_t ns = s1 - s0;
-				plan.assign(2 * (size_t(ns) + 1), 0);
-				int* seg = plan.data();     // survivors of query s0 + i: [seg[i], seg[i + 1])
-				int* pack = seg + ns + 1;   // its best min(matches, max_out) in the packed output: [pack[i], pack[i + 1])
-				int longest = 0;
-				for (uint32_t i = 0; i < ns; ++i) {
-					const int m = int(std::min<uint64_t>(cnt[s0 + i], max_out));
-					seg[i + 1] = seg[i] + int(cnt[s0 + i]);
-					pack[i + 1] = pack[i] + m;
-					longest = std::max(longest, m);
-				}
-				RX_CUDA(h->d_range_seg.ensure(plan.size()));
-				RX_CUDA(h->d_sel_ord.ensure(total));
-				RX_CUDA(h->d_sel_ord2.ensure(total));
-				RX_CUDA(h->d_sel_label.ensure(total));
-				RX_CUDA(h->d_sel_label2.ensure(total));
-				RX_CUDA(cudaMemcpyAsync(h->d_range_seg.p, plan.data(), plan.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-				int* dseg = h->d_range_seg.p;
-				const int* dpack = dseg + ns + 1;
-				ivf_range_emit_kernel<<<unsigned(tileAt[s1] - tileAt[s0]), kIvfRangeThreads, 0, st>>>(
-					h->d_keys.p, h->d_qoff.p + q0, h->d_qrows.p + q0, off[q0], h->d_radius.p + q0, h->d_tiles.p + tileAt[s0], s0, dseg, r.labels,
-					h->d_sel_count.p, h->d_sel_ord.p, h->d_sel_label.p);
-				RX_CUDA(cudaGetLastError());
-				if (int rc = ivfSortSurvivors(h, int(total), int(ns), dseg, dseg + 1, st)) {
-					return rc;
-				}
-				// the packed output goes to the sorts' second buffers, free again once the sorts are done
-				float* pdist = reinterpret_cast<float*>(h->d_sel_ord2.p);
-				const dim3 gg(ns, unsigned(std::min(1024, (longest + 255) / 256)));
-				ivf_range_gather_kernel<<<gg, 256, 0, st>>>(h->d_sel_ord.p, h->d_sel_label.p, dseg, dpack, pdist, h->d_sel_label2.p);
-				RX_CUDA(cudaGetLastError());
-				launches += 4;  // emit, two sorts, gather
-				dist.resize(size_t(pack[ns]));
-				lab.resize(size_t(pack[ns]));
-				RX_CUDA(cudaMemcpyAsync(dist.data(), pdist, dist.size() * 4, cudaMemcpyDeviceToHost, st));
-				RX_CUDA(cudaMemcpyAsync(lab.data(), h->d_sel_label2.p, lab.size() * 8, cudaMemcpyDeviceToHost, st));
-				RX_CUDA(cudaStreamSynchronize(st));
-				for (uint32_t i = 0; i < ns; ++i) {
-					const size_t at = size_t(q0 + s0 + i) * max_out;
-					std::copy(dist.begin() + pack[i], dist.begin() + pack[i + 1], out_dist + at);
-					std::copy(lab.begin() + pack[i], lab.begin() + pack[i + 1], out_label + at);
-				}
-			}
-		}
-		const uint64_t probed = off[nq];
-		g_stats.launches += launches;
-		g_stats.passes = 1;
-		// as rxgpu_ivf_search_knn_large_k: rows read once; each key written once and read once
-		g_stats.algorithmic_bytes += probed * ix->dim * 4 + (ix->metric == RXGPU_COS ? probed * 4 : 0) + probed * 16;
+		const IvfRangeEmit emit = [&](uint32_t q, uint64_t n, const float* dist, const uint64_t* label, uint64_t m) {
+			out_n[q] = n;
+			std::copy(dist, dist + m, out_dist + size_t(q) * max_out);
+			std::copy(label, label + m, out_label + size_t(q) * max_out);
+		};
+		return ivfRangeBatch(ix, h, nq, queries, radius, nprobe, max_out, emit);
 	} catch (const std::bad_alloc&) {
 		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
 	}
-	return 0;
 }
 
 }  // extern "C"

@@ -85,9 +85,32 @@ __device__ __forceinline__ void sel_pick(const uint32_t* hist, SelState* s, int 
 	}
 }
 
+// a survivor: its distance word, and its label -- or, with no labels (the local part of a sharded search), its row
 __device__ __forceinline__ void sel_emit(uint64_t key, const uint64_t* labels, uint32_t pos, uint32_t* out_ord, uint64_t* out_label) {
 	out_ord[pos] = uint32_t(key >> 32);
-	out_label[pos] = labels[uint32_t(key)];
+	out_label[pos] = labels ? labels[uint32_t(key)] : uint64_t(uint32_t(key));
+}
+
+// the survivors of the query chunk [q0, q0 + cq) -- ordered by (distance word, row) -- into a sharded KNN's payload at row q0:
+// one thread per slot, rows of `stride` entries
+__global__ void ivf_shard_emit_kernel(const uint32_t* ord, const uint64_t* row, const uint32_t* count, uint32_t k, uint32_t cq,
+									  const uint64_t* labels, uint32_t stride, float* out_dist, uint32_t* out_idx, uint64_t* out_label,
+									  uint32_t* out_count) {
+	const uint64_t i = blockIdx.x * uint64_t(blockDim.x) + threadIdx.x;
+	const uint32_t qi = uint32_t(i / k), j = uint32_t(i % k);
+	if (qi >= cq) {
+		return;
+	}
+	if (j == 0) {
+		out_count[qi] = count[qi];
+	}
+	if (j < count[qi]) {
+		const size_t at = size_t(qi) * stride + j;
+		const uint32_t r = uint32_t(row[i]);
+		out_dist[at] = key_dist(ord[i], false);  // as the fused path decodes it: a zero distance is +0
+		out_idx[at] = r;
+		out_label[at] = labels[r];
+	}
 }
 
 // one warp per query: rows[q] = sum of the sizes of its probed lists (work items probe-major, work[p * nq + q])

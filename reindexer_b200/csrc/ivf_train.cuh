@@ -7,6 +7,7 @@
 //   kmeans_split_kernel      -- split_clusters (:247-294) given the host's choices: copy, then the symmetric perturbation x (1 +- 2^-10)
 //                               taken in double and rounded once, as FAISS's `float *= double` does; pairs applied in order
 //   kmeans_renorm_kernel     -- fvec_renorm_L2 for spherical k-means: fp64 norm, each coordinate divided by it and rounded once
+//   kmeans_gather_rows_kernel -- the sharded training's row moves: the all-gathered sample into plan order, initial centroids from it
 #pragma once
 #include "common.cuh"
 
@@ -86,6 +87,15 @@ __global__ void kmeans_renorm_kernel(float* centroids, uint32_t pitch, uint32_t 
 		for (uint32_t j = lane; j < dim; j += 32) {
 			row[j] = __double2float_rn(__ddiv_rn(double(row[j]), nr));
 		}
+	}
+}
+
+// one CTA per output row: dst[i] (pitch dstPitch) = src[from[i]] (pitch dim), coordinates copied as they are
+__global__ void kmeans_gather_rows_kernel(const float* src, uint32_t dim, const uint64_t* from, float* dst, uint32_t dstPitch) {
+	const float* s = src + from[blockIdx.x] * dim;
+	float* d = dst + size_t(blockIdx.x) * dstPitch;
+	for (uint32_t j = threadIdx.x; j < dim; j += blockDim.x) {
+		d[j] = s[j];
 	}
 }
 

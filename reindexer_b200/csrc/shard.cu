@@ -5,6 +5,8 @@
 // below the k-th distance is in them, so no shard is scanned a second time) with a second, tiny all-gather.
 // Range batches: each shard answers its part with rxgpu_search_range_batch's core, two all-reduces agree on the totals and on a payload
 // width, one all-gather ships every shard's best min(matches, max_out) per query, and a warp per query merges them under hitLessByLabel.
+// IVF (rxgpu_sharded_ivf_search_knn / _range_batch): each shard's part of the IVF search (ivf.cu), then the same merge and range exchange,
+// with the words every rank must agree on (centroid fingerprint, nlist, nprobe, ...) and its status carried through the first exchange.
 // The exchanges go through commAllGather / commAllReduce: NCCL between processes, a host rendezvous between the threads of one process.
 // NCCL is resolved with dlopen at the first rxgpu_comm_* call: librxgpu.so itself keeps loading on a box without NCCL or a GPU.
 #include <cuda_runtime.h>
@@ -67,10 +69,11 @@ const NcclApi& nccl() {
 	} while (0)
 
 // Layout of one rank's contribution to the exchange (all sections 16-byte aligned):
-//   [dist f32 nq*k1][idx u32 nq*k1][label u64 nq*k1][count u32 nq][size u64, pad]
+//   [dist f32 nq*k1][idx u32 nq*k1][label u64 nq*k1][count u32 nq][size u64, pad] -- the IVF search's header (IvfHeader) in place of
+// [size u64, pad]
 struct PayloadLayout {
 	size_t off_dist, off_idx, off_label, off_count, off_size, bytes;
-	PayloadLayout(uint32_t nq, uint32_t k1) {
+	PayloadLayout(uint32_t nq, uint32_t k1, size_t header = 16) {
 		auto up = [](size_t x) { return (x + 15) & ~size_t(15); };
 		const size_t n = size_t(nq) * k1;
 		off_dist = 0;
@@ -78,7 +81,7 @@ struct PayloadLayout {
 		off_label = up(off_idx + n * 4);
 		off_count = up(off_label + n * 8);
 		off_size = up(off_count + size_t(nq) * 4);
-		bytes = up(off_size + 16);
+		bytes = up(off_size + header);
 	}
 };
 
@@ -159,6 +162,25 @@ struct RangeLayout {
 		off_kept = up(off_label + n * 8);
 		bytes = up(off_kept + size_t(nq) * 4);
 	}
+};
+
+// The header of a sharded IVF KNN payload: the shard's size first, as the merge reads it, then what every rank must agree on, and the
+// status of its local part
+struct IvfHeader {
+	uint64_t size, fingerprint;
+	uint32_t nlist, nprobe, k, dim, metric;
+	int32_t status;
+};
+
+// One rank's part of a sharded range batch: per query its matches in total and the best min(total, max_out) of them, best first under
+// hitLessByLabel, at dist / label [first, first + kept)
+struct RangeLocal {
+	std::vector<uint64_t> n;
+	std::vector<uint32_t> kept;
+	std::vector<size_t> first;
+	std::vector<float> dist;
+	std::vector<uint64_t> label;
+	explicit RangeLocal(uint32_t nq) : n(nq, 0), kept(nq, 0), first(nq, 0) {}
 };
 
 // One warp per query: lane s walks shard s's matches, already best first under hitLessByLabel.  Each round writes the warp-wide minimum
@@ -260,7 +282,8 @@ struct rxgpu_comm {
 	PinBuf<uint8_t> h_m_tie;
 	PinBuf<unsigned char> h_tie_recv;
 	PinBuf<uint64_t> h_size;
-	DevBuf<uint64_t> d_r_n;  // range batch: the per-query totals, then the agreed width (as u32)
+	DevBuf<uint64_t> d_r_n;  // range batch: the per-query totals
+	DevBuf<uint32_t> d_r_words;  // range batch: the agreed width (and the IVF search's status and words every rank must hold)
 	PinBuf<uint64_t> h_r_n;
 	PinBuf<unsigned char> h_r_send;  // this rank's range payload, staged for the copy to the device
 	~rxgpu_comm() {
@@ -346,6 +369,142 @@ int commAllGather(rxgpu_comm* c, const void* d_send, void* d_recv, size_t bytes,
 	return 0;
 }
 }  // namespace rxgpu
+
+namespace {
+// The device merge of the R payloads gathered in c->d_recv (layout `lay`, k1 >= k entries per query): the k best under (distance, global
+// row), then on the host the runs of bit-equal distances ordered by label, into out_* (host, nq x k); the merged rows stay in c->h_m_*.
+// With tieQ, the queries whose k-th and (k+1)-th distances are bit-equal go to tieQ, with that distance to tieD.
+int mergePayloads(rxgpu_comm* c, uint32_t nq, uint32_t k, uint32_t k1, const PayloadLayout& lay, cudaStream_t st, float* out_dist,
+				  uint64_t* out_label, uint32_t* out_count, std::vector<uint32_t>* tieQ, std::vector<float>* tieD) {
+	const size_t on = size_t(nq) * k;
+	RX_CUDA(c->d_m_dist.ensure(on));
+	RX_CUDA(c->d_m_gidx.ensure(on));
+	RX_CUDA(c->d_m_label.ensure(on));
+	RX_CUDA(c->d_m_count.ensure(nq));
+	RX_CUDA(c->d_m_tie.ensure(nq));
+	RX_CUDA(c->h_m_dist.ensure(on));
+	RX_CUDA(c->h_m_gidx.ensure(on));
+	RX_CUDA(c->h_m_label.ensure(on));
+	RX_CUDA(c->h_m_count.ensure(nq));
+	RX_CUDA(c->h_m_tie.ensure(nq));
+	const unsigned blocks = unsigned((uint64_t(nq) * 32 + 255) / 256);
+	shard_merge_kernel<<<blocks, 256, 0, st>>>(c->d_recv.p, uint32_t(c->nranks), nq, k, k1, lay, c->d_m_dist.p, c->d_m_gidx.p, c->d_m_label.p,
+											   c->d_m_count.p, c->d_m_tie.p);
+	RX_CUDA(cudaGetLastError());
+	RX_CUDA(cudaMemcpyAsync(c->h_m_dist.p, c->d_m_dist.p, on * 4, cudaMemcpyDeviceToHost, st));
+	RX_CUDA(cudaMemcpyAsync(c->h_m_gidx.p, c->d_m_gidx.p, on * 8, cudaMemcpyDeviceToHost, st));
+	RX_CUDA(cudaMemcpyAsync(c->h_m_label.p, c->d_m_label.p, on * 8, cudaMemcpyDeviceToHost, st));
+	RX_CUDA(cudaMemcpyAsync(c->h_m_count.p, c->d_m_count.p, size_t(nq) * 4, cudaMemcpyDeviceToHost, st));
+	RX_CUDA(cudaMemcpyAsync(c->h_m_tie.p, c->d_m_tie.p, nq, cudaMemcpyDeviceToHost, st));
+	RX_CUDA(cudaStreamSynchronize(st));
+	collectProfile();
+	// runs of bit-equal distances ordered by label (the drain order of the reference's heap, and the order of rxgpu_ivf_search_knn)
+	std::vector<Hit> top;
+	for (uint32_t q = 0; q < nq; ++q) {
+		const uint32_t n = c->h_m_count.p[q];
+		top.resize(n);
+		bool anyEqual = false;
+		for (uint32_t j = 0; j < n; ++j) {
+			top[j] = Hit{c->h_m_dist.p[size_t(q) * k + j], c->h_m_gidx.p[size_t(q) * k + j], c->h_m_label.p[size_t(q) * k + j]};
+			anyEqual |= j && !(top[j - 1].dist < top[j].dist);
+		}
+		if (anyEqual) {
+			orderTiesByLabel(top);
+		}
+		for (uint32_t j = 0; j < n; ++j) {
+			out_dist[size_t(q) * k + j] = top[j].dist;
+			out_label[size_t(q) * k + j] = top[j].label;
+		}
+		out_count[q] = n;
+		if (tieQ && c->h_m_tie.p[q] && n == k) {
+			tieQ->push_back(q);
+			tieD->push_back(c->h_m_dist.p[size_t(q) * k + k - 1]);
+		}
+	}
+	return 0;
+}
+
+// The exchange of the sharded range batches after each rank's local part `loc`: one MaxU32 all-reduce of the width every rank sends --
+// and, when `agree` is given, of this rank's status and of every word of `agree` beside its complement, so that the ranks learn at once
+// whether any failed (that code, on every rank) or differ in a word (errLogic) -- then the SumU64 all-reduce of the totals, one
+// all-gather of min(matches, max_out) per query and shard, and range_merge_kernel.  The totals go to out_n, the merged rows to
+// out_dist / out_label (host, nq x max_out).
+int rangeExchange(rxgpu_comm* c, uint32_t nq, uint64_t max_out, const RangeLocal& loc, int status, const std::string& why,
+				  const std::vector<uint32_t>* agree, cudaStream_t st, float* out_dist, uint64_t* out_label, uint64_t* out_n) {
+	const uint32_t R = uint32_t(c->nranks);
+	uint32_t W = *std::max_element(loc.kept.begin(), loc.kept.end());
+	if (max_out || agree) {
+		std::vector<uint32_t> words{W, uint32_t(status)};
+		if (agree) {
+			for (const uint32_t a : *agree) {
+				words.push_back(a);
+				words.push_back(~a);
+			}
+		}
+		RX_CUDA(c->d_r_words.ensure(words.size()));
+		RX_CUDA(cudaMemcpyAsync(c->d_r_words.p, words.data(), words.size() * 4, cudaMemcpyHostToDevice, st));
+		if (int rc = commAllReduce(c, c->d_r_words.p, words.size(), CommOp::MaxU32, st)) {
+			return rc;
+		}
+		RX_CUDA(cudaMemcpyAsync(words.data(), c->d_r_words.p, words.size() * 4, cudaMemcpyDeviceToHost, st));
+		RX_CUDA(cudaStreamSynchronize(st));
+		if (words[1]) {
+			return fail(int(words[1]), uint32_t(status) == words[1] ? why : "rxgpu: the sharded search failed on another rank");
+		}
+		for (size_t i = 2; i < words.size(); i += 2) {
+			if (words[i] != ~words[i + 1]) {  // max(a) == ~max(~a) = min(a) only when every rank holds the same word
+				return fail(RXGPU_ERR_LOGIC, "rxgpu: the shards of a sharded IVF search differ in their centroids, nlist, nprobe, dim or metric");
+			}
+		}
+		W = words[0];
+	}
+	RX_CUDA(c->h_r_n.ensure(nq));
+	RX_CUDA(c->d_r_n.ensure(nq));
+	RX_CUDA(cudaMemcpyAsync(c->d_r_n.p, loc.n.data(), size_t(nq) * 8, cudaMemcpyHostToDevice, st));
+	if (int rc = commAllReduce(c, c->d_r_n.p, nq, CommOp::SumU64, st)) {
+		return rc;
+	}
+	RX_CUDA(cudaMemcpyAsync(c->h_r_n.p, c->d_r_n.p, size_t(nq) * 8, cudaMemcpyDeviceToHost, st));
+	RX_CUDA(cudaStreamSynchronize(st));
+	std::memcpy(out_n, c->h_r_n.p, size_t(nq) * 8);
+	if (max_out == 0 || W == 0) {  // nothing to return, or no match on any shard
+		return 0;
+	}
+	// one all-gather of the padded payloads, the device merge, and only the merged rows cross to the host
+	const RangeLayout lay(nq, W);
+	RX_CUDA(c->h_r_send.ensure(lay.bytes));
+	float* h_dist = reinterpret_cast<float*>(c->h_r_send.p + lay.off_dist);
+	uint64_t* h_label = reinterpret_cast<uint64_t*>(c->h_r_send.p + lay.off_label);
+	for (uint32_t q = 0; q < nq; ++q) {
+		std::memcpy(h_dist + size_t(q) * W, loc.dist.data() + loc.first[q], size_t(loc.kept[q]) * 4);
+		std::memcpy(h_label + size_t(q) * W, loc.label.data() + loc.first[q], size_t(loc.kept[q]) * 8);
+	}
+	std::memcpy(c->h_r_send.p + lay.off_kept, loc.kept.data(), size_t(nq) * 4);
+	RX_CUDA(c->d_send.ensure(lay.bytes));
+	RX_CUDA(c->d_recv.ensure(lay.bytes * R));
+	unsigned char* snd = R > 1 ? c->d_send.p : c->d_recv.p;  // a single shard merges its own payload in place
+	RX_CUDA(cudaMemcpyAsync(snd, c->h_r_send.p, lay.bytes, cudaMemcpyHostToDevice, st));
+	if (R > 1) {
+		if (int rc = commAllGather(c, c->d_send.p, c->d_recv.p, lay.bytes, st)) {
+			return rc;
+		}
+	}
+	const uint32_t width = uint32_t(std::min<uint64_t>(max_out, uint64_t(R) * W));
+	const size_t on = size_t(nq) * width;
+	RX_CUDA(c->d_m_dist.ensure(on));
+	RX_CUDA(c->d_m_label.ensure(on));
+	const unsigned blocks = unsigned((uint64_t(nq) * 32 + 255) / 256);
+	range_merge_kernel<<<blocks, 256, 0, st>>>(c->d_recv.p, R, nq, W, lay, width, c->d_m_dist.p, c->d_m_label.p);
+	RX_CUDA(cudaGetLastError());
+	g_stats.launches += 1;
+	RX_CUDA(cudaMemcpy2DAsync(out_dist, size_t(max_out) * 4, c->d_m_dist.p, size_t(width) * 4, size_t(width) * 4, nq,
+							  cudaMemcpyDeviceToHost, st));
+	RX_CUDA(cudaMemcpy2DAsync(out_label, size_t(max_out) * 8, c->d_m_label.p, size_t(width) * 8, size_t(width) * 8, nq,
+							  cudaMemcpyDeviceToHost, st));
+	RX_CUDA(cudaStreamSynchronize(st));
+	return 0;
+}
+}  // namespace
 
 extern "C" {
 
@@ -504,58 +663,16 @@ int rxgpu_sharded_search_knn(rxgpu_comm* c, const rxgpu_index* ix, uint32_t nq, 
 			return rc;
 		}
 		const rxgpu_search_stats scanStats = g_stats;  // what the roofline figure describes: the shard scan, not the rare tie pass
-		// ---- 2. one all-gather, 3. device merge
+		// ---- 2. one all-gather, 3. device merge, 4. bit-equal distances ordered by label
 		if (R > 1) {
 			if (int rc = commAllGather(c, c->d_send.p, c->d_recv.p, lay.bytes, st)) {
 				return rc;
 			}
 		}
-		const size_t on = size_t(nq) * k;
-		RX_CUDA(c->d_m_dist.ensure(on));
-		RX_CUDA(c->d_m_gidx.ensure(on));
-		RX_CUDA(c->d_m_label.ensure(on));
-		RX_CUDA(c->d_m_count.ensure(nq));
-		RX_CUDA(c->d_m_tie.ensure(nq));
-		RX_CUDA(c->h_m_dist.ensure(on));
-		RX_CUDA(c->h_m_gidx.ensure(on));
-		RX_CUDA(c->h_m_label.ensure(on));
-		RX_CUDA(c->h_m_count.ensure(nq));
-		RX_CUDA(c->h_m_tie.ensure(nq));
-		if (int rc = rxgpu_merge_shards_device(R, nq, k, k1, c->d_recv.p, c->d_m_dist.p, c->d_m_gidx.p, c->d_m_label.p, c->d_m_count.p,
-											   c->d_m_tie.p, st)) {
-			return rc;
-		}
-		RX_CUDA(cudaMemcpyAsync(c->h_m_dist.p, c->d_m_dist.p, on * 4, cudaMemcpyDeviceToHost, st));
-		RX_CUDA(cudaMemcpyAsync(c->h_m_gidx.p, c->d_m_gidx.p, on * 8, cudaMemcpyDeviceToHost, st));
-		RX_CUDA(cudaMemcpyAsync(c->h_m_label.p, c->d_m_label.p, on * 8, cudaMemcpyDeviceToHost, st));
-		RX_CUDA(cudaMemcpyAsync(c->h_m_count.p, c->d_m_count.p, size_t(nq) * 4, cudaMemcpyDeviceToHost, st));
-		RX_CUDA(cudaMemcpyAsync(c->h_m_tie.p, c->d_m_tie.p, nq, cudaMemcpyDeviceToHost, st));
-		RX_CUDA(cudaStreamSynchronize(st));
-		collectProfile();
-		// ---- 4. host: runs of bit-equal distances ordered by label (the drain order of the reference's heap), output
 		std::vector<uint32_t> tieQ;
 		std::vector<float> tieD;
-		std::vector<Hit> top;
-		for (uint32_t q = 0; q < nq; ++q) {
-			const uint32_t n = c->h_m_count.p[q];
-			top.resize(n);
-			bool anyEqual = false;
-			for (uint32_t j = 0; j < n; ++j) {
-				top[j] = Hit{c->h_m_dist.p[size_t(q) * k + j], c->h_m_gidx.p[size_t(q) * k + j], c->h_m_label.p[size_t(q) * k + j]};
-				anyEqual |= j && !(top[j - 1].dist < top[j].dist);
-			}
-			if (anyEqual) {
-				orderTiesByLabel(top);
-			}
-			for (uint32_t j = 0; j < n; ++j) {
-				out_dist[size_t(q) * k + j] = top[j].dist;
-				out_label[size_t(q) * k + j] = top[j].label;
-			}
-			out_count[q] = n;
-			if (c->h_m_tie.p[q] && n == k) {
-				tieQ.push_back(q);
-				tieD.push_back(c->h_m_dist.p[size_t(q) * k + k - 1]);
-			}
+		if (int rc = mergePayloads(c, nq, k, k1, lay, st, out_dist, out_label, out_count, &tieQ, &tieD)) {
+			return rc;
 		}
 		// ---- 5. rare: a tie straddles the global k-th place of some queries (the same set on every rank) -> replay the reference's rule
 		if (!tieQ.empty()) {
@@ -647,16 +764,9 @@ int rxgpu_sharded_search_range_batch(rxgpu_comm* c, const rxgpu_index* ix, uint3
 	std::lock_guard<std::mutex> lck(c->mtx);
 	try {
 		cudaStream_t st = c->stream;
-		const uint32_t R = uint32_t(c->nranks);
 		// ---- 1. this shard's matches; the best min(n, max_out) of every query are kept, best first (a global top-max_out never needs more)
-		RX_CUDA(c->h_r_n.ensure(nq));
-		std::vector<uint32_t> kept(nq, 0);
-		std::vector<size_t> first(nq, 0);
-		std::vector<float> kd;
-		std::vector<uint64_t> kl;
-		if (ix->size == 0) {
-			std::memset(c->h_r_n.p, 0, size_t(nq) * 8);
-		} else {
+		RangeLocal loc(nq);
+		if (ix->size != 0) {
 			const float* d_q = queries;
 			if (!queries_on_device) {
 				RX_CUDA(c->d_queries.ensure(size_t(nq) * ix->dim));
@@ -666,78 +776,136 @@ int rxgpu_sharded_search_range_batch(rxgpu_comm* c, const rxgpu_index* ix, uint3
 			WsLease lease(ix);
 			lease.st = st;
 			const RangeEmit emit = [&](uint32_t q, const std::vector<Hit>& hits) {
-				c->h_r_n.p[q] = hits.size();
-				kept[q] = uint32_t(std::min<uint64_t>(hits.size(), max_out));
-				first[q] = kd.size();
-				for (uint32_t i = 0; i < kept[q]; ++i) {
-					kd.push_back(hits[i].dist);
-					kl.push_back(hits[i].label);
+				loc.n[q] = hits.size();
+				loc.kept[q] = uint32_t(std::min<uint64_t>(hits.size(), max_out));
+				loc.first[q] = loc.dist.size();
+				for (uint32_t i = 0; i < loc.kept[q]; ++i) {
+					loc.dist.push_back(hits[i].dist);
+					loc.label.push_back(hits[i].label);
 				}
 			};
 			if (int rc = rangeBatch(ix, *lease.ws, st, d_q, nq, radius, max_out, emit)) {
 				return rc;
 			}
 		}
-		// ---- 2. the totals over all shards, and the width every rank sends
-		RX_CUDA(c->d_r_n.ensure(size_t(nq) + 1));
-		RX_CUDA(cudaMemcpyAsync(c->d_r_n.p, c->h_r_n.p, size_t(nq) * 8, cudaMemcpyHostToDevice, st));
-		if (int rc = commAllReduce(c, c->d_r_n.p, nq, CommOp::SumU64, st)) {
-			return rc;
-		}
-		RX_CUDA(cudaMemcpyAsync(c->h_r_n.p, c->d_r_n.p, size_t(nq) * 8, cudaMemcpyDeviceToHost, st));
-		RX_CUDA(cudaStreamSynchronize(st));
-		std::memcpy(out_n, c->h_r_n.p, size_t(nq) * 8);
-		if (max_out == 0) {
-			return 0;
-		}
-		uint32_t* d_w = reinterpret_cast<uint32_t*>(c->d_r_n.p + nq);
-		c->h_r_n.p[0] = *std::max_element(kept.begin(), kept.end());
-		RX_CUDA(cudaMemcpyAsync(d_w, c->h_r_n.p, 4, cudaMemcpyHostToDevice, st));
-		if (int rc = commAllReduce(c, d_w, 1, CommOp::MaxU32, st)) {
-			return rc;
-		}
-		RX_CUDA(cudaMemcpyAsync(c->h_r_n.p, d_w, 4, cudaMemcpyDeviceToHost, st));
-		RX_CUDA(cudaStreamSynchronize(st));
-		const uint32_t W = *reinterpret_cast<const uint32_t*>(c->h_r_n.p);
-		if (W == 0) {  // no match on any shard
-			return 0;
-		}
-		// ---- 3. one all-gather of the padded payloads, 4. device merge, and only the merged rows cross to the host
-		const RangeLayout lay(nq, W);
-		RX_CUDA(c->h_r_send.ensure(lay.bytes));
-		float* h_dist = reinterpret_cast<float*>(c->h_r_send.p + lay.off_dist);
-		uint64_t* h_label = reinterpret_cast<uint64_t*>(c->h_r_send.p + lay.off_label);
-		for (uint32_t q = 0; q < nq; ++q) {
-			std::memcpy(h_dist + size_t(q) * W, kd.data() + first[q], size_t(kept[q]) * 4);
-			std::memcpy(h_label + size_t(q) * W, kl.data() + first[q], size_t(kept[q]) * 8);
-		}
-		std::memcpy(c->h_r_send.p + lay.off_kept, kept.data(), size_t(nq) * 4);
+		// ---- 2. the width every rank sends and the totals over all shards, 3. one all-gather, 4. device merge
+		return rangeExchange(c, nq, max_out, loc, 0, std::string(), nullptr, st, out_dist, out_label, out_n);
+	} catch (const std::bad_alloc&) {
+		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
+	}
+}
+
+int rxgpu_sharded_ivf_search_knn(rxgpu_comm* c, const rxgpu_index* ix, uint32_t nq, const float* queries, int queries_on_device, uint32_t k,
+								 uint32_t nprobe, float* out_dist, uint64_t* out_label, uint32_t* out_count) {
+	(void)queries_on_device;  // the coarse pass stages host and device queries alike
+	if (!c) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: null communicator");
+	}
+	if (int rc = checkIndex(ix)) {
+		return rc;
+	}
+	if (ix->device != c->device) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: the shard lives on another device than its communicator");
+	}
+	if (nq && (!queries || !out_count || !out_dist || !out_label)) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: null argument");
+	}
+	g_stats = rxgpu_search_stats{};
+	if (nq == 0) {
+		return 0;
+	}
+	if (k == 0 || k > 65535u) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: IVF search needs k in [1, 65535]");
+	}
+	std::lock_guard<std::mutex> lck(c->mtx);
+	try {
+		cudaStream_t st = c->stream;
+		const PayloadLayout lay(nq, k, sizeof(IvfHeader));
+		const uint32_t R = uint32_t(c->nranks);
 		RX_CUDA(c->d_send.ensure(lay.bytes));
 		RX_CUDA(c->d_recv.ensure(lay.bytes * R));
 		unsigned char* snd = R > 1 ? c->d_send.p : c->d_recv.p;  // a single shard merges its own payload in place
-		RX_CUDA(cudaMemcpyAsync(snd, c->h_r_send.p, lay.bytes, cudaMemcpyHostToDevice, st));
+		// ---- 1. this shard's best k under (distance, local row), straight into the send buffer (on the index's stream, done on return)
+		IvfShardView v{};
+		const int status = ivfShardKnn(ix, nq, queries, k, nprobe, k, reinterpret_cast<float*>(snd + lay.off_dist),
+									   reinterpret_cast<uint32_t*>(snd + lay.off_idx), reinterpret_cast<uint64_t*>(snd + lay.off_label),
+									   reinterpret_cast<uint32_t*>(snd + lay.off_count), v);
+		const std::string why = status ? g_err : std::string();
+		const IvfHeader mine{v.rows, v.fingerprint, v.nlist, v.nprobe, k, ix->dim, uint32_t(ix->metric), status};
+		RX_CUDA(cudaMemcpyAsync(snd + lay.off_size, &mine, sizeof(mine), cudaMemcpyHostToDevice, st));
+		// ---- 2. one all-gather; every rank reads every header, so all return the same error or none
 		if (R > 1) {
 			if (int rc = commAllGather(c, c->d_send.p, c->d_recv.p, lay.bytes, st)) {
 				return rc;
 			}
 		}
-		const uint32_t width = uint32_t(std::min<uint64_t>(max_out, uint64_t(R) * W));
-		const size_t on = size_t(nq) * width;
-		RX_CUDA(c->d_m_dist.ensure(on));
-		RX_CUDA(c->d_m_label.ensure(on));
-		const unsigned blocks = unsigned((uint64_t(nq) * 32 + 255) / 256);
-		range_merge_kernel<<<blocks, 256, 0, st>>>(c->d_recv.p, R, nq, W, lay, width, c->d_m_dist.p, c->d_m_label.p);
-		RX_CUDA(cudaGetLastError());
-		g_stats.launches += 1;
-		RX_CUDA(cudaMemcpy2DAsync(out_dist, size_t(max_out) * 4, c->d_m_dist.p, size_t(width) * 4, size_t(width) * 4, nq,
-								  cudaMemcpyDeviceToHost, st));
-		RX_CUDA(cudaMemcpy2DAsync(out_label, size_t(max_out) * 8, c->d_m_label.p, size_t(width) * 8, size_t(width) * 8, nq,
+		std::vector<IvfHeader> hdr(R);
+		RX_CUDA(cudaMemcpy2DAsync(hdr.data(), sizeof(IvfHeader), c->d_recv.p + lay.off_size, lay.bytes, sizeof(IvfHeader), R,
 								  cudaMemcpyDeviceToHost, st));
 		RX_CUDA(cudaStreamSynchronize(st));
+		for (uint32_t r = 0; r < R; ++r) {
+			if (hdr[r].status) {
+				return fail(hdr[r].status, r == uint32_t(c->rank) ? why : "rxgpu: the sharded IVF search failed on rank " + std::to_string(r));
+			}
+		}
+		for (uint32_t r = 1; r < R; ++r) {
+			const IvfHeader& a = hdr[0];
+			const IvfHeader& b = hdr[r];
+			if (a.fingerprint != b.fingerprint || a.nlist != b.nlist || a.nprobe != b.nprobe || a.k != b.k || a.dim != b.dim || a.metric != b.metric) {
+				return fail(RXGPU_ERR_LOGIC, "rxgpu: the shards of a sharded IVF search differ in their centroids, nlist, nprobe, k, dim or metric");
+			}
+		}
+		// ---- 3. device merge under (distance, global row), 4. the k survivors by (distance, label)
+		if (int rc = mergePayloads(c, nq, k, k, lay, st, out_dist, out_label, out_count, nullptr, nullptr)) {
+			return rc;
+		}
+		g_stats.launches += 1;
 	} catch (const std::bad_alloc&) {
 		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
 	}
 	return 0;
+}
+
+int rxgpu_sharded_ivf_search_range_batch(rxgpu_comm* c, const rxgpu_index* ix, uint32_t nq, const float* queries, int queries_on_device,
+										 const float* radius, uint32_t nprobe, uint64_t max_out, float* out_dist, uint64_t* out_label,
+										 uint64_t* out_n) {
+	(void)queries_on_device;  // the coarse pass stages host and device queries alike
+	if (!c) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: null communicator");
+	}
+	if (int rc = checkIndex(ix)) {
+		return rc;
+	}
+	if (ix->device != c->device) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: the shard lives on another device than its communicator");
+	}
+	if (nq && (!queries || !radius || !out_n || (max_out && (!out_dist || !out_label)))) {
+		return fail(RXGPU_ERR_PARAMS, "rxgpu: null argument");
+	}
+	g_stats = rxgpu_search_stats{};
+	if (nq == 0) {
+		return 0;
+	}
+	std::lock_guard<std::mutex> lck(c->mtx);
+	try {
+		// ---- 1. this shard's matches (the core of rxgpu_ivf_search_range_batch), the best min(n, max_out) of every query kept
+		RangeLocal loc(nq);
+		IvfShardView v{};
+		const IvfRangeEmit emit = [&](uint32_t q, uint64_t n, const float* dist, const uint64_t* label, uint64_t m) {
+			loc.n[q] = n;
+			loc.kept[q] = uint32_t(m);
+			loc.first[q] = loc.dist.size();
+			loc.dist.insert(loc.dist.end(), dist, dist + m);
+			loc.label.insert(loc.label.end(), label, label + m);
+		};
+		const int status = ivfShardRange(ix, nq, queries, radius, nprobe, max_out, emit, v);
+		const std::string why = status ? g_err : std::string();
+		const std::vector<uint32_t> agree{uint32_t(v.fingerprint), uint32_t(v.fingerprint >> 32), v.nlist, v.nprobe, ix->dim, uint32_t(ix->metric)};
+		// ---- 2. the status, the agreed words and the width; the totals, 3. one all-gather, 4. device merge
+		return rangeExchange(c, nq, max_out, loc, status, why, &agree, c->stream, out_dist, out_label, out_n);
+	} catch (const std::bad_alloc&) {
+		return fail(RXGPU_ERR_SYSTEM, "rxgpu: out of host memory");
+	}
 }
 
 }  // extern "C"
