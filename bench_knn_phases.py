@@ -6,9 +6,10 @@
 Runs bench.py's device-resident step (search_knn_device, queries and results in HBM) and prints one JSON line with
   * step_ms       the step time from CUDA events around --steps steps, with the profiler off;
   * kernels       device time per step of every kernel, memset and copy of the step, from one torch.profiler run of its own
-                  (CUDA activities, --steps steps), grouped by kernel name (tc_prepare_queries, tc_init_tau, knn_tc_filter,
-                  knn_rerank, knn_merge_lists, ...), with the launches per step;
-  * candidates    candidates per query from the search statistics (what knn_rerank gathers), and the exact-scan fallbacks;
+                  (CUDA activities, --steps steps), grouped by kernel name (tc_prepare_queries, tc_seed_slices, tc_seed_merge,
+                  knn_tc_filter, knn_rerank, knn_merge_lists, ...), with the launches per step;
+  * candidates    candidates per query in the lists from the search statistics, and the exact-scan fallbacks;
+  * gathered      rows per query knn_rerank gathered (the candidates under the query's final threshold), from the stamped run;
   * bookkeepers   the counters of one run of the stamped diagnostic instantiation (knn_tc.cuh: kTcDiagStamps, selected with
                   rxgpu_tc_diag): hits, rows rescored by the bookkeepers, bound-list inserts, the bookkeepers' cycles spent rescoring
                   against the consumer warpgroups' cycles, and the enqueues that found a candidate queue full.
@@ -34,8 +35,9 @@ from bench_range import card  # noqa: E402
 SLOTS, WALK, MARK_EVERY = 32, 8192, 64
 TILE, BLOCKS, HITS, QWAIT, PER_WG = 8, 9, 10, 11, 12
 RESCORED, INSERTS, RESCORE_CYC = 2 * PER_WG + 4, 2 * PER_WG + 5, 2 * PER_WG + 6  # summed over the two bookkeeper warps
+GATHERED = 41  # knn_tc.cuh: kTcDgGathered, in CTA 0's slots
 MAX_CTAS = 1024
-GROUPS = ["tc_prepare_queries", "tc_init_tau", "knn_tc_filter", "knn_rerank", "knn_merge_lists", "knn_select_topk", "knn_scan_warp"]
+GROUPS = ["tc_prepare_queries", "tc_seed_slices", "tc_seed_merge", "tc_init_tau", "knn_tc_filter", "knn_rerank", "knn_merge_lists", "knn_select_topk", "knn_scan_warp"]
 
 
 def group_of(name):
@@ -157,6 +159,7 @@ def main(argv=None):
         "step_ms": step_ms, "qps": nq / (step_ms * 1e-3),
         "device_ms_per_step_profiled": device_sum, "kernels": kernels,
         "candidates_per_query": st["tc_candidates"] / nq, "fallbacks": st["tc_fallbacks"],
+        "gathered_per_query": float(c[GATHERED]) / nq,
         "bookkeepers": book,
     }
     print(json.dumps(line, default=float))

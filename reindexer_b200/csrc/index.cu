@@ -752,7 +752,7 @@ int tcPrepare(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float
 // lower bound is at or below the query's threshold tau go to ws.d_cand_rows[q][candCap], and ws.d_cand_count[q] counts them all (also
 // past candCap: an overflowed list).  fixedTau: init_rows = UINT32_MAX keeps every row out of the bound list, so tau never moves
 // (knn_tc.cuh header comment) and k1 is not used; otherwise tau tightens to the k1-th best exact distance of the bound list that
-// tc_init_tau seeded.
+// the seed (tc_seed_slices, tc_seed_merge) filled.
 int tcLaunch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const TcBatch& b, uint32_t k1, uint32_t candCap, uint32_t nrows, bool fixedTau) {
 	const uint32_t nq = b.nq, nqb = b.nqb, cluster = b.cluster, ngroups = b.ngroups, kchunks = b.kchunks, pitchQ = ix->pitch_q;
 	const uint32_t ntiles = (nrows + kTcTileRows - 1) / kTcTileRows;
@@ -787,6 +787,7 @@ int tcLaunch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const TcBatc
 	a.qf = ws.d_qf.p;
 	a.pitch = ix->pitch;
 	a.cand_rows = ws.d_cand_rows.p;
+	a.cand_lb = fixedTau ? nullptr : ws.d_cand_lb.p;
 	a.cand_count = ws.d_cand_count.p;
 	a.cand_cap = candCap;
 	a.n = nrows;
@@ -832,7 +833,7 @@ int tcLaunch(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const TcBatc
 	return 0;
 }
 
-// The candidate filter over a whole batch and all rows.  KNN (h_tau == nullptr): tau starts from tc_init_tau and tightens to the k1-th
+// The candidate filter over a whole batch and all rows.  KNN (h_tau == nullptr): tau starts from the seed and tightens to the k1-th
 // best exact distance of the bound list.  Range search: h_tau[q] = float_ord(radius) fixes tau.
 int tcFilter(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float* d_queries, uint32_t nq, uint32_t k1, uint32_t candCap,
 			 const unsigned int* h_tau) {
@@ -845,11 +846,16 @@ int tcFilter(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, const float*
 	} else {
 		RX_CUDA(ws.d_ub_list.ensure(size_t(b.nqPad) * kTcMaxK1));
 		RX_CUDA(ws.d_ub_lock.ensure(b.nqPad));
-		RX_CUDA(raiseSmemCeilingOnce(tc_init_tau, ix->device, int(tc_init_smem_bytes())));
-		tc_init_tau<<<(nq + kTcInitQ - 1) / kTcInitQ, 256, tc_init_smem_bytes(), st>>>(
+		RX_CUDA(ws.d_cand_lb.ensure(size_t(b.nqPad) * candCap));
+		RX_CUDA(ws.d_seed_part.ensure(size_t(nq) * kTcSeedSlices * kTcMaxK1));
+		const size_t smem = tc_seed_smem_bytes(b.kchunks);
+		RX_CUDA(raiseSmemCeilingOnce(tc_seed_slices, ix->device, int(tc_seed_smem_bytes(2048 / kTcChunkK))));
+		tc_seed_slices<<<dim3((nq + kTcSeedQ - 1) / kTcSeedQ, kTcSeedSlices), 256, smem, st>>>(
 			ix->d_rows, ix->pitch, b.kchunks, ix->metric == RXGPU_COS ? ix->d_norms : nullptr, uint32_t(std::min<uint64_t>(ix->size, kTcInitRows)),
-			ws.d_qf.p, nq, k1, ix->metric, ws.d_tau.p, ws.d_ub_list.p, ws.d_ub_lock.p);
-		g_stats.launches += 1;
+			ws.d_qf.p, nq, k1, ix->metric, ws.d_seed_part.p);
+		tc_seed_merge<<<(nq + 7) / 8, 256, 0, st>>>(ws.d_seed_part.p, nq, k1, ws.d_tau.p, ws.d_ub_list.p, ws.d_ub_lock.p);
+		RX_CUDA(cudaGetLastError());
+		g_stats.launches += 2;
 	}
 	return tcLaunch(ix, ws, st, b, k1, candCap, ix->shadow_slots, h_tau != nullptr);
 }
@@ -968,17 +974,20 @@ int scanTopKTensorCore(const rxgpu_index* ix, Workspace& ws, cudaStream_t st, co
 		return rc;
 	}
 	RX_CUDA(ws.d_lists.ensure(size_t(nq) * k1));
-	// exact re-rank of the candidates with the arithmetic of knn_scan_warp, then decode + labels
+	// exact re-rank of the candidates under the final thresholds with the arithmetic of knn_scan_warp, then decode + labels
 	const size_t rsmem = size_t((ix->dim + 127) / 128) * 512 + size_t(kScanWarps) * (k1 + kCandBuf) * 8;
 	const float* norms = ix->metric == RXGPU_COS ? ix->d_norms : nullptr;
+	unsigned long long* gathered = g_tc_diag.load() ? g_tc_diag_buf + kTcDgGathered : nullptr;
 	if (ix->metric == RXGPU_L2) {
 		RX_CUDA(raiseSmemCeilingOnce(knn_rerank<true>, ix->device, kScanSmemBudget));
 		knn_rerank<true><<<nq, kScanThreads, rsmem, st>>>(ix->d_rows, ix->pitch, ix->dim, norms, d_queries, ws.d_cand_rows.p,
-														   ws.d_cand_count.p, candCap, k1, ws.d_lists.p);
+														   ws.d_cand_count.p, candCap, k1, ws.d_lists.p, nullptr, nullptr, nullptr,
+														   nullptr, nullptr, ws.d_cand_lb.p, ws.d_tau.p, gathered);
 	} else {
 		RX_CUDA(raiseSmemCeilingOnce(knn_rerank<false>, ix->device, kScanSmemBudget));
 		knn_rerank<false><<<nq, kScanThreads, rsmem, st>>>(ix->d_rows, ix->pitch, ix->dim, norms, d_queries, ws.d_cand_rows.p,
-															ws.d_cand_count.p, candCap, k1, ws.d_lists.p);
+															ws.d_cand_count.p, candCap, k1, ws.d_lists.p, nullptr, nullptr, nullptr,
+															nullptr, nullptr, ws.d_cand_lb.p, ws.d_tau.p, gathered);
 	}
 	MergeArgs m{};
 	m.lists = ws.d_lists.p;

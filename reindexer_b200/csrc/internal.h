@@ -142,7 +142,9 @@ struct Workspace {
 	DevBuf<float> d_qf;              // the fp32 queries zero padded to the codes' pitch (exact distances of the bound list)
 	DevBuf<unsigned int> d_tau, d_cand_count, d_ub_lock;
 	DevBuf<float> d_ub_list;
+	DevBuf<float> d_seed_part;  // the seed's per-slice lists [nq][kTcSeedSlices][kTcMaxK1] (tc_seed_slices -> tc_seed_merge)
 	DevBuf<uint32_t> d_cand_rows;
+	DevBuf<float> d_cand_lb;  // KNN on the filter: the lower bound of every listed row (knn_rerank gathers those under the final tau)
 	PinBuf<unsigned int> h_cand_count;
 	DevBuf<unsigned int> d_stage_status;  // KNN with staged thresholds: per-query fallback status, and the candidates re-ranked
 	PinBuf<unsigned int> h_stage_status;

@@ -2,8 +2,9 @@
 //
 // knn_scan_warp is HBM-bound only while <= ~16 queries share a pass; a batch of 1024 queries is FMA-bound there.  This kernel
 // computes APPROXIMATE scores for a block of NQ queries against every row with int8 operands on the tensor cores and keeps, per
-// query, only the rows that can still be among the k best under a CERTIFIED error bound; the survivors (~430 per query at config 1)
-// are then re-ranked with the exact fp32 routine of knn_scan_warp, so the final result is identical to the exact scan.
+// query, only the rows that can still be among the k best under a CERTIFIED error bound; the survivors under the final threshold
+// (~65 of ~420 candidates per query at config 1) are then re-ranked with the exact fp32 routine of knn_scan_warp, so the final
+// result is identical to the exact scan.
 //
 // Quantisation (tc_quantize, the same for rows and queries; fp32 vector v of dimension D):
 //   scale     s_v = max|v_i| / 127 (fp32; 0 for an all-zero row)      codes  c_v = round(v / s_v), clamped to +-127
@@ -26,14 +27,17 @@
 // that every such pair reaches the exact re-rank.  Rows and queries that small only arise from subnormal-scale data.
 //   threshold     tau_q = the largest entry of the query's BOUND LIST: k1 EXACT distances (the exact scan's own arithmetic,
 //                 row_dists_warp) of k1 distinct rows (one small list per query in HBM, updated under a per-query lock -- only
-//                 O(k log n) successful inserts per query over a whole pass); a row is a candidate iff lb <= tau_q.  tc_init_tau
-//                 seeds the list with the exact k1 best of the first kTcInitRows rows; a bookkeeper computes the exact distance d of
-//                 a candidate row beyond them whose midpoint d~ is below the threshold and inserts d when it is below it too.
+//                 O(k log n) successful inserts per query over a whole pass); a row is a candidate iff lb <= tau_q.  The seed
+//                 (tc_seed_slices, tc_seed_merge) fills the list with the exact k1 best of the first kTcInitRows rows; a
+//                 bookkeeper computes the exact distance d of a candidate row beyond them whose midpoint d~ is below the threshold
+//                 and inserts d when it is below it too.
 //                 Every list entry is the exact distance of a distinct row (every tile is visited once per query, seed rows are
 //                 never inserted again), so tau_q is at or above the final k1-th best exact distance at every moment: every row of
 //                 the true top k1 has lb <= d <= tau_q and stays a candidate, and so does every row at or below the k-th distance
 //                 (the tie replay from the lists).  Which rows get rescored only decides how fast tau_q tightens, never whether
-//                 it is valid.  tau only decreases.
+//                 it is valid.  tau only decreases.  The re-rank gathers only the candidates with lb <= the final tau_q: one with
+//                 lb > tau_q has d >= lb > tau_q >= the k1-th best exact distance, so it is neither among the k1 best nor at or
+//                 below the k-th distance (the tie replay still reads the full lists).
 //   range search  tau_q = the query's radius, seeded by the host and never tightened (init_rows = UINT32_MAX: no row reaches the
 //                 bound list, so ub_list, ub_lock and k1 are never read).  A row matches iff its exact distance d < radius, and every
 //                 such row has lb <= d < tau_q, so it is a candidate; the exact re-rank (knn_rerank's range mode) then keeps the
@@ -96,12 +100,13 @@ struct TcArgs {
 	float* ub_list;            // [nq_total][kTcMaxK1] the bound list: the k1 smallest exact distances of the rows inserted by any CTA
 							   // (guarded by ub_lock)
 	unsigned int* ub_lock;     // [nq_total]
-	uint32_t init_rows;        // ROWS [0, init_rows) are already represented in ub_list by tc_init_tau (never insert them twice)
+	uint32_t init_rows;        // ROWS [0, init_rows) are already represented in ub_list by the seed (never insert them twice)
 	const float* rows;         // fp32 rows [n][pitch] and the Cosine norm coefficients (nullptr otherwise): the bookkeepers' exact
 	const float* norm_coefs;   // distances of the rows they insert into the bound list
 	const float* qf;           // [nq_total][kchunks * 128] fp32 queries, zero padded (tc_prepare_queries)
 	uint32_t pitch;
 	uint32_t* cand_rows;       // [nq_total][cand_cap]
+	float* cand_lb;            // [nq_total][cand_cap] the lower bound d~ - err of every listed row (KNN with a bound list; else nullptr)
 	unsigned int* cand_count;  // [nq_total]
 	uint32_t cand_cap;
 	uint32_t n;                // slots: a prefix of the shadow's slots (all of them, or a stage's prefix)
@@ -155,8 +160,9 @@ enum : uint32_t {
 	kTcDgRescored = kTcDgProd + 1,  // bookkeepers (all three warps summed): rows whose exact distance they computed (count), ...
 	kTcDgInserts,                   // ... bound-list inserts attempted under the lock (count), ...
 	kTcDgRescoreCycles,             // ... and clock64 cycles spent computing those distances (stamped instantiation only)
+	kTcDgGathered,                  // CTA 0's slot only: rows knn_rerank gathered after the filter (count)
 };
-static_assert(kTcDgRescoreCycles < kTcDiagSlots, "diagnostic counters fit their slots");
+static_assert(kTcDgGathered < kTcDiagSlots, "diagnostic counters fit their slots");
 
 // shared memory: query block, the stage ring, barriers, per-query constants, then per consumer warpgroup thresholds and block thresholds
 __host__ __device__ inline size_t tc_smem_bytes(uint32_t nq_block, uint32_t kchunks, uint32_t stages = kTcStages) {
@@ -618,6 +624,9 @@ __device__ __forceinline__ void tc_bookkeeper(const TcArgs& a, TcQueue* qu, cons
 			const unsigned pos = base + __popc(peers & ((1u << lane) - 1u));
 			if (pos < a.cand_cap) {
 				a.cand_rows[size_t(q0 + ql) * a.cand_cap + pos] = row;
+				if (a.cand_lb != nullptr) {
+					a.cand_lb[size_t(q0 + ql) * a.cand_cap + pos] = d - err;
+				}
 			}
 		}
 		// the midpoint rather than the upper bound d + err: tau then follows the k1-th best exact distance instead of trailing it by
@@ -1050,13 +1059,19 @@ __global__ void __launch_bounds__(kScanThreads) knn_rerank(const float* rows, ui
 															uint32_t cand_cap, uint32_t k1, uint64_t* lists /* [gridDim.x][k1] */,
 															const uint32_t* qsel = nullptr, const float* tie_bound = nullptr,
 															const float* radius = nullptr, uint64_t* range_keys = nullptr,
-															unsigned int* range_count = nullptr) {
+															unsigned int* range_count = nullptr, const float* cand_lb = nullptr,
+															const unsigned int* tau = nullptr, unsigned long long* gathered = nullptr) {
 	// qsel: CTA b serves query qsel[b] (default: query b).  tie_bound != nullptr = tie mode (kModeTieRows): among the candidates
 	// with dist <= tie_bound[b], the first k1 in internal row order (key = row << 32 | ord(dist)) -- every row at or below the k-th
 	// distance is a candidate, so this replaces a second scan of the whole shard when the reference's tie rule must be replayed.
 	// radius != nullptr = range mode: every candidate with dist < radius[q] (strict, as the exact range scan) is appended, unordered,
 	// as make_key(dist, row) to range_keys[q][cand_cap] and counted in range_count[q]; lists and k1 are not used.  The matches are a
 	// subset of the query's candidates, so they never exceed cand_cap.
+	// cand_lb != nullptr (top-k mode after a filter with a bound list): candidate i is gathered only when cand_lb[q][i] <= the final
+	// threshold ord_float(tau[q]) (NaN: gathered).  Its exact distance is at or above its lower bound, and the final threshold is at
+	// or above the k1-th best distance, so a skipped row can be neither among the k1 best nor at the k-th distance.  Each chunk of
+	// kScanThreads candidates is compacted in shared memory first, so the warps share only the rows they gather.  gathered != nullptr:
+	// the rows gathered are added to it (diagnostics).
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const uint32_t q = qsel ? qsel[blockIdx.x] : blockIdx.x;
@@ -1084,28 +1099,55 @@ __global__ void __launch_bounds__(kScanThreads) knn_rerank(const float* rows, ui
 	const uint32_t ncand = min(cand_count[q], cand_cap);
 	const float4* rows4 = reinterpret_cast<const float4*>(rows);
 	const uint32_t* my = cand_rows + size_t(q) * cand_cap;
-	for (uint32_t i = warp; i < ncand; i += kScanWarps) {
-		const uint32_t row = my[i];
-		const float dist = row_dist_warp<kIsL2>(rows4, pitch4, nch, row, sq4, norm_coefs, lane);
-		if (range) {
-			if (lane == 0 && dist < rad) {
-				range_keys[size_t(q) * cand_cap + atomicAdd(&range_count[q], 1u)] = make_key(dist, row);
-			}
-			continue;
+	const float* my_lb = cand_lb ? cand_lb + size_t(q) * cand_cap : nullptr;
+	const float tau_q = cand_lb ? ord_float(tau[q]) : 0.f;
+	__shared__ uint32_t s_rows[kScanThreads];
+	__shared__ uint32_t s_warp_n[kScanWarps];
+	for (uint32_t c0 = 0; c0 < ncand; c0 += kScanThreads) {
+		const uint32_t i = c0 + threadIdx.x;
+		const bool keep = i < ncand && !(my_lb != nullptr && my_lb[i] > tau_q);
+		const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+		if (lane == 0) {
+			s_warp_n[warp] = __popc(ballot);
 		}
-		const uint64_t key = !tie ? make_key(dist, row) : (dist <= bound ? ((uint64_t(row) << 32) | float_ord(dist)) : kKeyNone);
-		if (key < thr) {  // warp-uniform
-			if (lane == 0) {
-				wkeys[k1 + cnt] = key;
+		__syncthreads();
+		uint32_t base = 0, nkeep = 0;
+#pragma unroll
+		for (int w = 0; w < kScanWarps; ++w) {
+			base += w < warp ? s_warp_n[w] : 0u;
+			nkeep += s_warp_n[w];
+		}
+		if (keep) {
+			s_rows[base + __popc(ballot & ((1u << lane) - 1u))] = my[i];
+		}
+		if (gathered != nullptr && threadIdx.x == 0) {
+			atomicAdd(gathered, (unsigned long long)nkeep);
+		}
+		__syncthreads();
+		for (uint32_t j = warp; j < nkeep; j += kScanWarps) {
+			const uint32_t row = s_rows[j];
+			const float dist = row_dist_warp<kIsL2>(rows4, pitch4, nch, row, sq4, norm_coefs, lane);
+			if (range) {
+				if (lane == 0 && dist < rad) {
+					range_keys[size_t(q) * cand_cap + atomicAdd(&range_count[q], 1u)] = make_key(dist, row);
+				}
+				continue;
 			}
-			++cnt;
-			__syncwarp();
-			if (cnt == kCandBuf) {
-				warp_select(wkeys, k1 + cnt, k1, lane);
-				thr = wkeys[k1 - 1];
-				cnt = 0;
+			const uint64_t key = !tie ? make_key(dist, row) : (dist <= bound ? ((uint64_t(row) << 32) | float_ord(dist)) : kKeyNone);
+			if (key < thr) {  // warp-uniform
+				if (lane == 0) {
+					wkeys[k1 + cnt] = key;
+				}
+				++cnt;
+				__syncwarp();
+				if (cnt == kCandBuf) {
+					warp_select(wkeys, k1 + cnt, k1, lane);
+					thr = wkeys[k1 - 1];
+					cnt = 0;
+				}
 			}
 		}
+		__syncthreads();  // s_rows and s_warp_n are refilled by the next chunk
 	}
 	if (range) {
 		return;
@@ -1508,100 +1550,141 @@ __global__ void tc_block_consts(const float4* rowc, const uint32_t* slot_row, ui
 	}
 }
 
-// tau_init[q] = the k1-th best EXACT distance among the first `nrows` (<= kTcInitRows) rows, and ub_list[q] their k1 best: computed
-// with row_dists_warp, the exact scan's own arithmetic, so every list entry is a row's exact-scan distance (knn_tc.cuh header).  One
-// block serves kTcInitQ queries (tc_prepare_queries' zero-padded fp32 copy) so a row comes from L2 once per kTcInitQ queries; a warp
-// keeps four rows (128-bit loads) in flight; the k1 smallest distances of a query are then picked by one warp (k1 rounds of a
-// warp-wide argmin).
-constexpr int kTcInitQ = 4;
+// The seed: ub_list[q] = the k1 best EXACT distances among the first `nrows` (<= kTcInitRows) rows, ascending, -inf beyond k1, and
+// tau[q] = the k1-th of them (+inf while fewer than k1 rows exist), computed with row_dists_warp, the exact scan's own arithmetic, so
+// every list entry is a row's exact-scan distance (knn_tc.cuh header).  Two kernels:
+//   tc_seed_slices  CTA (t, s) computes the distances of query tile t (kTcSeedQ queries of tc_prepare_queries' zero-padded fp32 copy,
+//                   staged in shared memory) to the kTcSeedSlice rows of slice s, so a row comes from L2 once per kTcSeedQ queries (a
+//                   warp keeps four rows, 128-bit loads, in flight), then keeps each query's k1 smallest of the slice, ascending
+//                   (k1 rounds of a warp-wide argmin; ties to the lower row), in part[q][s][0, k1) (+inf where the slice has fewer).
+//   tc_seed_merge   one warp per query merges the kTcSeedSlices sorted lists (ties to the lower slice, so to the lower row).
+// NaN distances are never picked (they sort as +inf).  Padding queries (q >= nq) are left untouched.
+constexpr int kTcSeedQ = 16;
 constexpr uint32_t kTcInitRows = 4096;  // DESIGN 3.2: 4096 against 1024 and 2048 at config 1 (fewer early hits and full queues)
-__host__ __device__ inline size_t tc_init_smem_bytes() { return size_t(kTcInitQ) * kTcInitRows * sizeof(float); }
-__global__ void __launch_bounds__(256) tc_init_tau(const float* rows, uint32_t pitch, uint32_t kchunks, const float* norm_coefs, uint32_t nrows,
-												   const float* qf, uint32_t nq, uint32_t k1, int metric, unsigned int* tau, float* ub_list,
-												   unsigned int* ub_lock) {
-	extern __shared__ __align__(16) float s_d[];  // [kTcInitQ][kTcInitRows]
-	const uint32_t q0 = blockIdx.x * kTcInitQ;
+constexpr uint32_t kTcSeedSlice = 512;
+constexpr uint32_t kTcSeedSlices = kTcInitRows / kTcSeedSlice;
+__host__ __device__ inline size_t tc_seed_smem_bytes(uint32_t kchunks) {
+	return size_t(kTcSeedQ) * (size_t(kchunks) * 128 + kTcSeedSlice) * sizeof(float);
+}
+__global__ void __launch_bounds__(256) tc_seed_slices(const float* rows, uint32_t pitch, uint32_t kchunks, const float* norm_coefs,
+													  uint32_t nrows, const float* qf, uint32_t nq, uint32_t k1, int metric,
+													  float* part /* [nq][kTcSeedSlices][kTcMaxK1] */) {
+	extern __shared__ __align__(16) float s_seed[];  // queries [kTcSeedQ][kchunks * 128], then distances [kTcSeedQ][kTcSeedSlice]
+	const uint32_t q0 = blockIdx.x * kTcSeedQ, slice = blockIdx.y, row0 = slice * kTcSeedSlice;
 	const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-	const float4* rows4 = reinterpret_cast<const float4*>(rows);
-	const float4* q4[kTcInitQ];
-#pragma unroll
-	for (int qi = 0; qi < kTcInitQ; ++qi) {  // padding queries of the last block read query q0 (their distances are never picked)
-		q4[qi] = reinterpret_cast<const float4*>(qf) + size_t(q0 + qi < nq ? q0 + qi : q0) * kchunks * 32u;
+	const uint32_t qlen4 = kchunks * 32u;
+	float4* sq4 = reinterpret_cast<float4*>(s_seed);
+	float* s_d = s_seed + size_t(kTcSeedQ) * qlen4 * 4;
+	for (uint32_t i = threadIdx.x; i < kTcSeedQ * qlen4; i += blockDim.x) {  // padding queries of the last tile copy query q0
+		const uint32_t qi = i / qlen4, q = q0 + qi < nq ? q0 + qi : q0;
+		sq4[i] = reinterpret_cast<const float4*>(qf)[size_t(q) * qlen4 + (i - qi * qlen4)];
 	}
+	__syncthreads();
+	const float4* rows4 = reinterpret_cast<const float4*>(rows);
 	constexpr uint32_t kRows = 4;  // rows in flight per warp
-	for (uint32_t r0 = warp * kRows; r0 < kTcInitRows; r0 += 8 * kRows) {
-		float dist[kRows][kTcInitQ];
-		if (r0 < nrows) {
+	for (uint32_t r0 = warp * kRows; r0 < kTcSeedSlice; r0 += 8 * kRows) {
+		float dist[kRows][kTcSeedQ];
+		if (row0 + r0 < nrows) {
 			uint32_t rr[kRows];
-			const float4* qp[kRows][kTcInitQ];
+			const float4* qp[kRows][kTcSeedQ];
 #pragma unroll
 			for (uint32_t x = 0; x < kRows; ++x) {
-				rr[x] = min(r0 + x, nrows - 1);
+				rr[x] = min(row0 + r0 + x, nrows - 1);
 #pragma unroll
-				for (int qi = 0; qi < kTcInitQ; ++qi) {
-					qp[x][qi] = q4[qi];
+				for (int qi = 0; qi < kTcSeedQ; ++qi) {
+					qp[x][qi] = sq4 + qi * qlen4;
 				}
 			}
 			if (metric == kL2) {
-				row_dists_warp<true, kRows, kTcInitQ>(rows4, pitch / 4, kchunks, rr, qp, nullptr, lane, dist);
+				row_dists_warp<true, kRows, kTcSeedQ>(rows4, pitch / 4, kchunks, rr, qp, nullptr, lane, dist);
 			} else {
-				row_dists_warp<false, kRows, kTcInitQ>(rows4, pitch / 4, kchunks, rr, qp, norm_coefs, lane, dist);
+				row_dists_warp<false, kRows, kTcSeedQ>(rows4, pitch / 4, kchunks, rr, qp, norm_coefs, lane, dist);
 			}
 		}
 #pragma unroll
 		for (uint32_t x = 0; x < kRows; ++x) {
 #pragma unroll
-			for (int qi = 0; qi < kTcInitQ; ++qi) {
+			for (int qi = 0; qi < kTcSeedQ; ++qi) {
 				if (lane == uint32_t(qi)) {
 					const uint32_t r = r0 + x;
-					s_d[qi * kTcInitRows + r] = r < nrows ? dist[x][qi] : INFINITY;
+					s_d[qi * kTcSeedSlice + r] = row0 + r < nrows ? dist[x][qi] : INFINITY;
 				}
 			}
 		}
 	}
 	__syncthreads();
-	if (warp < kTcInitQ && q0 + warp < nq) {  // warp w: the k1 smallest of query q0 + w (rows < nrows sort first, the rest are +inf)
-		const uint32_t q = q0 + warp;
-		float* d = s_d + warp * kTcInitRows;
-		float last = INFINITY;
-		for (uint32_t round = 0; round < kTcMaxK1; ++round) {
+	for (uint32_t qi = warp; qi < kTcSeedQ; qi += 8) {  // the k1 smallest of the slice (rows < nrows sort first, the rest are +inf)
+		const uint32_t q = q0 + qi;
+		if (q >= nq) {
+			break;
+		}
+		float* d = s_d + qi * kTcSeedSlice;
+		float* out = part + (size_t(q) * kTcSeedSlices + slice) * kTcMaxK1;
+		for (uint32_t round = 0; round < k1; ++round) {
 			float best = INFINITY;
 			uint32_t at = lane;
-			if (round < k1) {
-				for (uint32_t j = lane; j < kTcInitRows; j += 32) {
-					const float y = d[j];
-					if (y < best) {
-						best = y;
-						at = j;
-					}
+			for (uint32_t j = lane; j < kTcSeedSlice; j += 32) {
+				const float y = d[j];
+				if (y < best) {
+					best = y;
+					at = j;
 				}
-				for (int off = 16; off > 0; off >>= 1) {
-					const float ob = __shfl_xor_sync(0xffffffffu, best, off);
-					const uint32_t oa = __shfl_xor_sync(0xffffffffu, at, off);
-					if (ob < best || (ob == best && oa < at)) {
-						best = ob;
-						at = oa;
-					}
+			}
+			for (int off = 16; off > 0; off >>= 1) {
+				const float ob = __shfl_xor_sync(0xffffffffu, best, off);
+				const uint32_t oa = __shfl_xor_sync(0xffffffffu, at, off);
+				if (ob < best || (ob == best && oa < at)) {
+					best = ob;
+					at = oa;
 				}
-				if (lane == 0) {
-					d[at] = INFINITY;
-				}
-				__syncwarp();
-				last = best;
 			}
 			if (lane == 0) {
-				ub_list[size_t(q) * kTcMaxK1 + round] = round < k1 ? best : -INFINITY;
+				d[at] = INFINITY;
+				out[round] = best;
 			}
+			__syncwarp();
+		}
+	}
+}
+__global__ void __launch_bounds__(256) tc_seed_merge(const float* part, uint32_t nq, uint32_t k1, unsigned int* tau, float* ub_list,
+													 unsigned int* ub_lock) {
+	static_assert(kTcSeedSlices <= 32, "one lane per slice");
+	const uint32_t lane = threadIdx.x & 31, q = (blockIdx.x * blockDim.x + threadIdx.x) / 32;
+	if (q >= nq) {
+		return;
+	}
+	const float* mine = part + (size_t(q) * kTcSeedSlices + lane) * kTcMaxK1;
+	uint32_t head = 0;
+	float last = INFINITY;
+	for (uint32_t round = 0; round < kTcMaxK1; ++round) {
+		float best = INFINITY;
+		if (round < k1) {
+			const float h = lane < kTcSeedSlices && head < k1 ? mine[head] : INFINITY;
+			best = h;
+			uint32_t at = lane;
+			for (int off = 16; off > 0; off >>= 1) {
+				const float ob = __shfl_xor_sync(0xffffffffu, best, off);
+				const uint32_t oa = __shfl_xor_sync(0xffffffffu, at, off);
+				if (ob < best || (ob == best && oa < at)) {
+					best = ob;
+					at = oa;
+				}
+			}
+			head += lane == at ? 1u : 0u;
+			last = best;
 		}
 		if (lane == 0) {
-			tau[q] = float_ord(last);  // +inf while fewer than k1 rows exist
-			ub_lock[q] = 0;
+			ub_list[size_t(q) * kTcMaxK1 + round] = round < k1 ? best : -INFINITY;
 		}
+	}
+	if (lane == 0) {
+		tau[q] = float_ord(last);  // +inf while fewer than k1 rows exist
+		ub_lock[q] = 0;
 	}
 }
 
 // queries fp32 [nq][dim] -> int8 codes [nq_pad][pitch] (zero padded) + (s_q, r_q, n_q, 1 / k_q), k_q = s_q (1 when s_q = 0), and the
-// fp32 queries zero padded to the same pitch, qf [nq_pad][pitch] (the exact distances of tc_init_tau and the filter's bookkeepers)
+// fp32 queries zero padded to the same pitch, qf [nq_pad][pitch] (the exact distances of the seed and the filter's bookkeepers)
 __global__ void tc_prepare_queries(const float* queries, uint32_t nq, uint32_t nq_pad, uint32_t dim, uint32_t pitch, unsigned char* codes,
 								   float4* qc, float* qf) {
 	const uint32_t q = (blockIdx.x * blockDim.x + threadIdx.x) / 32;
